@@ -126,7 +126,7 @@ int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* amax_g, i
                        int ntaps_out, const int* entries_host, int nentries, int nsplit, cudaStream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------
- * InstanceNorm2d / BatchNorm (train mode) + fused GLU / LeakyReLU / residual
+ * InstanceNorm2d / BatchNorm (train and eval mode) + fused GLU / LeakyReLU / residual
  * -- replaces ref: model.py:19-27 (GLU), 47, 70, 75, 497, 602, 992, 1011 (norm layers).
  * groups = N (instance norm) or 1 (batch norm); P pixels per group; contiguous rows of C channels.
  * amax_out / amax_dy (optional): receive max|out| / max|dy| as float bits, so that a convolution consuming the
@@ -151,6 +151,16 @@ int og_norm_backward(const float* y, const float* g, int groups, long long P, in
                      const float* rstd, const float* gamma, const float* beta, int act, float slope, double* bstats,
                      float* dy, float* dgamma, float* dbeta, int accumulate_param_grads, unsigned* amax_dy,
                      cudaStream_t stream);
+/* BatchNorm in eval mode (ref: nn.BatchNorm{1,2}d after .eval(), evaluator.py:110): the running statistics, only read,
+ * give mean = running_mean and rstd = 1 / sqrt(running_var + eps), which og_norm_apply (groups = 1) consumes.
+ * og_bn_eval_backward is the matching backward: activation backward, then dy = g' * gamma * rstd,
+ * dgamma = sum g' * (y - mean) * rstd, dbeta = sum g' (no batch-statistic terms; per-channel sums in a fixed order,
+ * so repeated calls give identical results).  dgamma / dbeta may both be null. */
+int og_bn_eval_coef(const float* running_mean, const float* running_var, int C, float eps, float* mean, float* rstd,
+                    cudaStream_t stream);
+int og_bn_eval_backward(const float* y, const float* g, long long P, int Cy, const float* mean, const float* rstd,
+                        const float* gamma, const float* beta, int act, float slope, float* dy, float* dgamma,
+                        float* dbeta, int accumulate_param_grads, unsigned* amax_dy, cudaStream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------
  * Attention -- replaces ref: GlobalAttention.py:32-70 (func_attention), 73-122 (GlobalAttentionGeneral),

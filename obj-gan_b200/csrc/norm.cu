@@ -1,4 +1,4 @@
-// InstanceNorm2d / BatchNorm{1,2}d (train mode) with fused activation, forward and backward, NHWC.
+// InstanceNorm2d / BatchNorm{1,2}d (train and eval mode) with fused activation, forward and backward, NHWC.
 //
 // Reference semantics (image_generation/model.py): nn.InstanceNorm2d defaults (no affine, eps 1e-5, biased
 // variance; model.py:70, 602, 1198) and nn.BatchNorm2d/1d in train mode (batch statistics, biased variance
@@ -491,6 +491,112 @@ __global__ void __launch_bounds__(256) norm_apply_split_kernel(
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// BatchNorm in eval mode (ref: nn.BatchNorm{1,2}d after .eval(), evaluator.py:110): the running statistics replace the
+// batch statistics, so the normalisation is a fixed per-channel affine map.  The forward pass is og_bn_eval_coef
+// (mean / rstd in the form og_norm_apply takes) followed by og_norm_apply with groups = 1.
+// ------------------------------------------------------------------------------------------------
+__global__ void bn_eval_coef_kernel(const float* __restrict__ running_mean, const float* __restrict__ running_var,
+                                    int C, float eps, float* __restrict__ mean, float* __restrict__ rstd) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= C) return;
+  mean[i] = running_mean[i];
+  rstd[i] = (float)(1.0 / sqrt((double)running_var[i] + (double)eps));
+}
+
+// Backward of the fixed affine + activation: dy = dn * gamma * rstd, with no batch-statistic terms.  Same thread mapping
+// as norm_bwd_apply_kernel (grid (ceil(Co4/32), chunks), block (32, 8)).  When part is non-null, the CTA's per-channel
+// sums (sum dn, sum dn * xhat) are reduced inside the CTA in a fixed order (fp64) and stored to plane blockIdx.y of
+// part ([chunks][2][Cy] doubles); bn_eval_param_grad_kernel adds the planes in a fixed order -- no atomics, so the
+// parameter gradients are the same on every run.
+template <int ACT>
+__global__ void __launch_bounds__(256) bn_eval_bwd_kernel(const float* __restrict__ y, const float* __restrict__ g,
+                                                          int Cy, long long P, int pix_per_block,
+                                                          const float* __restrict__ mean,
+                                                          const float* __restrict__ rstd,
+                                                          const float* __restrict__ gamma,
+                                                          const float* __restrict__ beta, float slope,
+                                                          float* __restrict__ dy, double* __restrict__ part,
+                                                          unsigned* __restrict__ amax) {
+  const int Co = (ACT == OG_NA_GLU) ? Cy / 2 : Cy;
+  const int Co4 = Co >> 2;
+  const int c4 = blockIdx.x * 32 + threadIdx.x;
+  const long long p0 = (long long)blockIdx.y * pix_per_block;
+  const long long p1 = min(P, p0 + pix_per_block);
+  constexpr int NV = (ACT == OG_NA_GLU) ? 16 : 8;
+  double acc[NV];
+#pragma unroll
+  for (int i = 0; i < NV; ++i) acc[i] = 0;
+  float mx = 0.f;
+  if (c4 < Co4) {
+    const int c = c4 * 4;
+    ChanConst k;
+    load_chan<ACT>(k, mean, rstd, gamma, beta, 0, Cy, Co, c);
+    const float4 s = make_float4(k.r.x * k.ga.x, k.r.y * k.ga.y, k.r.z * k.ga.z, k.r.w * k.ga.w);
+    const float4 s2 = make_float4(k.r2.x * k.ga2.x, k.r2.y * k.ga2.y, k.r2.z * k.ga2.z, k.r2.w * k.ga2.w);
+    const float* yb = y + c;
+    const float* gb = g + c;
+    float* db = dy + c;
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (long long p = p0 + threadIdx.y; p < p1; p += 8) {
+      const float4 v = ldg4(yb + p * Cy), go = ldg4(gb + p * Co);
+      const float4 v2 = (ACT == OG_NA_GLU) ? ldg4(yb + p * Cy + Co) : zero;
+      float4 xh, dn, xh2, dn2;
+      act_grad4<ACT>(k, v, v2, go, slope, xh, dn, xh2, dn2);
+      const float4 o = make_float4(dn.x * s.x, dn.y * s.y, dn.z * s.z, dn.w * s.w);
+      st4(db + p * Cy, o);
+      mx = amax4(mx, o);
+      if (ACT == OG_NA_GLU) {
+        const float4 o2 = make_float4(dn2.x * s2.x, dn2.y * s2.y, dn2.z * s2.z, dn2.w * s2.w);
+        st4(db + p * Cy + Co, o2);
+        mx = amax4(mx, o2);
+      }
+      acc[0] += dn.x; acc[1] += dn.y; acc[2] += dn.z; acc[3] += dn.w;
+      acc[4] += (double)dn.x * xh.x; acc[5] += (double)dn.y * xh.y;
+      acc[6] += (double)dn.z * xh.z; acc[7] += (double)dn.w * xh.w;
+      if (ACT == OG_NA_GLU) {
+        acc[NV - 8] += dn2.x; acc[NV - 7] += dn2.y; acc[NV - 6] += dn2.z; acc[NV - 5] += dn2.w;
+        acc[NV - 4] += (double)dn2.x * xh2.x; acc[NV - 3] += (double)dn2.y * xh2.y;
+        acc[NV - 2] += (double)dn2.z * xh2.z; acc[NV - 1] += (double)dn2.w * xh2.w;
+      }
+    }
+  }
+  if (amax) block_amax_256(mx, amax);
+  if (!part) return;
+  __shared__ double sh[8][32][NV];
+#pragma unroll
+  for (int i = 0; i < NV; ++i) sh[threadIdx.y][threadIdx.x][i] = acc[i];
+  __syncthreads();
+  const int t = threadIdx.y * 32 + threadIdx.x;
+  double* plane = part + (long long)blockIdx.y * 2 * Cy;
+  for (int item = t; item < 32 * NV; item += 256) {
+    const int cx = item / NV, kk = item % NV;
+    double a = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) a += sh[j][cx][kk];
+    const int cc4 = blockIdx.x * 32 + cx;
+    if (cc4 < Co4) {
+      const int half = kk >> 3;              // 0: "a" half, 1: gate half (GLU only)
+      const int ch = half * Co + cc4 * 4 + (kk & 3);
+      plane[((kk & 7) >> 2) * Cy + ch] = a;  // [0][ch] = sum dn, [1][ch] = sum dn * xhat
+    }
+  }
+}
+
+// dbeta = sum_s part[s][0][c], dgamma = sum_s part[s][1][c], planes added in the order s = 0, 1, ...
+__global__ void bn_eval_param_grad_kernel(const double* __restrict__ part, int S, int C, float* dgamma, float* dbeta,
+                                          int accumulate) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= C) return;
+  double sb = 0, sg = 0;
+  for (int s = 0; s < S; ++s) {
+    sb += part[(long long)s * 2 * C + i];
+    sg += part[(long long)s * 2 * C + C + i];
+  }
+  dgamma[i] = accumulate ? dgamma[i] + (float)sg : (float)sg;
+  dbeta[i] = accumulate ? dbeta[i] + (float)sb : (float)sb;
+}
+
 static int elem_blocks(long long total) {
   long long b = (total + 255) / 256;
   long long cap = (long long)og_num_sms() * 32;
@@ -567,6 +673,59 @@ OG_API int og_norm_backward(const float* y, const float* g, int groups, long lon
   }
 #undef OG_LAUNCH_BWD
   OG_RETURN_LAST_ERROR();
+}
+
+// eval-mode BatchNorm: mean = running_mean, rstd = 1 / sqrt(running_var + eps) (fp32 [C]); the buffers are only read
+OG_API int og_bn_eval_coef(const float* running_mean, const float* running_var, int C, float eps, float* mean,
+                           float* rstd, cudaStream_t stream) {
+  if (C <= 0) return (int)cudaErrorInvalidValue;
+  bn_eval_coef_kernel<<<og_cdiv(C, 256), 256, 0, stream>>>(running_mean, running_var, C, eps, mean, rstd);
+  OG_RETURN_LAST_ERROR();
+}
+
+// Backward of og_norm_apply (groups = 1) with og_bn_eval_coef's statistics.  g: gradient w.r.t. the fused output
+// ([P][Co]); dy: gradient w.r.t. y ([P][Cy]).  dgamma / dbeta optional (both or neither); accumulate_param_grads adds
+// into them instead of overwriting.
+OG_API int og_bn_eval_backward(const float* y, const float* g, long long P, int Cy, const float* mean,
+                               const float* rstd, const float* gamma, const float* beta, int act, float slope, float* dy,
+                               float* dgamma, float* dbeta, int accumulate_param_grads, unsigned* amax_dy,
+                               cudaStream_t stream) {
+  const int Co = act == OG_NA_GLU ? Cy / 2 : Cy;
+  if (Cy % 4 || Co % 4 || (dgamma == nullptr) != (dbeta == nullptr)) return (int)cudaErrorInvalidValue;
+  if (amax_dy) OG_CHECK(cudaMemsetAsync(amax_dy, 0, sizeof(unsigned), stream));
+  if (P == 0) {
+    if (dgamma && !accumulate_param_grads) {
+      OG_CHECK(cudaMemsetAsync(dgamma, 0, sizeof(float) * Cy, stream));
+      OG_CHECK(cudaMemsetAsync(dbeta, 0, sizeof(float) * Cy, stream));
+    }
+    return 0;
+  }
+  const int cg = og_cdiv(Co / 4, 32);
+  const int ppb = pix_chunk(P, cg, 1);
+  const dim3 grid(cg, og_cdiv(P, ppb), 1), block(32, 8);
+  double* part = nullptr;
+  if (dgamma) {
+    float* w = nullptr;
+    OG_CHECK(og_work_alloc(&w, (size_t)grid.y * 2 * Cy * 2, stream));     // doubles as pairs of floats
+    part = reinterpret_cast<double*>(w);
+  }
+  if (act == OG_NA_GLU)
+    bn_eval_bwd_kernel<OG_NA_GLU><<<grid, block, 0, stream>>>(y, g, Cy, P, ppb, mean, rstd, gamma, beta, slope, dy, part, amax_dy);
+  else if (act == OG_NA_LRELU)
+    bn_eval_bwd_kernel<OG_NA_LRELU><<<grid, block, 0, stream>>>(y, g, Cy, P, ppb, mean, rstd, gamma, beta, slope, dy, part, amax_dy);
+  else
+    bn_eval_bwd_kernel<OG_NA_NONE><<<grid, block, 0, stream>>>(y, g, Cy, P, ppb, mean, rstd, gamma, beta, slope, dy, part, amax_dy);
+  int rc = (int)cudaGetLastError();
+  if (part) {
+    if (!rc) {
+      bn_eval_param_grad_kernel<<<og_cdiv(Cy, 256), 256, 0, stream>>>(part, (int)grid.y, Cy, dgamma, dbeta,
+                                                                     accumulate_param_grads);
+      rc = (int)cudaGetLastError();
+    }
+    const cudaError_t e = cudaFreeAsync(part, stream);
+    if (!rc) rc = (int)e;
+  }
+  return rc;
 }
 
 // *out_word = float bits of an upper bound of max|og_norm_apply output| (see norm_apply_split_kernel): max|gamma| *

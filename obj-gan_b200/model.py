@@ -77,8 +77,9 @@ class LinearP(nn.Module):
 
 
 class BatchNormP(nn.Module):
-    """nn.BatchNorm{1,2}d parameters/buffers; always train-mode statistics (the reference trainer never
-    switches G or the Ds to eval(): trainer.py:331-472)."""
+    """nn.BatchNorm{1,2}d parameters/buffers.  Train mode (the trainer never switches G or the Ds to eval():
+    trainer.py:331-472) normalises with the batch statistics and updates the running buffers; eval mode (the
+    evaluator's netG.eval(), evaluator.py:110) normalises with the running statistics and leaves the buffers alone."""
 
     def __init__(self, c):
         super().__init__()
@@ -90,7 +91,8 @@ class BatchNormP(nn.Module):
 
     def forward(self, y, act):
         return ops.batch_norm_act(y, self.weight, self.bias,
-                                  (self.running_mean, self.running_var, self.num_batches_tracked), act)
+                                  (self.running_mean, self.running_var, self.num_batches_tracked), act,
+                                  training=self.training)
 
 
 class _Slots(nn.Module):

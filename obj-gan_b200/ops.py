@@ -682,7 +682,55 @@ def instance_norm_act(y, act, res=None, split_pad=None, keep_f32=True):
     return _NormAct.apply(y, None, None, res, None, True, act, split_pad, keep_f32)
 
 
-def batch_norm_act(y, gamma, beta, buffers, act):
+class _BatchNormEvalAct(torch.autograd.Function):
+    """Eval-mode BatchNorm (running statistics) + fused activation.  The running buffers are only read: eval() must
+    not move them, and the output of a sample must not depend on the other samples of its batch."""
+
+    @staticmethod
+    def forward(ctx, y, gamma, beta, running_mean, running_var, act):
+        _chk(y, gamma, beta, running_mean, running_var)
+        y = y.contiguous()
+        n, h, w, cy = y.shape
+        assert gamma.numel() == cy, "BatchNorm layers of this model never need channel padding"
+        P = n * h * w
+        mean = torch.empty(cy, device=y.device, dtype=torch.float32)
+        rstd = torch.empty(cy, device=y.device, dtype=torch.float32)
+        _call("og_bn_eval_coef", _p(running_mean), _p(running_var), cy, NORM_EPS, _p(mean), _p(rstd))
+        co = cy // 2 if act == NA_GLU else cy
+        out = torch.empty((n, h, w, co), device=y.device, dtype=torch.float32)
+        _call("og_norm_apply", _p(y), 1, P, cy, _p(mean), _p(rstd), _p(gamma), _p(beta), 0, act, LRELU_SLOPE,
+              _p(out), _p(_tag_amax(out)))
+        ctx.cfg = (P, cy, act)
+        ctx.sinks = (_grad_sink(gamma), _grad_sink(beta))
+        ctx.save_for_backward(y, mean, rstd, gamma, beta)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        y, mean, rstd, gamma, beta = ctx.saved_tensors
+        P, cy, act = ctx.cfg
+        g = g.contiguous()
+        dy = torch.empty_like(y)
+        dgamma = dbeta = None
+        want_pg = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
+        direct = want_pg and ctx.sinks[0] is not None and ctx.sinks[1] is not None
+        if direct:
+            dgamma, dbeta = ctx.sinks
+        elif want_pg:
+            dgamma = torch.empty_like(gamma)
+            dbeta = torch.empty_like(beta)
+        _call("og_bn_eval_backward", _p(y), _p(g), P, cy, _p(mean), _p(rstd), _p(gamma), _p(beta), act, LRELU_SLOPE,
+              _p(dy), _p(dgamma), _p(dbeta), 1 if direct else 0, _p(_tag_amax(dy)))
+        if direct:
+            dgamma = dbeta = None
+        return dy, dgamma, dbeta, None, None, None
+
+
+def batch_norm_act(y, gamma, beta, buffers, act, training=True):
+    """BatchNorm (+ fused activation).  ``training``: batch statistics, and the running buffers (running_mean,
+    running_var, num_batches_tracked) are updated; otherwise the running statistics normalise and nothing is updated."""
+    if not training:
+        return _BatchNormEvalAct.apply(y, gamma, beta, buffers[0], buffers[1], act)
     return _NormAct.apply(y, gamma, beta, None, buffers, False, act)
 
 

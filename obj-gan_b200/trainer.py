@@ -27,6 +27,29 @@ BRANCH_ADAM = os.environ.get("OBJGAN_BRANCH_ADAM", "1") == "1"   # exchange + op
 PACK_PLAN = os.environ.get("OBJGAN_PACK_PLAN", "1") == "1"       # re-pack a network's operand copies right after Adam
 
 
+def prepare_data(dev: dict, num_classes: int | None = None, into: dict | None = None) -> dict:
+    """Device-side tail of the reference's host data path (ref: trainDataset.py:79-128 ``prepare_data``,
+    miscc/load.py:160-176, miscc/utils.py:502-522 ``form_clabels_feat``): from the per-roi masks, the roi class ids
+    and the class-label embeddings already on the device, build the 80-channel class heat maps of the three
+    scales and the (B, 50, Rmax, 1) label-embedding tensor -- 86 % of the bytes the reference copies host->device
+    every step are these derived tensors.  ``num_classes``: heat-map channels (None: one per row of
+    ``clabels_emb``).  ``into``: dict holding preallocated ``hmaps`` / ``slabels_feat`` buffers (the static inputs of
+    a captured graph) to fill instead of allocating."""
+    from . import synth
+    dst = into if into is not None else dev
+    ncls = num_classes if num_classes is not None else dev["clabels_emb"].shape[0]
+    cls, nr = dev["roi_cls"], dev["num_rois"]
+    clamp = float(dev.get("hmap_clamp", synth.HMAP_CLAMP))
+    have = into is not None and "hmaps" in into
+    hm = [ops.form_hmaps(m, cls, nr, ncls, clamp, out=(into["hmaps"][i] if have else None))
+          for i, m in enumerate(dev["bt_masks"])]
+    rmax = int(dev["glb_max_num_roi"])
+    sl = ops.form_clabels_feat(dev["clabels_emb"], cls, nr, rmax,
+                               out=(into["slabels_feat"] if into is not None and "slabels_feat" in into else None))
+    dst["hmaps"], dst["slabels_feat"] = hm, sl
+    return dst
+
+
 class FlatBucket:
     """Parameters of one network as views of a single flat buffer (+ matching grad / Adam state)."""
 
@@ -159,25 +182,8 @@ class StepATrainer:
         return out
 
     def prepare_data(self, dev: dict, into: dict | None = None) -> dict:
-        """Device-side tail of the reference's host data path (ref: trainDataset.py:79-128 ``prepare_data``,
-        miscc/load.py:160-176, miscc/utils.py:502-522 ``form_clabels_feat``): from the per-roi masks, the roi class ids
-        and the class-label embeddings already on the device, build the 80-channel class heat maps of the three
-        scales and the (B, 50, Rmax, 1) label-embedding tensor -- 86 % of the bytes the reference copies host->device
-        every step are these derived tensors.  ``into``: dict holding preallocated ``hmaps`` / ``slabels_feat`` buffers
-        (the static inputs of a captured graph) to fill instead of allocating."""
-        from . import synth
-        dst = into if into is not None else dev
-        ncls = self.netG.num_classes if hasattr(self.netG, "num_classes") else dev["clabels_emb"].shape[0]
-        cls, nr = dev["roi_cls"], dev["num_rois"]
-        clamp = float(dev.get("hmap_clamp", synth.HMAP_CLAMP))
-        have = into is not None and "hmaps" in into
-        hm = [ops.form_hmaps(m, cls, nr, ncls, clamp, out=(into["hmaps"][i] if have else None))
-              for i, m in enumerate(dev["bt_masks"])]
-        rmax = int(dev["glb_max_num_roi"])
-        sl = ops.form_clabels_feat(dev["clabels_emb"], cls, nr, rmax,
-                                   out=(into["slabels_feat"] if into is not None and "slabels_feat" in into else None))
-        dst["hmaps"], dst["slabels_feat"] = hm, sl
-        return dst
+        """Builds the derived inputs of a compact batch on the device (module-level ``prepare_data``)."""
+        return prepare_data(dev, getattr(self.netG, "num_classes", None), into)
 
     def generate(self, inp):
         g = self.netG
