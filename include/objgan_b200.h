@@ -293,6 +293,33 @@ int og_pack_weights_f16_multi(const long long* jobs, int njobs, int total_blocks
 int og_permute_channels(const float* x, const long long* perm, int B, int C, long long P, float* out,
                         cudaStream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * Shape generator (SHP_G_NET, ref: model.py:798-985) and heat maps from generated masks (miscc/utils.py:524-584)
+ *  og_form_bbox_maps : the loader's one-hot box maps (ref: miscc/load.py:178-189, 625-641) from the compact batch.
+ *                      rois / fm_rois: float64 [B][boxes][*stride] rows (x, y, w, h, ...), cls / num_rois int64.
+ *                      maps NHWC [2][B][R][S][S][Cp]: forward sequence (slot t), then backward (slot boxes-1-t: the
+ *                      reversal covers all box slots before the [:R] slice); fmaps [B][R][F][F] from fm_rois / 2.
+ *                      Box edges: min(round-half-even(v), size - 1), upper bound exclusive; slots >= num_rois are 0.
+ *  og_clstm_cell     : one ConvLSTM step (ref: model.py:818-863) of BOTH directions.  gx_*: x-part of Gates incl. bias
+ *                      for every step, NHWC [B*R][HW][4*Ch] (image b*R + t); gh_*: conv(h_{t-1}, W_h) [B][HW][4*Ch],
+ *                      both null at t = 0 (zero state: c_prev = 0).  c_* [B][HW][Ch] updated in place; h_* [B][HW][Ch]
+ *                      written; h also written to joint [B*R][HW][Cj]: forward at (b*R + t, channels [0, Ch)),
+ *                      backward at (b*R + R-1-t, channels [Ch, 2Ch)).
+ *  og_mul_pixels     : out[p][c] = x[p][c] * s[p] (the crop by the box feature maps, ref: model.py:969-972)
+ *  og_gen_hmaps      : form_hmaps' normalisation and class composite.  slots NHWC [B][P][Cs] (lane t = roi slot t,
+ *                      Cs <= 16): slots t < num_rois[b] normalised in place, the others left raw; hmap NHWC
+ *                      [B][P][Cp] written (class channels, every present one renormalised).  cls [B][boxes].
+ *                      Fixed-order reductions, no atomics. */
+int og_form_bbox_maps(const double* rois, int rois_stride, const double* fm_rois, int fm_stride, const long long* cls,
+                      const long long* num_rois, int B, int boxes, int R, int ncls, int Cp, int S, int F, float* maps,
+                      float* fmaps, cudaStream_t stream);
+int og_clstm_cell(const float* gx_f, const float* gx_b, const float* gh_f, const float* gh_b, float* c_f, float* c_b,
+                  float* h_f, float* h_b, float* joint, int B, int R, int t, int HW, int Ch, int Cj,
+                  cudaStream_t stream);
+int og_mul_pixels(const float* x, const float* s, long long P, int C, float* out, cudaStream_t stream);
+int og_gen_hmaps(float* slots, int B, long long P, int Cs, const long long* cls, int boxes, const long long* num_rois,
+                 int ncls, int Cp, float* hmap, cudaStream_t stream);
+
 /* zero-fill (a memset node when captured in a CUDA graph; no kernel launch) */
 int og_zero_bytes(float* p, long long bytes, cudaStream_t stream);
 

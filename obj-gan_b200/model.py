@@ -157,6 +157,18 @@ def upBlock(in_planes, out_planes):
     return UpBlock(in_planes, out_planes)
 
 
+class UpBlockIN(_Slots):
+    """upBlock(norm=nn.InstanceNorm2d) (ref: model.py:43-49, 910-911): key ``1.weight`` only (the instance norm has no
+    parameters)."""
+
+    def __init__(self, cin, cout):
+        super().__init__(_1=Conv2dP(cin, cout * 2, 3, 1, 1, mode=UPSAMPLE2X, split=cout))
+        assert cout % 8 == 0
+
+    def forward(self, x):  # NHWC
+        return ops.instance_norm_act(self[1](x), NA_GLU)
+
+
 class HmapResBlock(nn.Module):
     """ref: model.py:63-81.  keys ``block.1.weight`` (2C, C, 3, 3) and ``block.5.weight`` (C, C, 3, 3)."""
 
@@ -473,6 +485,142 @@ class G_NET(_Base):
             att_maps.append(att)
             bt_att_maps.append(ops.to_nchw(bt_att, L))
         return fake_imgs, bt_c_codes, att_maps, bt_att_maps, mu, logvar
+
+
+# --------------------------------------------------------------------------------------------------
+# shape generator (ref: model.py:798-985): one soft mask per roi slot from the layout's box maps.  Inference only.
+# --------------------------------------------------------------------------------------------------
+class _DownBlock3x3(_Slots):
+    """downBlock_3x3 (ref: model.py:800-806): conv3x3 stride 2, no bias -> InstanceNorm2d -> LeakyReLU(0.2)."""
+
+    def __init__(self, cin, cout):
+        super().__init__(_0=Conv2dP(cin, cout, 3, 2, 1))
+
+    def forward(self, x):  # NHWC
+        return ops.instance_norm_act(self[0](x), NA_LRELU)
+
+
+class CLSTMCell(_Base):
+    """ref: model.py:818-863.  key ``Gates.{weight,bias}``: conv over cat(x_t, h_{t-1}).  Run by SHP_G_NET as two
+    convolutions split by input channels: the x-part (with the bias) once for all steps, the h-part inside the loop
+    (skipped at t = 0, where h = 0).  The split copies are derived from ``Gates.weight`` and refreshed whenever it
+    changes (load_state_dict, in-place edits)."""
+
+    def __init__(self, input_size, hidden_size, kernel_size, padding):
+        super().__init__()
+        self.input_size, self.hidden_size = input_size, hidden_size
+        self.Gates = Conv2dP(input_size + hidden_size, 4 * hidden_size, kernel_size, 1, padding, bias=True)
+        self._split_key = None
+        self._wx = self._wh = None
+        self._caches = (ops.PackedWeights(), ops.PackedWeights())
+
+    def split_weights(self):
+        w = self.Gates.weight
+        key = (w.data_ptr(), w._version, ops._epoch_of(w))
+        if key != self._split_key:
+            ci = self.input_size
+            if self._wx is None or self._wx.device != w.device:
+                self._wx = torch.empty_like(w[:, :ci]).contiguous()
+                self._wh = torch.empty_like(w[:, ci:]).contiguous()
+            self._wx.copy_(w.detach()[:, :ci])          # bumps _version: the packed operand copies are rebuilt
+            self._wh.copy_(w.detach()[:, ci:])
+            self._split_key = key
+        return self._wx, self._wh
+
+    def gates_x(self, x):
+        """x-part of Gates plus its bias: NHWC (N, H, W, input_size) -> (N, H, W, 4 * hidden_size)."""
+        return ops.conv2d(x, self.split_weights()[0], self.Gates.bias, self._caches[0], stride=1, pad=self.Gates.pad)
+
+    def gates_h(self, h):
+        """h-part of Gates (no bias): NHWC (N, H, W, hidden_size) -> (N, H, W, 4 * hidden_size)."""
+        return ops.conv2d(h, self.split_weights()[1], None, self._caches[1], stride=1, pad=self.Gates.pad)
+
+
+class ShapeResBlock(nn.Module):
+    """ResBlock(channel_num, norm=nn.InstanceNorm2d) (ref: model.py:866-882): keys ``block.{0,3,6}.weight``; zero
+    padding, and no norm after the last convolution."""
+
+    def __init__(self, channel_num):
+        super().__init__()
+        c = channel_num
+        self.block = _Slots(_0=Conv2dP(c, 2 * c, 3, 1, 1, split=c), _3=Conv2dP(c, 2 * c, 3, 1, 1, split=c),
+                            _6=Conv2dP(c, c, 3, 1, 1))
+
+    def forward(self, x):  # NHWC
+        y = ops.instance_norm_act(self.block[0](x), NA_GLU)
+        y = ops.instance_norm_act(self.block[3](y), NA_GLU)
+        return ops.add(self.block[6](y), x)
+
+
+class GET_SHAPE_G(nn.Module):
+    """ref: model.py:885-895.  key ``img.0.weight``: conv1x1 nbf -> 1, no bias, sigmoid."""
+
+    def __init__(self, nbf):
+        super().__init__()
+        self.img = _Slots(_0=Conv2dP(nbf, 1, 1, 1, 0, act=ACT_SIGMOID))
+
+    def forward_nhwc(self, h):
+        return self.img[0](h)
+
+
+class SHP_G_NET(_Base):
+    """ref: model.py:898-985 -- same constructor, forward signature and state_dict.  Inference only: a forward with grad
+    mode on and parameters that require grad raises."""
+
+    def __init__(self, num_classes):
+        super().__init__()
+        nbf = num_classes
+        self.nbf = nbf
+        self.fm_size = cfg.ROI.FM_SIZE
+        self.downsample1 = _DownBlock3x3(nbf, nbf * 2)
+        self.downsample2 = _DownBlock3x3(nbf * 2, nbf * 4)
+        self.fwd_convlstm = CLSTMCell(nbf * 4, nbf * 2, 3, 1)
+        self.bwd_convlstm = CLSTMCell(nbf * 4, nbf * 2, 3, 1)
+        self.jointConv = _Slots(_0=Conv2dP(nbf * 8, nbf * 8, 3, 1, 1, split=nbf * 4))
+        self.residual = nn.Sequential(*[ShapeResBlock(nbf * 4) for _ in range(cfg.GAN.R_NUM)])
+        self.upsample1 = UpBlockIN(nbf * 4, nbf * 2)
+        self.upsample2 = UpBlockIN(nbf * 2, nbf)
+        self.img_net = GET_SHAPE_G(nbf)
+
+    def _check_inference(self, *inputs):
+        ops.inference_only("SHP_G_NET", *inputs, *self.parameters())
+
+    def forward_nhwc(self, z_code, maps, bbox_fmaps):
+        """z_code (B, R, 4*nbf); maps NHWC (2*B*R, S, S, cpad(nbf)): the forward sequence (image b*R + t), then the
+        backward one (what ops.form_bbox_maps builds); bbox_fmaps (B, R, F, F).  Returns the masks as NHWC
+        (B*R, S, S, 8), channel 0 (the conv head's padded output)."""
+        self._check_inference(z_code, maps, bbox_fmaps)
+        b, r = z_code.shape[0], z_code.shape[1]
+        n = b * r
+        if n == 0:
+            return torch.zeros((0, maps.shape[1], maps.shape[2], 8), device=maps.device, dtype=torch.float32)
+        h = self.downsample2(self.downsample1(maps))               # both sequences in one pass: (2BR, F, F, 4*nbf)
+        gx = (self.fwd_convlstm.gates_x(h[:n]), self.bwd_convlstm.gates_x(h[n:]))
+        fm, ch, cz = h.shape[1], self.nbf * 2, self.nbf * 4
+        joint = torch.empty((n, fm, fm, 2 * ch + cz), device=h.device, dtype=torch.float32)
+        ops.fill_channels(joint, z_code.reshape(n, cz), 2 * ch)  # z broadcast over the map (model.py:931-935, 962)
+        c = (torch.empty((b, fm, fm, ch), device=h.device, dtype=torch.float32),
+             torch.empty((b, fm, fm, ch), device=h.device, dtype=torch.float32))
+        hs = None
+        for t in range(r):
+            gh = None if t == 0 else (self.fwd_convlstm.gates_h(hs[0]), self.bwd_convlstm.gates_h(hs[1]))
+            hs = ops.clstm_cell(gx, gh, c, joint, t)
+        y = ops.instance_norm_act(self.jointConv[0](joint), NA_GLU)
+        y = ops.mul_pixels(y, bbox_fmaps)                            # crop (model.py:969-972)
+        y = self.residual(y)
+        y = self.upsample2(self.upsample1(y))
+        return self.img_net.forward_nhwc(y)
+
+    def forward(self, z_code, bbox_maps_fwd, bbox_maps_bwd, bbox_fmaps):
+        """NCHW like the reference: z_code (B, R, 4*nbf), bbox_maps_* (B, R, nbf, S, S), bbox_fmaps (B, R, F, F) ->
+        (B, R, 1, S, S)."""
+        self._check_inference(z_code, bbox_maps_fwd, bbox_maps_bwd, bbox_fmaps)
+        b, r = z_code.shape[0], z_code.shape[1]
+        s = bbox_maps_fwd.shape[-1]
+        maps = ops.nchw_rows([bbox_maps_fwd.reshape(b * r, self.nbf, s, s), bbox_maps_bwd.reshape(b * r, self.nbf, s, s)],
+                             cpad(self.nbf))
+        out = self.forward_nhwc(z_code.contiguous(), maps, bbox_fmaps.contiguous())
+        return ops.to_nchw(out, 1).view(b, r, 1, s, s)
 
 
 # --------------------------------------------------------------------------------------------------

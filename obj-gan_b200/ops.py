@@ -1356,6 +1356,138 @@ def form_clabels_feat(clabels_emb, roi_cls, num_rois, rmax, out=None):
     return out
 
 
+# --------------------------------------------------------------------------------------------------
+# Shape generator stage (SHP_G_NET and the heat maps of its masks).  Inference only: none of these has a backward.
+# --------------------------------------------------------------------------------------------------
+def inference_only(what, *ts):
+    """Raises when autograd would have to record ``what`` (a tensor it reads requires grad and grad mode is on)."""
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts):
+        raise RuntimeError(f"{what} is inference only (it has no backward): run it under torch.no_grad()")
+
+
+def _i64(t):
+    assert t.dtype == torch.int64
+    return t.contiguous()
+
+
+def form_bbox_maps(rois0, fm_rois, roi_cls, num_rois, rmax, num_classes, size=64, fsize=16):
+    """The loader's box maps (ref: miscc/load.py:178-189, 625-641) on the device, from the box tables of the batch:
+    ``rois0`` / ``fm_rois`` (B, BOXES, >=4) float64 (x, y, w, h at 64 / 32 pixels), ``roi_cls`` (B, BOXES) int64.
+    Returns the forward and backward sequences as ONE NHWC tensor (2*B*rmax, size, size, cpad(num_classes)) --
+    image b*rmax + t of the forward half, then the backward half, whose slot t is box slot BOXES-1-t -- and
+    bbox_fmaps (B, rmax, fsize, fsize)."""
+    _chk(rois0, fm_rois, roi_cls, num_rois)
+    r0 = rois0.to(torch.float64).contiguous()
+    fm = fm_rois.to(torch.float64).contiguous()
+    b, boxes = roi_cls.shape
+    assert r0.shape[:2] == (b, boxes) and fm.shape[:2] == (b, boxes) and rmax <= boxes
+    cp = cpad(num_classes)
+    dev = r0.device
+    maps = torch.empty((2 * b * rmax, size, size, cp), device=dev, dtype=torch.float32)
+    fmaps = torch.empty((b, rmax, fsize, fsize), device=dev, dtype=torch.float32)
+    _call("og_form_bbox_maps", _p(r0), r0.shape[2], _p(fm), fm.shape[2], _p(_i64(roi_cls)), _p(_i64(num_rois)), b, boxes,
+          rmax, num_classes, cp, size, fsize, _p(maps), _p(fmaps))
+    return maps, fmaps
+
+
+def nchw_rows(xs, cp):
+    """NCHW tensors (N_i, C, H, W) -> one NHWC tensor (sum N_i, H, W, cp), stacked along the batch."""
+    _chk(*xs)
+    n = sum(x.shape[0] for x in xs)
+    _, c, h, w = xs[0].shape
+    out = torch.empty((n, h, w, cp), device=xs[0].device, dtype=torch.float32)
+    off = 0
+    for x in xs:
+        x = x.detach().contiguous()
+        _call("og_nchw_to_nhwc", _p(x), x.shape[0], c, h, w, cp, _p(out[off:]))
+        off += x.shape[0]
+    return out
+
+
+def fill_channels(dst, rows, doff):
+    """dst[i, :, :, doff:doff+C] = rows[i] for an NHWC tensor dst (N, H, W, Cd) and rows (N, C)."""
+    _chk(dst, rows)
+    n, h, w, cd = dst.shape
+    rows = rows.detach().contiguous().view(n, -1)
+    _call("og_broadcast_channels", _p(rows), n, rows.shape[1], _p(dst), cd, doff, h * w)
+    return dst
+
+
+def clstm_cell(gx, gh, c, joint, t):
+    """One step of both ConvLSTM directions (ref: model.py:818-863).  gx = (fwd, bwd) x-parts of Gates with bias for all
+    steps, NHWC (B*R, H, W, 4*Ch); gh = None at t = 0 (zero state) or the (fwd, bwd) h-parts (B, H, W, 4*Ch); c = (fwd,
+    bwd) cell states (B, H, W, Ch), updated in place.  h goes to joint (B*R, H, W, Cj) channels [0, Ch) of slot t
+    (forward) and [Ch, 2*Ch) of slot R-1-t (backward); returns (h_fwd, h_bwd)."""
+    inference_only("the ConvLSTM cell", *gx, *(gh or ()), *c)
+    _chk(*gx, *(gh or ()), *c, joint)
+    b, hh, ww, ch = c[0].shape
+    r = gx[0].shape[0] // b
+    assert gx[0].shape == (b * r, hh, ww, 4 * ch) and joint.shape[:3] == (b * r, hh, ww)
+    hf, hb = torch.empty_like(c[0]), torch.empty_like(c[1])
+    _call("og_clstm_cell", _p(gx[0]), _p(gx[1]), _p(gh[0]) if gh else 0, _p(gh[1]) if gh else 0, _p(c[0]), _p(c[1]),
+          _p(hf), _p(hb), _p(joint), b, r, t, hh * ww, ch, joint.shape[3])
+    return hf, hb
+
+
+def mul_pixels(x, s):
+    """x * s broadcast over channels: x NHWC (N, H, W, C), s with N*H*W elements (one factor per pixel)."""
+    inference_only("mul_pixels", x, s)
+    _chk(x, s)
+    x = x.contiguous()
+    n, h, w, c = x.shape
+    assert s.numel() == n * h * w
+    out = torch.empty_like(x)
+    _call("og_mul_pixels", _p(x), _p(s.contiguous()), n * h * w, c, _p(out))
+    return out
+
+
+def _resize_nhwc(x, size):
+    """F.interpolate(bilinear, align_corners=True) to size x size; the identity when the size does not change."""
+    n, h, w, c = x.shape
+    if (h, w) == (size, size):
+        return x
+    y = torch.empty((n, size, size, c), device=x.device, dtype=torch.float32)
+    _call("og_bilinear_fwd", _p(x), n, h, w, c, size, size, _p(y))
+    return y
+
+
+def _nchw_of(x, c):
+    n, h, w, cp = x.shape
+    out = torch.empty((n, c, h, w), device=x.device, dtype=torch.float32)
+    _call("og_nhwc_to_nchw", _p(x), n, c, h, w, cp, _p(out))
+    return out
+
+
+def form_gen_hmaps(raw_masks, roi_cls, num_rois, sizes=(64, 128, 256), num_classes=80):
+    """form_hmaps (ref: miscc/utils.py:524-584) on the device: the generated masks (B, R, 64, 64) (or (B, R, 1, 64, 64))
+    -> (hmaps[len(sizes)], bt_masks[len(sizes)], fm_bt_masks).  hmaps are (B, num_classes, s, s); the per-roi tensors are
+    (B, BOXES, s, s) with the slots past R zero, the shapes a batch with ground-truth masks has.  Slots
+    num_rois[b] <= t < R are not normalised: they keep the raw sigmoid values, as in the reference."""
+    _chk(raw_masks, roi_cls, num_rois)
+    inference_only("form_gen_hmaps", raw_masks)
+    raw = raw_masks.detach()
+    if raw.dim() == 5:
+        raw = raw[:, :, 0]
+    raw = raw.contiguous()
+    b, r, h, w = raw.shape
+    boxes = roi_cls.shape[1]
+    assert roi_cls.shape[0] == b and r <= boxes
+    cs = (boxes + 3) // 4 * 4               # one lane per box slot; lanes >= R are zero
+    top = max(sizes)
+    dev = raw.device
+    x = torch.empty((b, h, w, cs), device=dev, dtype=torch.float32)
+    _call("og_nchw_to_nhwc", _p(raw), b, r, h, w, cs, _p(x))
+    slots = _resize_nhwc(x, top)            # normalised in place below
+    cp = cpad(num_classes)
+    hm = torch.empty((b, top, top, cp), device=dev, dtype=torch.float32)
+    _call("og_gen_hmaps", _p(slots), b, top * top, cs, _p(_i64(roi_cls)), boxes, _p(_i64(num_rois)), num_classes, cp,
+          _p(hm))
+    hmaps = [_nchw_of(_resize_nhwc(hm, s), num_classes) for s in sizes]
+    bt_masks = [_nchw_of(_resize_nhwc(slots, s), boxes) for s in sizes]
+    fm_bt_masks = _nchw_of(_resize_nhwc(slots, sizes[0] // 2), boxes)
+    return hmaps, bt_masks, fm_bt_masks
+
+
 class _WordsPairs(torch.autograd.Function):
     """All B x NC (image, caption) pairs of words_loss in one launch (ref: miscc/losses.py:87-127): func_attention,
     word / attended-context cosine and the Eq. (10) pooling.  ctx_feat (B, ndf, ih, iw) carries the gradient;

@@ -1,12 +1,17 @@
 """Sampling from a trained generator: the reference's evaluator path (ref: evaluator.py:108-138 builds G_NET, calls
 ``netG.eval()`` and loads ``netG_epoch_N.pth``; evaluator.py:312 draws the noise) on the sm_90a kernels.
 
+With a shape generator (``SHP_G_NET``, ref: evaluator.py:111-144), a batch that brings boxes but no masks is sampled the
+way the reference's default evaluator mode does it (cfg.TEST.USE_GT_BOX_SEG = 1 / 2, evaluator.py:314-332): box maps ->
+SHP_G_NET -> form_hmaps -> label embeddings -> G_NET, all on the device and inside the same per-shape CUDA graph.
+
 ``GSampler`` holds its own G_NET in eval mode, so BatchNorm normalises with the running statistics and never updates
 them.  A forward pass is ~200 library calls, which cost far more host time than the kernels take at small batch, so
 every input shape is captured once into a CUDA graph and replayed after that:
 
-  * graphs are keyed by (B, L, Rmax, glb_max_num_roi): batch, caption length, roi slots of ``slabels_feat`` and the
-    roi width of the returned ``bt_c_code``.  Rmax is NOT padded to BOXES_NUM to share one graph: the bottom-up paint
+  * graphs are keyed by (B, L, Rmax, glb_max_num_roi, generated shapes): batch, caption length, roi slots of
+    ``slabels_feat`` (glb_max_num_roi when the shapes are generated), the roi width of the returned ``bt_c_code``, and
+    whether the masks come from the batch or from the shape generator.  Rmax is NOT padded to BOXES_NUM to share one graph: the bottom-up paint
     takes a max over the roi axis, and an extra zero slot contributes 0 to that max, which changes the result wherever
     every real roi's product is negative;
   * the first call with a key runs eagerly (the warm-up: packed weight copies, allocator), then captures; later calls
@@ -20,13 +25,17 @@ from __future__ import annotations
 import torch
 
 from . import lib as _lib
-from . import model
+from . import model, ops
 from .config import cfg
+from .synth import IMG_SIZES
 from .trainer import prepare_data
 
 # what G_NET.forward reads, in its argument order (ref: model.py:747)
 G_ARGS = ("z", "sent_emb", "words_embs", "glove_words_embs", "slabels_feat", "mask", "hmaps", "rois", "fm_rois",
           "num_rois", "bt_masks", "fm_bt_masks", "glb_max_num_roi")
+# what the generated-shape path reads: the layout (boxes and classes), the shape noise, and the label embeddings
+GEN_ARGS = ("z", "eps", "noise_shp", "sent_emb", "words_embs", "glove_words_embs", "mask", "rois", "fm_rois", "num_rois",
+            "roi_cls", "clabels_emb", "glb_max_num_roi")
 
 
 def _map(x, f):
@@ -57,19 +66,26 @@ class _Graph:
 class GSampler:
     """Eval-mode G_NET forward with the reference's inputs and 6-tuple output, CUDA-graph replayed per input shape."""
 
-    def __init__(self, netG: model.G_NET):
+    def __init__(self, netG: model.G_NET, netShpG: model.SHP_G_NET | None = None):
         self.netG = netG.eval()
-        for p in self.netG.parameters():
-            p.requires_grad_(False)
+        self.netShpG = netShpG.eval() if netShpG is not None else None
+        for net in (self.netG, self.netShpG):
+            for p in (net.parameters() if net is not None else ()):
+                p.requires_grad_(False)
         self.device = next(self.netG.parameters()).device
         self._graphs = {}
         self._pool = None
 
     @classmethod
-    def from_snapshot(cls, path: str, num_classes: int = 80, device="cuda") -> "GSampler":
-        """A reference-format generator snapshot (``netG_epoch_N.pth``, what StepBTrainer.save_model writes)."""
-        s = cls(_new_g(num_classes, device))
+    def from_snapshot(cls, path: str, num_classes: int = 80, device="cuda", shape_snapshot: str | None = None) -> "GSampler":
+        """A reference-format generator snapshot (``netG_epoch_N.pth``, what StepBTrainer.save_model writes), and
+        optionally a shape generator snapshot (the reference's ``cfg.TEST.NET_SHP_G``; keys with or without the
+        ``module.`` prefix that nn.DataParallel adds)."""
+        shp = _new_shp_g(num_classes, device) if shape_snapshot is not None else None
+        s = cls(_new_g(num_classes, device), shp)
         s.load_state_dict(torch.load(path, map_location="cpu"))
+        if shape_snapshot is not None:
+            s.load_shape_state_dict(torch.load(shape_snapshot, map_location="cpu"))
         return s
 
     @classmethod
@@ -84,6 +100,14 @@ class GSampler:
         self._graphs.clear()
         self.netG.load_state_dict({k: v.to(self.device) for k, v in state_dict.items()}, strict=True)
 
+    def load_shape_state_dict(self, state_dict: dict) -> None:
+        """Loads SHP_G_NET weights (strict; a ``module.`` prefix on every key is dropped) and drops every captured
+        graph."""
+        if self.netShpG is None:
+            raise ValueError("this sampler has no shape generator: build it with GSampler(netG, netShpG)")
+        self._graphs.clear()
+        self.netShpG.load_state_dict(strip_module_prefix(state_dict), strict=True)
+
     # ------------------------------------------------------------------ inputs
     def _prepare(self, inp: dict) -> dict:
         """Device copies of the inputs G_NET reads (+ the derived tensors of a compact batch), with z and the CA_NET
@@ -91,21 +115,56 @@ class GSampler:
         dev = {}
         for k, v in inp.items():
             dev[k] = _map(v, lambda t: t.to(self.device, non_blocking=True))
-        if "hmaps" not in dev and "roi_cls" in dev:
+        gen = self._generates(dev)
+        if gen and dev.get("roi_cls") is None:
+            dev["roi_cls"] = dev["rois"][0][..., 4].to(torch.int64)
+        if not gen and "hmaps" not in dev and "roi_cls" in dev:
             prepare_data(dev, self.netG.num_classes)
         b = dev["sent_emb"].shape[0]
         if dev.get("z") is None:
             dev["z"] = torch.randn(b, cfg.GAN.Z_DIM, device=self.device)      # noise_img.data.normal_(0, 1)
         if dev.get("eps") is None:
             dev["eps"] = torch.randn(b, cfg.GAN.CONDITION_DIM, device=self.device)   # CA_NET.reparametrize
-        return {k: dev[k] for k in (*G_ARGS, "eps")}
+        if gen and dev.get("noise_shp") is None:                              # noise_shp.data.normal_(0, 1)
+            dev["noise_shp"] = torch.randn(b, cfg.ROI.BOXES_NUM, 4 * self.netShpG.nbf, device=self.device)
+        return {k: dev[k] for k in (GEN_ARGS if gen else (*G_ARGS, "eps"))}
+
+    def _generates(self, dev: dict) -> bool:
+        """Whether the batch's masks come from the shape generator (the batch brings no ``bt_masks``)."""
+        if dev.get("bt_masks") is not None:
+            return False
+        if self.netShpG is None:
+            raise ValueError("the batch has no masks (bt_masks) and this sampler has no shape generator: build it with "
+                             "GSampler(netG, netShpG) or GSampler.from_snapshot(..., shape_snapshot=...)")
+        return True
 
     @staticmethod
     def _key(dev: dict) -> tuple:
-        return (dev["z"].shape[0], dev["words_embs"].shape[2], dev["slabels_feat"].shape[2],
-                int(dev["glb_max_num_roi"]))
+        gen = "noise_shp" in dev
+        rmax = int(dev["glb_max_num_roi"]) if gen else dev["slabels_feat"].shape[2]
+        return (dev["z"].shape[0], dev["words_embs"].shape[2], rmax, int(dev["glb_max_num_roi"]), gen)
+
+    def _shapes(self, dev: dict) -> dict:
+        """Box maps -> SHP_G_NET -> form_hmaps (ref: evaluator.py:315-328): the raw masks (B, R, 64, 64) and the heat
+        maps / per-roi masks G_NET reads, R = glb_max_num_roi."""
+        nbf = self.netShpG.nbf
+        rmax = int(dev["glb_max_num_roi"])
+        b = dev["z"].shape[0]
+        maps, fmaps = ops.form_bbox_maps(dev["rois"][0], dev["fm_rois"], dev["roi_cls"], dev["num_rois"], rmax, nbf,
+                                         IMG_SIZES[0], cfg.ROI.FM_SIZE)
+        z = dev["noise_shp"][:, :rmax].contiguous()                       # noise_shp[:, :max_num_roi]
+        raw = self.netShpG.forward_nhwc(z, maps, fmaps)
+        s = IMG_SIZES[0]
+        raw_masks = ops.to_nchw(raw, 1).view(b, rmax, s, s)
+        hmaps, bt_masks, fm_bt_masks = ops.form_gen_hmaps(raw_masks, dev["roi_cls"], dev["num_rois"], IMG_SIZES, nbf)
+        return dict(raw_masks=raw_masks, bbox_fmaps=fmaps, hmaps=hmaps, bt_masks=bt_masks, fm_bt_masks=fm_bt_masks)
 
     def _forward(self, dev: dict):
+        if "noise_shp" in dev:
+            d = dict(dev, **self._shapes(dev))
+            d["slabels_feat"] = ops.form_clabels_feat(dev["clabels_emb"], dev["roi_cls"], dev["num_rois"],
+                                                      int(dev["glb_max_num_roi"]))
+            dev = d
         g = self.netG
         g.ca_net.eps_override = dev["eps"]
         try:
@@ -119,9 +178,19 @@ class GSampler:
         with torch.no_grad():
             return self._forward(self._prepare(inp))
 
+    def sample_shapes(self, inp: dict) -> dict:
+        """The generated shapes of a batch without masks (eager): ``raw_masks`` (B, R, 64, 64), the SHP_G_NET output the
+        reference's evaluator displays (evaluator.py:317-320), ``bbox_fmaps`` (B, R, 16, 16), and what G_NET reads:
+        ``hmaps`` (3 scales), ``bt_masks`` (3 scales) and ``fm_bt_masks``, the per-roi ones zero-padded to BOXES_NUM
+        slots.  ``noise_shp`` (B, BOXES_NUM, 4 * num_classes) is taken from the batch when present."""
+        with torch.no_grad():
+            dev = self._prepare({k: v for k, v in inp.items() if k not in ("bt_masks", "fm_bt_masks", "hmaps")})
+            return self._shapes(dev)
+
     def sample(self, inp: dict):
         """fake_imgs, bt_c_codes, att_maps, bt_att_maps, mu, logvar for the batch ``inp`` (the input dict of
-        StepATrainer.generate, full or compact); z / eps are taken from it when present."""
+        StepATrainer.generate, full or compact); z / eps are taken from it when present.  A batch without ``bt_masks``
+        gets its masks from the shape generator (``noise_shp`` taken from it when present)."""
         with torch.no_grad():
             dev = self._prepare(inp)
             key = self._key(dev)
@@ -130,9 +199,9 @@ class GSampler:
                 out = self._forward(dev)          # warm-up: packed weights, allocator state
                 self._graphs[key] = self._capture(dev)
                 return out
-            for k in G_ARGS + ("eps",):
+            for k, v in entry.static_in.items():
                 if k != "glb_max_num_roi":
-                    _copy_into(entry.static_in[k], dev[k])
+                    _copy_into(v, dev[k])
             entry.graph.replay()
             _lib.get().launches += entry.launches
             return _clone_out(entry.static_out)
@@ -147,7 +216,8 @@ class GSampler:
             static_out = self._forward(static_in)
         launches = _lib.get().launches - n0
         _lib.get().launches = n0              # recorded, not executed
-        return _Graph(graph, static_in, static_out, launches, _packed_copies(self.netG))
+        return _Graph(graph, static_in, static_out, launches,
+                      _packed_copies(self.netG) + (_packed_copies(self.netShpG) if self.netShpG is not None else []))
 
 
 def _new_g(num_classes, device):
@@ -160,13 +230,29 @@ def _new_g(num_classes, device):
         model.FAST_INIT = fast
 
 
+def _new_shp_g(num_classes, device):
+    fast, model.FAST_INIT = model.FAST_INIT, True
+    try:
+        return model.SHP_G_NET(num_classes).to(device)
+    finally:
+        model.FAST_INIT = fast
+
+
+def strip_module_prefix(state_dict: dict) -> dict:
+    """A state_dict saved from an nn.DataParallel wrapper (every key ``module.``-prefixed, as the reference's evaluator
+    and shape trainer save it) as the bare module's."""
+    if state_dict and all(k.startswith("module.") for k in state_dict):
+        return {k[len("module."):]: v for k, v in state_dict.items()}
+    return dict(state_dict)
+
+
 def _packed_copies(net):
     """Every kernel-native weight copy the network's layers hold right now (kept alive by a graph that read them)."""
     keep = []
     for m in net.modules():
-        c = getattr(m, "_cache", None)
-        if c is not None:
-            keep.append((c.f, c.t, dict(c.hl), c.amax))
+        for c in (getattr(m, "_cache", None), *getattr(m, "_caches", ())):
+            if c is not None:
+                keep.append((c.f, c.t, dict(c.hl), c.amax))
     return keep
 
 
