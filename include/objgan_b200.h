@@ -320,6 +320,27 @@ int og_mul_pixels(const float* x, const float* s, long long P, int C, float* out
 int og_gen_hmaps(float* slots, int B, long long P, int Cs, const long long* cls, int boxes, const long long* num_rois,
                  int ncls, int Cp, float* hmap, cudaStream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * Text encoder and word inputs of caption-conditioned sampling (ref: model.py:85-179 RNN_ENCODER in eval mode,
+ * evaluator.py:337-351, 148-164)
+ *  og_lstm_bidir      : the whole recurrence of a one-layer bidirectional LSTM (H = 128 per direction) in one launch.
+ *                       gx [B*L][8H]: x-part of the gates plus b_ih + b_hh at every step (row b*L + t; forward
+ *                       direction in channels [0, 4H), backward in [4H, 8H), gate order i, f, g, o); whh_* [4H][H];
+ *                       lens [B] int64 in [1, L].  Sample b runs its own lens[b] steps each way from a zero state;
+ *                       words [B][2H][L] (forward in channels [0, H), backward in [H, 2H), every column t >= lens[b]
+ *                       zero); sent [B][2H] = [forward h after token lens[b]-1, backward h after token 0].  Fixed-order
+ *                       fp32 FMA, no atomics: a sample's outputs do not depend on B or on its place in the batch.
+ *  og_text_inputs     : glove_words [B][E][L] = glove[glove_ids[b][t]] and mask [B][L] bytes = (captions[b][t] == 0),
+ *                       t < L, from row-major int64 id tables with row strides cap_ld / glove_ld (>= L).
+ *  og_class_label_emb : prepare_cat_emb: row k of the labels [n][lab_ld] is the mean of its first lens[k] GloVe vectors
+ *                       when lens[k] is 1 or 2, else zeros; out [n][E] row i = row order[i]. */
+int og_lstm_bidir(const float* gx, const float* whh_f, const float* whh_b, const long long* lens, int B, int L, int H,
+                  float* words, float* sent, cudaStream_t stream);
+int og_text_inputs(const long long* captions, int cap_ld, const long long* glove_ids, int glove_ld, const float* glove,
+                   int E, int B, int L, float* glove_words, unsigned char* mask, cudaStream_t stream);
+int og_class_label_emb(const float* glove, int E, const long long* labels, int lab_ld, const long long* lens,
+                       const long long* order, int n, float* out, cudaStream_t stream);
+
 /* zero-fill (a memset node when captured in a CUDA graph; no kernel launch) */
 int og_zero_bytes(float* p, long long bytes, cudaStream_t stream);
 

@@ -21,6 +21,7 @@ def default_cfg():
     c = AttrDict()
     c.GPU_IDS = "0"
     c.CUDA = True
+    c.RNN_TYPE = "LSTM"    # the text encoder's recurrent cell; RNN_ENCODER implements the LSTM only
     c.TREE = AttrDict(BRANCH_NUM=3, BASE_SIZE=64)
     c.TRAIN = AttrDict(
         BATCH_SIZE=16, DISCRIMINATOR_LR=2e-4, GENERATOR_LR=2e-4, BUATTN_NORM=True,

@@ -624,6 +624,100 @@ class SHP_G_NET(_Base):
 
 
 # --------------------------------------------------------------------------------------------------
+# text encoder
+# --------------------------------------------------------------------------------------------------
+class _EmbeddingP(nn.Module):
+    """nn.Embedding's ``weight`` (ntoken, ninput), initialised like RNN_ENCODER.init_weights (model.py:125-127)."""
+
+    def __init__(self, ntoken, ninput):
+        super().__init__()
+        self.weight = nn.Parameter(torch.empty(ntoken, ninput).uniform_(-0.1, 0.1))
+
+
+class _BiLSTMP(nn.Module):
+    """One-layer bidirectional nn.LSTM's parameters, in its state_dict order and with its initialisation."""
+
+    def __init__(self, ninput, nhidden):
+        super().__init__()
+        k = 1.0 / np.sqrt(nhidden)
+        for sfx in ("", "_reverse"):
+            for name, shape in (("weight_ih", (4 * nhidden, ninput)), ("weight_hh", (4 * nhidden, nhidden)),
+                                ("bias_ih", (4 * nhidden,)), ("bias_hh", (4 * nhidden,))):
+                self.register_parameter(f"{name}_l0{sfx}", nn.Parameter(torch.empty(shape).uniform_(-k, k)))
+
+
+class RNN_ENCODER(_Base):
+    """ref: model.py:85-179 -- same constructor, state_dict keys / shapes and ``forward(captions, cap_lens, max_len)``
+    -> (words_emb (B, nhidden, max_len), sent_emb (B, nhidden)).  Inference only (the reference always runs it after
+    .eval(): trainer.py:100, evaluator.py:95): dropout is not implemented, so a forward in training mode raises, and so
+    does one with grad mode on and parameters that require grad.  One-layer bidirectional LSTM only.
+
+    The batch need not be sorted by length: each sample runs its own cap_lens[b] steps, with results bitwise
+    independent of its place in the batch.  The forward is three library calls -- the token lookup
+    (og_gather_rows from a channel-padded copy of ``encoder.weight``), the x-part of the gates of both directions for
+    every step (one 1x1 og_conv2d_simt with bias b_ih + b_hh) and the recurrence (og_lstm_bidir) -- and reads no
+    lengths on the host.  The padded copies are derived from the parameters and refreshed whenever they change."""
+
+    def __init__(self, ntoken, ninput=300, drop_prob=0.5, nhidden=128, nlayers=1, bidirectional=True):
+        super().__init__()
+        if cfg.RNN_TYPE != "LSTM" or nlayers != 1 or not bidirectional:
+            raise NotImplementedError("RNN_ENCODER supports the one-layer bidirectional LSTM only")
+        self.n_steps = cfg.TEXT.WORDS_NUM
+        self.ntoken, self.ninput, self.drop_prob = ntoken, ninput, drop_prob
+        self.nlayers, self.bidirectional, self.rnn_type = nlayers, bidirectional, cfg.RNN_TYPE
+        self.num_directions = 2
+        self.nhidden = nhidden // self.num_directions
+        self.encoder = _EmbeddingP(ntoken, ninput)
+        self.rnn = _BiLSTMP(ninput, self.nhidden)
+        self._derived_key = None
+        self._emb = self._wih = self._bias = None
+        self._cache = ops.PackedWeights()
+
+    def _params_key(self):
+        ps = list(self.parameters())
+        return tuple((p.data_ptr(), p._version) for p in ps) + (ops._epoch_of(ps[0]),)
+
+    def derived_weights(self):
+        """(encoder.weight padded to cpad(ninput) channels, W_ih of both directions as a (8H, ninput, 1, 1) conv weight,
+        b_ih + b_hh of both directions (8H,)), rebuilt when a parameter changes, in place (stable addresses)."""
+        key = self._params_key()
+        if key != self._derived_key:
+            w, r = self.encoder.weight, self.rnn
+            dev, cp, g = w.device, cpad(self.ninput), 4 * self.nhidden
+            if self._emb is None or self._emb.device != dev:
+                self._emb = torch.empty((self.ntoken, cp), device=dev, dtype=torch.float32)
+                self._wih = torch.empty((2 * g, self.ninput, 1, 1), device=dev, dtype=torch.float32)
+                self._bias = torch.empty((2 * g,), device=dev, dtype=torch.float32)
+            ops.zeros_into(self._emb)
+            ops.copy_channels(w.detach(), self.ninput, self._emb, cp, self.ntoken)
+            wih = self._wih.view(2 * g, self.ninput)
+            wih[:g].copy_(r.weight_ih_l0.detach())
+            wih[g:].copy_(r.weight_ih_l0_reverse.detach())
+            ops.add_into(r.bias_ih_l0, r.bias_hh_l0, self._bias[:g])
+            ops.add_into(r.bias_ih_l0_reverse, r.bias_hh_l0_reverse, self._bias[g:])
+            self._derived_key = self._params_key()
+        return self._emb, self._wih, self._bias
+
+    def _check_inference(self, *inputs):
+        if self.training:
+            raise RuntimeError("RNN_ENCODER is inference only and has no dropout: call .eval() first")
+        ops.inference_only("RNN_ENCODER", *inputs, *self.parameters())
+
+    def forward(self, captions, cap_lens, max_len, mask=None):
+        """captions (B, >= max_len) int64 token ids, cap_lens (B,) int64 in [1, max_len] (device tensors; not read on
+        the host), max_len: the words_emb width (the reference passes max(cap_lens))."""
+        self._check_inference()
+        b, max_len = captions.shape[0], int(max_len)
+        assert captions.shape[1] >= max_len and cap_lens.shape == (b,)
+        emb, wih, bias = self.derived_weights()
+        ids = captions[:, :max_len]
+        ids = ids if ids.is_contiguous() else ids.contiguous()
+        x = ops.gather_rows(emb, ids.reshape(-1))                                     # (B*L, cpad(ninput))
+        gx = ops.linear_rows(x, wih, bias, self._cache)                               # (B*L, 8H)
+        return ops.lstm_bidir(gx, self.rnn.weight_hh_l0, self.rnn.weight_hh_l0_reverse, cap_lens, max_len)
+
+
+# --------------------------------------------------------------------------------------------------
 # discriminators
 # --------------------------------------------------------------------------------------------------
 class _EncodeImage(nn.Module):

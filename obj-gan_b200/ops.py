@@ -1715,3 +1715,88 @@ def adam_ema_(p, g, m, v, avg, step, *, lr=2e-4, b1=0.5, b2=0.999, eps=1e-8, gsc
           int(step), _p(step_dev), float(gscale), float(decay))
     if bump:
         bump_param_epoch()
+
+
+# --------------------------------------------------------------------------------------------------
+# Text stage (the text encoder and the word inputs of caption-conditioned sampling).  Inference only.
+# --------------------------------------------------------------------------------------------------
+def zeros_into(t):
+    """t.zero_() through cudaMemsetAsync."""
+    _chk(t)
+    _call("og_zero_bytes", _p(t), t.numel() * 4)
+
+
+def copy_channels(src, sstride, dst, dstride, rows):
+    """dst[p, :sstride] = src[p, :] for p < rows: row-major src (rows, sstride) into the wider rows of dst."""
+    _chk(src, dst)
+    _call("og_copy_channels", _p(src.contiguous()), sstride, 0, _p(dst), dstride, 0, sstride, rows, 0)
+
+
+def add_into(a, b, out):
+    """out = a + b elementwise (out: a contiguous view of the same size)."""
+    _chk(a, b, out)
+    _call("og_add", _p(a.detach().contiguous()), _p(b.detach().contiguous()), _p(out), a.numel())
+
+
+def linear_rows(x, w, bias, cache):
+    """y = x w^T + bias over rows as one 1x1 og_conv2d_simt (exact fp32, no split-K): x (N, cpad(Ci)) with zero pad
+    lanes, w (Co, Ci, 1, 1), bias (Co,) -> (N, Co)."""
+    _chk(x, w, bias)
+    n, c = x.shape
+    co, ci = w.shape[:2]
+    assert c == cpad(ci) and co % 4 == 0
+    wf, _ = cache.get(w, c, co, 0, 0, False)
+    return _conv_raw(x.contiguous(), wf, n, 1, 1, c, 1, 1, co, 1, 1, 1, 0, PAD_ZERO, bias, ACT_NONE,
+                     splitk=False).view(n, co)
+
+
+def lstm_bidir(gx, whh_f, whh_b, cap_lens, max_len):
+    """The recurrence of a one-layer bidirectional LSTM (H = 128) in one launch: gx (B*max_len, 8H) x-parts of the gates
+    with both biases (og_lstm_bidir), cap_lens (B,) int64 in [1, max_len] on the device -> words_emb (B, 2H, max_len),
+    every column t >= cap_lens[b] zero, and sent_emb (B, 2H)."""
+    _chk(gx, whh_f, whh_b, cap_lens)
+    inference_only("lstm_bidir", gx, whh_f, whh_b)
+    h = whh_f.shape[1]
+    b = cap_lens.shape[0]
+    assert gx.shape == (b * max_len, 8 * h) and whh_f.shape == whh_b.shape == (4 * h, h)
+    words = torch.empty((b, 2 * h, max_len), device=gx.device, dtype=torch.float32)
+    sent = torch.empty((b, 2 * h), device=gx.device, dtype=torch.float32)
+    _call("og_lstm_bidir", _p(gx.contiguous()), _p(whh_f.detach().contiguous()), _p(whh_b.detach().contiguous()),
+          _p(_i64(cap_lens)), b, max_len, h, _p(words), _p(sent))
+    return words, sent
+
+
+def text_inputs(captions, glove_captions, glove, max_len):
+    """evaluator.py:340-351 on the device: (glove_words_embs (B, E, max_len) = glove[glove_captions[:, :max_len]]
+    transposed, mask (B, max_len) bool = (captions == 0)[:, :max_len]) in one launch."""
+    _chk(captions, glove_captions, glove)
+    c, g = _i64(captions), _i64(glove_captions)
+    b, e = c.shape[0], glove.shape[1]
+    words = torch.empty((b, e, max_len), device=glove.device, dtype=torch.float32)
+    mask = torch.empty((b, max_len), device=glove.device, dtype=torch.uint8)
+    _call("og_text_inputs", _p(c), c.shape[1], _p(g), g.shape[1], _p(glove.detach().contiguous()), e, b, max_len,
+          _p(words), _p(mask))
+    return words, mask.view(torch.bool)
+
+
+def class_label_emb(glove_weight, cat_labels, cat_label_lens, order):
+    """prepare_cat_emb (ref: evaluator.py:148-164, trainer.py:227-241) on the device: over the length-sorted labels
+    ``cat_labels`` (N, W) int64 (GloVe ids) and ``cat_label_lens`` (N,) of load.py:305-355, row k is the mean of the
+    label's GloVe vectors when it has 1 or 2 tokens and zeros otherwise; the result is indexed by ``order`` (the
+    "resort" indices).  Returns (N, E)."""
+    lab, lens, order = _i64(cat_labels), _i64(cat_label_lens), _i64(order)
+    n, e = order.shape[0], glove_weight.shape[1]
+    if not _lib.DRY_RUN:                       # built once per sampler: a host read of the tables is cheap here
+        lab_h, lens_h, order_h = lab.cpu(), lens.cpu(), order.cpu()
+        read = (torch.arange(lab_h.shape[1]).view(1, -1) < lens_h.view(-1, 1)) & (lens_h <= 2).view(-1, 1)
+        if lens_h.shape[0] != lab_h.shape[0] or bool(((lens_h == 2) & (lab_h.shape[1] < 2)).any()):
+            raise ValueError("cat_label_lens does not match cat_labels")
+        if bool(((lab_h < 0) | (lab_h >= glove_weight.shape[0]))[read].any()):
+            raise ValueError("a class label token is outside the GloVe table")
+        if bool(((order_h < 0) | (order_h >= lab_h.shape[0])).any()):
+            raise ValueError("cat_label_order indexes past the labels")
+    _chk(glove_weight, lab, lens, order)
+    out = torch.empty((n, e), device=glove_weight.device, dtype=torch.float32)
+    _call("og_class_label_emb", _p(glove_weight.detach().contiguous()), e, _p(lab), lab.shape[1], _p(lens), _p(order),
+          n, _p(out))
+    return out

@@ -5,13 +5,18 @@ With a shape generator (``SHP_G_NET``, ref: evaluator.py:111-144), a batch that 
 way the reference's default evaluator mode does it (cfg.TEST.USE_GT_BOX_SEG = 1 / 2, evaluator.py:314-332): box maps ->
 SHP_G_NET -> form_hmaps -> label embeddings -> G_NET, all on the device and inside the same per-shape CUDA graph.
 
+With a text encoder (``RNN_ENCODER``) and the GloVe table (ref: evaluator.py:90-95, 337-351), a batch that brings
+``captions``, ``cap_lens`` and ``glove_captions`` instead of ``words_embs`` is encoded on the device inside the same
+graph: token ids -> text encoder + GloVe lookups + padding mask -> (shape generator) -> G_NET.
+
 ``GSampler`` holds its own G_NET in eval mode, so BatchNorm normalises with the running statistics and never updates
 them.  A forward pass is ~200 library calls, which cost far more host time than the kernels take at small batch, so
 every input shape is captured once into a CUDA graph and replayed after that:
 
-  * graphs are keyed by (B, L, Rmax, glb_max_num_roi, generated shapes): batch, caption length, roi slots of
-    ``slabels_feat`` (glb_max_num_roi when the shapes are generated), the roi width of the returned ``bt_c_code``, and
-    whether the masks come from the batch or from the shape generator.  Rmax is NOT padded to BOXES_NUM to share one graph: the bottom-up paint
+  * graphs are keyed by (B, L, Rmax, glb_max_num_roi, text, generated shapes): batch, caption length (max(cap_lens)
+    for a caption batch), roi slots of ``slabels_feat`` (glb_max_num_roi when the shapes are generated), the roi
+    width of the returned ``bt_c_code``, whether the word embeddings come from the batch or from the text encoder,
+    and whether the masks come from the batch or from the shape generator.  Rmax is NOT padded to BOXES_NUM to share one graph: the bottom-up paint
     takes a max over the roi axis, and an extra zero slot contributes 0 to that max, which changes the result wherever
     every real roi's product is negative;
   * the first call with a key runs eagerly (the warm-up: packed weight copies, allocator), then captures; later calls
@@ -36,6 +41,9 @@ G_ARGS = ("z", "sent_emb", "words_embs", "glove_words_embs", "slabels_feat", "ma
 # what the generated-shape path reads: the layout (boxes and classes), the shape noise, and the label embeddings
 GEN_ARGS = ("z", "eps", "noise_shp", "sent_emb", "words_embs", "glove_words_embs", "mask", "rois", "fm_rois", "num_rois",
             "roi_cls", "clabels_emb", "glb_max_num_roi")
+# what the text encoder stage computes, and what it reads instead (ref: evaluator.py:337-351)
+TEXT_OUT = ("sent_emb", "words_embs", "glove_words_embs", "mask")
+TEXT_ARGS = ("captions", "cap_lens", "glove_captions", "max_len")
 
 
 def _map(x, f):
@@ -66,26 +74,51 @@ class _Graph:
 class GSampler:
     """Eval-mode G_NET forward with the reference's inputs and 6-tuple output, CUDA-graph replayed per input shape."""
 
-    def __init__(self, netG: model.G_NET, netShpG: model.SHP_G_NET | None = None):
+    def __init__(self, netG: model.G_NET, netShpG: model.SHP_G_NET | None = None,
+                 text_encoder: model.RNN_ENCODER | None = None, glove=None, clabels_emb=None):
+        """``glove``: the GloVe table (V, 50) as a tensor or an nn.Embedding (the reference's ``glove_emb``);
+        ``clabels_emb``: (num_classes, 50) label embeddings (see ops.class_label_emb) used when a batch has none."""
         self.netG = netG.eval()
         self.netShpG = netShpG.eval() if netShpG is not None else None
-        for net in (self.netG, self.netShpG):
+        self.text_encoder = text_encoder.eval() if text_encoder is not None else None
+        for net in (self.netG, self.netShpG, self.text_encoder):
             for p in (net.parameters() if net is not None else ()):
                 p.requires_grad_(False)
         self.device = next(self.netG.parameters()).device
+        glove = getattr(glove, "weight", glove)
+        self.glove = glove.detach().to(self.device).float().contiguous() if glove is not None else None
+        self.clabels_emb = clabels_emb.detach().to(self.device).float().contiguous() if clabels_emb is not None else None
         self._graphs = {}
         self._pool = None
 
     @classmethod
-    def from_snapshot(cls, path: str, num_classes: int = 80, device="cuda", shape_snapshot: str | None = None) -> "GSampler":
+    def from_snapshot(cls, path: str, num_classes: int = 80, device="cuda", shape_snapshot: str | None = None,
+                      text_snapshot: str | None = None, glove=None, cat_labels=None, cat_label_lens=None,
+                      cat_label_order=None) -> "GSampler":
         """A reference-format generator snapshot (``netG_epoch_N.pth``, what StepBTrainer.save_model writes), and
-        optionally a shape generator snapshot (the reference's ``cfg.TEST.NET_SHP_G``; keys with or without the
-        ``module.`` prefix that nn.DataParallel adds)."""
+        optionally a shape generator snapshot (the reference's ``cfg.TEST.NET_SHP_G``) and a text encoder snapshot
+        (``cfg.TRAIN.NET_E``; ntoken is read from its ``encoder.weight``); keys with or without the ``module.`` prefix
+        that nn.DataParallel adds.  ``glove``: the GloVe table; ``cat_labels`` / ``cat_label_lens`` /
+        ``cat_label_order``: the length-sorted class labels, their lengths and the resort indices of the reference's
+        load_cat_label (load.py:305-355), from which the label embeddings are computed once (prepare_cat_emb)."""
         shp = _new_shp_g(num_classes, device) if shape_snapshot is not None else None
-        s = cls(_new_g(num_classes, device), shp)
+        enc = None
+        if text_snapshot is not None:
+            text_sd = strip_module_prefix(torch.load(text_snapshot, map_location="cpu"))
+            enc = model.RNN_ENCODER(text_sd["encoder.weight"].shape[0], nhidden=cfg.TEXT.EMBEDDING_DIM).to(device)
+        clabels = None
+        if cat_labels is not None:
+            if glove is None:
+                raise ValueError("cat_labels need the GloVe table (glove=...)")
+            gw = getattr(glove, "weight", glove).detach().to(device).float()
+            clabels = ops.class_label_emb(gw, cat_labels.to(device), cat_label_lens.to(device),
+                                          cat_label_order.to(device))
+        s = cls(_new_g(num_classes, device), shp, enc, glove, clabels)
         s.load_state_dict(torch.load(path, map_location="cpu"))
         if shape_snapshot is not None:
             s.load_shape_state_dict(torch.load(shape_snapshot, map_location="cpu"))
+        if text_snapshot is not None:
+            s.load_text_state_dict(text_sd)
         return s
 
     @classmethod
@@ -108,6 +141,14 @@ class GSampler:
         self._graphs.clear()
         self.netShpG.load_state_dict(strip_module_prefix(state_dict), strict=True)
 
+    def load_text_state_dict(self, state_dict: dict) -> None:
+        """Loads RNN_ENCODER weights (strict; a ``module.`` prefix on every key is dropped) and drops every captured
+        graph."""
+        if self.text_encoder is None:
+            raise ValueError("this sampler has no text encoder: build it with GSampler(netG, text_encoder=...)")
+        self._graphs.clear()
+        self.text_encoder.load_state_dict(strip_module_prefix(state_dict), strict=True)
+
     # ------------------------------------------------------------------ inputs
     def _prepare(self, inp: dict) -> dict:
         """Device copies of the inputs G_NET reads (+ the derived tensors of a compact batch), with z and the CA_NET
@@ -115,19 +156,55 @@ class GSampler:
         dev = {}
         for k, v in inp.items():
             dev[k] = _map(v, lambda t: t.to(self.device, non_blocking=True))
+        text = self._text_mode(dev)
+        if dev.get("clabels_emb") is None and self.clabels_emb is not None:
+            dev["clabels_emb"] = self.clabels_emb
         gen = self._generates(dev)
         if gen and dev.get("roi_cls") is None:
             dev["roi_cls"] = dev["rois"][0][..., 4].to(torch.int64)
         if not gen and "hmaps" not in dev and "roi_cls" in dev:
             prepare_data(dev, self.netG.num_classes)
-        b = dev["sent_emb"].shape[0]
+        b = dev["num_rois"].shape[0]
         if dev.get("z") is None:
             dev["z"] = torch.randn(b, cfg.GAN.Z_DIM, device=self.device)      # noise_img.data.normal_(0, 1)
         if dev.get("eps") is None:
             dev["eps"] = torch.randn(b, cfg.GAN.CONDITION_DIM, device=self.device)   # CA_NET.reparametrize
         if gen and dev.get("noise_shp") is None:                              # noise_shp.data.normal_(0, 1)
             dev["noise_shp"] = torch.randn(b, cfg.ROI.BOXES_NUM, 4 * self.netShpG.nbf, device=self.device)
-        return {k: dev[k] for k in (GEN_ARGS if gen else (*G_ARGS, "eps"))}
+        keys = GEN_ARGS if gen else (*G_ARGS, "eps")
+        if text:
+            keys = tuple(k for k in keys if k not in TEXT_OUT) + TEXT_ARGS
+        return {k: dev[k] for k in keys}
+
+    def _text_mode(self, dev: dict) -> bool:
+        """Whether the batch's word embeddings come from the text encoder (captions and no ``words_embs``).  Checks the
+        caption inputs before anything is launched (one device -> host read, like the reference's
+        int(torch.max(cap_lens))) and sets ``max_len`` = max(cap_lens)."""
+        if dev.get("words_embs") is not None or dev.get("captions") is None:
+            return False
+        if self.text_encoder is None or self.glove is None:
+            raise ValueError("the batch has captions but no words_embs, and this sampler has no text encoder and GloVe "
+                             "table: build it with GSampler(netG, text_encoder=..., glove=...) or "
+                             "GSampler.from_snapshot(..., text_snapshot=..., glove=...)")
+        caps, lens, gcaps = dev["captions"], dev["cap_lens"], dev["glove_captions"]
+        b = caps.shape[0]
+        if caps.dim() != 2 or lens.shape != (b,) or gcaps.dim() != 2 or gcaps.shape[0] != b:
+            raise ValueError("captions (B, T), cap_lens (B,) and glove_captions (B, T') must agree on B")
+        for name, t in (("captions", caps), ("cap_lens", lens), ("glove_captions", gcaps)):
+            if t.dtype != torch.int64:
+                raise ValueError(f"{name} must be int64")
+        lo_c, hi_c, lo_g, hi_g, lo_l, hi_l = torch.stack(
+            [caps.min(), caps.max(), gcaps.min(), gcaps.max(), lens.min(), lens.max()]).tolist()
+        words_num = cfg.TEXT.WORDS_NUM
+        if lo_l < 1 or hi_l > min(words_num, caps.shape[1], gcaps.shape[1]):
+            raise ValueError(f"cap_lens must lie in [1, {words_num}] and within the caption width, got [{lo_l}, {hi_l}]")
+        if lo_c < 0 or hi_c >= self.text_encoder.ntoken:
+            raise ValueError(f"caption token ids must lie in [0, {self.text_encoder.ntoken}), got [{lo_c}, {hi_c}]")
+        if lo_g < 0 or hi_g >= self.glove.shape[0]:
+            raise ValueError(f"GloVe token ids must lie in [0, {self.glove.shape[0]}), got [{lo_g}, {hi_g}]")
+        dev["max_len"] = int(hi_l)
+        dev["captions"], dev["glove_captions"] = caps.contiguous(), gcaps.contiguous()
+        return True
 
     def _generates(self, dev: dict) -> bool:
         """Whether the batch's masks come from the shape generator (the batch brings no ``bt_masks``)."""
@@ -141,8 +218,17 @@ class GSampler:
     @staticmethod
     def _key(dev: dict) -> tuple:
         gen = "noise_shp" in dev
+        text = "captions" in dev
         rmax = int(dev["glb_max_num_roi"]) if gen else dev["slabels_feat"].shape[2]
-        return (dev["z"].shape[0], dev["words_embs"].shape[2], rmax, int(dev["glb_max_num_roi"]), gen)
+        length = dev["max_len"] if text else dev["words_embs"].shape[2]
+        return (dev["z"].shape[0], length, rmax, int(dev["glb_max_num_roi"]), text, gen)
+
+    def _text(self, dev: dict) -> dict:
+        """captions -> RNN_ENCODER (words_embs, sent_emb), GloVe lookups and mask (ref: evaluator.py:337-351)."""
+        n = dev["max_len"]
+        words, sent = self.text_encoder(dev["captions"], dev["cap_lens"], n)
+        glove_words, mask = ops.text_inputs(dev["captions"], dev["glove_captions"], self.glove, n)
+        return dict(words_embs=words, sent_emb=sent, mask=mask, glove_words_embs=glove_words)
 
     def _shapes(self, dev: dict) -> dict:
         """Box maps -> SHP_G_NET -> form_hmaps (ref: evaluator.py:315-328): the raw masks (B, R, 64, 64) and the heat
@@ -160,6 +246,8 @@ class GSampler:
         return dict(raw_masks=raw_masks, bbox_fmaps=fmaps, hmaps=hmaps, bt_masks=bt_masks, fm_bt_masks=fm_bt_masks)
 
     def _forward(self, dev: dict):
+        if "captions" in dev:
+            dev = dict(dev, **self._text(dev))
         if "noise_shp" in dev:
             d = dict(dev, **self._shapes(dev))
             d["slabels_feat"] = ops.form_clabels_feat(dev["clabels_emb"], dev["roi_cls"], dev["num_rois"],
@@ -186,6 +274,16 @@ class GSampler:
         with torch.no_grad():
             dev = self._prepare({k: v for k, v in inp.items() if k not in ("bt_masks", "fm_bt_masks", "hmaps")})
             return self._shapes(dev)
+
+    def encode_text(self, inp: dict) -> dict:
+        """The text stage of a caption batch (eager): ``words_embs`` (B, 256, max_len), ``sent_emb`` (B, 256), ``mask``
+        (B, max_len) bool and ``glove_words_embs`` (B, 50, max_len), max_len = max(cap_lens)."""
+        with torch.no_grad():
+            dev = {k: _map(v, lambda t: t.to(self.device, non_blocking=True)) for k, v in inp.items()
+                   if k in ("captions", "cap_lens", "glove_captions")}
+            if not self._text_mode(dev):
+                raise ValueError("encode_text needs captions, cap_lens and glove_captions")
+            return self._text(dev)
 
     def sample(self, inp: dict):
         """fake_imgs, bt_c_codes, att_maps, bt_att_maps, mu, logvar for the batch ``inp`` (the input dict of
@@ -216,8 +314,8 @@ class GSampler:
             static_out = self._forward(static_in)
         launches = _lib.get().launches - n0
         _lib.get().launches = n0              # recorded, not executed
-        return _Graph(graph, static_in, static_out, launches,
-                      _packed_copies(self.netG) + (_packed_copies(self.netShpG) if self.netShpG is not None else []))
+        nets = [n for n in (self.netG, self.netShpG, self.text_encoder) if n is not None]
+        return _Graph(graph, static_in, static_out, launches, [c for n in nets for c in _packed_copies(n)])
 
 
 def _new_g(num_classes, device):
