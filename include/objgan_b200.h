@@ -340,6 +340,44 @@ int og_text_inputs(const long long* captions, int cap_ld, const long long* glove
                    int E, int B, int L, float* glove_words, unsigned char* mask, cudaStream_t stream);
 int og_class_label_emb(const float* glove, int E, const long long* labels, int lab_ld, const long long* lens,
                        const long long* order, int n, float* out, cudaStream_t stream);
+/* og_lstm_bidir_state: og_lstm_bidir that also writes the final cell state cell [B][2H] in the layout of sent (the
+ *                       forward c after token lens[b]-1, the backward c after token 0), the encoder state the box
+ *                       decoder starts from (ref: box_generation/seq2seq/models/PreEncoderRNN.py:59-99). */
+int og_lstm_bidir_state(const float* gx, const float* whh_f, const float* whh_b, const long long* lens, int B, int L,
+                        int H, float* words, float* sent, float* cell, cudaStream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------
+ * Box generator of caption-to-image sampling (ref: box_generation/seq2seq/models/DecoderRNN.py:81-183, 260-292,
+ * 350-384 in inference; seq2seq/evaluator/evaluator.py:74-139; image_generation/miscc/load.py:653-776)
+ *  og_box_label_table : table [NL][1024] = b_ih + b_hh + W_ih[:, 100:356] emb[l], one fmaf chain per entry in column
+ *                       order; W_ih [1024][356] row-major, emb [NL][256].
+ *  og_box_decode      : every decoding step of B samples in one launch.  h0 / c0 [B][256] (encoder directions
+ *                       concatenated); wt [356][1024] = [W_ih[:, 0:100] | W_hh]^T; *_w (50, 2) and *_b (50,) of
+ *                       xy_embedding / wh_embedding / next_xy_embedding; lout_t [256][NL], xyo_t [256+NL][30] and
+ *                       who_t [256+NL+50][30] the transposed heads; noise [B][S][6] = (u_xy, n1, n2, u_wh, n3, n4),
+ *                       uniforms in [0, 1) and standard normals.  The first step reads label sos and (x0, y0, w0, r0);
+ *                       a sample stops after the step whose label is eos or after S steps.  labels [B][S] (-1 after
+ *                       the end), samples [B][S][4] normalised (x, y, w, r; 0 after the end), steps [B]; dbg null or
+ *                       [B][S][NL + 60]: p, then the xy and wh mixture parameters (pi, mu_x, mu_y, sigma_x, sigma_y,
+ *                       rho, 5 each, sigma before the temperature), 0 after the end.  Fixed-order fp32, no atomics: a
+ *                       sample's results do not depend on B or its place in the batch.  NL <= 128.
+ *  og_box_layout      : the evaluator's post-processing and load_gen_insanns per sample, in float64: mean_std [4][2]
+ *                       (mean, std of x, y, w, r), label_to_class [NL] (class row, -1 for the special tokens),
+ *                       count_stats [C][2] (mu, sigma of the per-class count), noise_cnt [B][C] standard normals.
+ *                       rois [3][B][R][6] at 64, 128 and 256 pixels, fm_rois [B][R][6], roi_cls [B][R], num_rois [B],
+ *                       zero-padded to R slots.  S <= 16. */
+int og_box_label_table(const float* emb, const float* w_ih, const float* b_ih, const float* b_hh, int NL, float* table,
+                       cudaStream_t stream);
+int og_box_decode(const float* h0, const float* c0, const float* table, const float* wt, const float* xy_w,
+                  const float* xy_b, const float* wh_w, const float* wh_b, const float* nxy_w, const float* nxy_b,
+                  const float* lout_t, const float* lout_b, const float* xyo_t, const float* xyo_b, const float* who_t,
+                  const float* who_b, const float* noise, int B, int S, int NL, int sos, int eos, float x0, float y0,
+                  float w0, float r0, long long* labels, float* samples, long long* steps, float* dbg,
+                  cudaStream_t stream);
+int og_box_layout(const long long* labels, const float* samples, const long long* steps, const double* mean_std,
+                  const long long* label_to_class, const double* count_stats, const float* noise_cnt, int B, int S,
+                  int NL, int C, int R, int min_size, double* rois, double* fm_rois, long long* roi_cls,
+                  long long* num_rois, cudaStream_t stream);
 
 /* zero-fill (a memset node when captured in a CUDA graph; no kernel launch) */
 int og_zero_bytes(float* p, long long bytes, cudaStream_t stream);

@@ -45,9 +45,12 @@ struct LstmArgs {
   float* words;          // [B][2H][L]
   float* sent;           // [B][2H]
   int B, L;
+  float* cell;           // [B][2H]: c after the same token as sent (CELL instantiations only)
 };
 
-template <int SPW>
+// CELL: also write the final cell state (the encoder state the box decoder starts from); the instantiations without it
+// are the text encoder's.
+template <int SPW, bool CELL>
 __global__ void __cluster_dims__(LSTM_CLUSTER, 1, 1) __launch_bounds__(LSTM_THREADS, 1)
     lstm_bidir_kernel(LstmArgs a) {
   extern __shared__ float4 smem4[];
@@ -134,6 +137,9 @@ __global__ void __cluster_dims__(LSTM_CLUSTER, 1, 1) __launch_bounds__(LSTM_THRE
           const int p = dir ? len[s] - 1 - t : t;
           a.words[(bidx[s] * 2 * LSTM_H + wout) * a.L + p] = h;
           if (t == len[s] - 1) a.sent[bidx[s] * 2 * LSTM_H + wout] = h;   // fwd: h after the last token; bwd: at token 0
+          if constexpr (CELL) {
+            if (t == len[s] - 1) a.cell[bidx[s] * 2 * LSTM_H + wout] = c[s];
+          }
         }
       }
     }
@@ -144,31 +150,44 @@ __global__ void __cluster_dims__(LSTM_CLUSTER, 1, 1) __launch_bounds__(LSTM_THRE
   }
 }
 
-template <int SPW>
+template <int SPW, bool CELL>
 static int lstm_launch(const LstmArgs& a, cudaStream_t stream) {
   static bool ready = false;                          // dynamic smem above 48 KB is opt-in, once per instantiation
   const size_t smem = lstm_smem_bytes(SPW);
   if (!ready) {
-    OG_CHECK(cudaFuncSetAttribute(lstm_bidir_kernel<SPW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    OG_CHECK(cudaFuncSetAttribute(lstm_bidir_kernel<SPW, CELL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)smem));
     ready = true;
   }
   const int bt = LSTM_WARPS * SPW;
   const dim3 grid(2 * LSTM_CLUSTER, og_cdiv(a.B, bt));
-  lstm_bidir_kernel<SPW><<<grid, LSTM_THREADS, smem, stream>>>(a);
+  lstm_bidir_kernel<SPW, CELL><<<grid, LSTM_THREADS, smem, stream>>>(a);
   OG_RETURN_LAST_ERROR();
 }
 
-OG_API int og_lstm_bidir(const float* gx, const float* whh_f, const float* whh_b, const long long* lens, int B, int L,
-                         int H, float* words, float* sent, cudaStream_t stream) {
+template <bool CELL>
+static int lstm_dispatch(const float* gx, const float* whh_f, const float* whh_b, const long long* lens, int B, int L,
+                         int H, float* words, float* sent, float* cell, cudaStream_t stream) {
   if (H != LSTM_H || B < 0 || L < 0) return (int)cudaErrorInvalidValue;
   if (B == 0 || L == 0) return 0;
   LstmArgs a;
   a.gx = gx; a.whh_f = whh_f; a.whh_b = whh_b; a.lens = lens; a.words = words; a.sent = sent; a.B = B; a.L = L;
+  a.cell = cell;
   // the smallest tile that holds the batch (up to 64 samples): fewer samples per warp shorten each step's FMA chain
-  if (B <= 8) return lstm_launch<1>(a, stream);
-  if (B <= 16) return lstm_launch<2>(a, stream);
-  if (B <= 32) return lstm_launch<4>(a, stream);
-  return lstm_launch<8>(a, stream);
+  if (B <= 8) return lstm_launch<1, CELL>(a, stream);
+  if (B <= 16) return lstm_launch<2, CELL>(a, stream);
+  if (B <= 32) return lstm_launch<4, CELL>(a, stream);
+  return lstm_launch<8, CELL>(a, stream);
+}
+
+OG_API int og_lstm_bidir(const float* gx, const float* whh_f, const float* whh_b, const long long* lens, int B, int L,
+                         int H, float* words, float* sent, cudaStream_t stream) {
+  return lstm_dispatch<false>(gx, whh_f, whh_b, lens, B, L, H, words, sent, nullptr, stream);
+}
+
+OG_API int og_lstm_bidir_state(const float* gx, const float* whh_f, const float* whh_b, const long long* lens, int B,
+                               int L, int H, float* words, float* sent, float* cell, cudaStream_t stream) {
+  return lstm_dispatch<true>(gx, whh_f, whh_b, lens, B, L, H, words, sent, cell, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

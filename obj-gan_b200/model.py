@@ -707,14 +707,164 @@ class RNN_ENCODER(_Base):
         """captions (B, >= max_len) int64 token ids, cap_lens (B,) int64 in [1, max_len] (device tensors; not read on
         the host), max_len: the words_emb width (the reference passes max(cap_lens))."""
         self._check_inference()
+        gx, max_len = self._gate_inputs(captions, cap_lens, max_len)
+        return ops.lstm_bidir(gx, self.rnn.weight_hh_l0, self.rnn.weight_hh_l0_reverse, cap_lens, max_len)
+
+    def _gate_inputs(self, captions, cap_lens, max_len):
+        """The x-part of the gates of both directions for the first max_len tokens: (B*max_len, 8H), max_len."""
         b, max_len = captions.shape[0], int(max_len)
         assert captions.shape[1] >= max_len and cap_lens.shape == (b,)
         emb, wih, bias = self.derived_weights()
         ids = captions[:, :max_len]
         ids = ids if ids.is_contiguous() else ids.contiguous()
         x = ops.gather_rows(emb, ids.reshape(-1))                                     # (B*L, cpad(ninput))
-        gx = ops.linear_rows(x, wih, bias, self._cache)                               # (B*L, 8H)
-        return ops.lstm_bidir(gx, self.rnn.weight_hh_l0, self.rnn.weight_hh_l0_reverse, cap_lens, max_len)
+        return ops.linear_rows(x, wih, bias, self._cache), max_len                    # (B*L, 8H)
+
+
+class PreEncoderRNN(RNN_ENCODER):
+    """The box generator's caption encoder (ref: box_generation/seq2seq/models/PreEncoderRNN.py:6-99) -- the same
+    constructor, state_dict keys and shapes, and ``forward(captions, cap_lens)`` -> (output (B, T, 2H), (h_n, c_n)),
+    h_n / c_n (2, B, H), T = max(cap_lens).  The reference builds it with nhidden=256 and loads the image side's
+    text_encoder100.pth (sample.py:179-182), so it is RNN_ENCODER's network and shares its gate-input path; the
+    recurrence also returns the final cell state (og_lstm_bidir_state).  Inference only, like RNN_ENCODER; one-layer
+    bidirectional LSTM with nhidden=256 only.  Captions of any length are read in full (the box path does not truncate
+    them to WORDS_NUM); the recurrence has no length limit and is tested to 64 tokens."""
+
+    def __init__(self, ntoken, ninput=300, drop_prob=0.5, nhidden=128, nlayers=1, bidirectional=True):
+        if nhidden != 256 or nlayers != 1 or not bidirectional:
+            raise NotImplementedError("PreEncoderRNN supports the one-layer bidirectional LSTM with nhidden=256 only")
+        _Base.__init__(self)
+        self.ntoken, self.ninput, self.drop_prob = ntoken, ninput, drop_prob
+        self.nlayers, self.bidirectional, self.rnn_type = nlayers, bidirectional, "LSTM"
+        self.num_directions = 2
+        self.nhidden = nhidden // self.num_directions
+        self.encoder = _EmbeddingP(ntoken, ninput)
+        self.rnn = _BiLSTMP(ninput, self.nhidden)
+        self._derived_key = None
+        self._emb = self._wih = self._bias = None
+        self._cache = ops.PackedWeights()
+
+    def encode_state(self, captions, cap_lens, max_len):
+        """(words (B, 2H, max_len), h (B, 2H), c (B, 2H)): the state with its directions concatenated, as the decoder
+        reads it (DecoderRNN._cat_directions).  cap_lens is not read on the host."""
+        self._check_inference()
+        gx, max_len = self._gate_inputs(captions, cap_lens, max_len)
+        return ops.lstm_bidir_state(gx, self.rnn.weight_hh_l0, self.rnn.weight_hh_l0_reverse, cap_lens, max_len)
+
+    def forward(self, captions, cap_lens):
+        cap_lens = torch.as_tensor(cap_lens, dtype=torch.int64, device=captions.device)
+        words, h, c = self.encode_state(captions, cap_lens, int(cap_lens.max()))   # pad_packed_sequence's width
+        b, hid = captions.shape[0], self.nhidden
+        return words.transpose(1, 2), (h.view(b, 2, hid).transpose(0, 1), c.view(b, 2, hid).transpose(0, 1))
+
+
+class _LinearP(nn.Module):
+    """nn.Linear's ``weight`` / ``bias``."""
+
+    def __init__(self, fin, fout):
+        super().__init__()
+        k = 1.0 / np.sqrt(fin)
+        self.weight = nn.Parameter(torch.empty(fout, fin).uniform_(-k, k))
+        self.bias = nn.Parameter(torch.empty(fout).uniform_(-k, k))
+
+
+class _LSTMP(nn.Module):
+    """One-layer unidirectional nn.LSTM's parameters."""
+
+    def __init__(self, ninput, nhidden):
+        super().__init__()
+        k = 1.0 / np.sqrt(nhidden)
+        for name, shape in (("weight_ih", (4 * nhidden, ninput)), ("weight_hh", (4 * nhidden, nhidden)),
+                            ("bias_ih", (4 * nhidden,)), ("bias_hh", (4 * nhidden,))):
+            self.register_parameter(f"{name}_l0", nn.Parameter(torch.empty(shape).uniform_(-k, k)))
+
+
+class DecoderRNN(_Base):
+    """The box decoder (ref: box_generation/seq2seq/models/DecoderRNN.py:21-79) -- the same constructor, state_dict
+    keys and shapes -- and its inference branch (:260-292) as ``sample``.  Inference only (the reference samples after
+    .eval(), sample.py:165): a sample in training mode raises, and so does one with grad mode on and parameters that
+    require grad.  The attention variant, the GRU cell, more than one layer, and any hidden size but 256 or mixture size
+    but 5 raise NotImplementedError."""
+
+    def __init__(self, l_word2index, x_mean, y_mean, w_mean, r_mean, batch_size, max_len, hidden_size, gmm_comp_num,
+                 n_layers=1, rnn_cell="lstm", bidirectional=False, input_dropout_p=0, dropout_p=0, use_attention=False):
+        super().__init__()
+        if use_attention or str(rnn_cell).lower() != "lstm" or n_layers != 1 or hidden_size != 256 or \
+                gmm_comp_num != 5 or not bidirectional:
+            raise NotImplementedError("DecoderRNN supports the one-layer LSTM decoder without attention (hidden_size "
+                                      "256, 5 mixture components) on a bidirectional encoder only")
+        self.l_word2index = dict(l_word2index)
+        self.l_output_size = len(l_word2index)
+        if self.l_output_size > 128:
+            raise NotImplementedError("DecoderRNN supports at most 128 labels")
+        self.l_sos_id, self.l_eos_id = l_word2index["<sos>"], l_word2index["<eos>"]
+        self.x_mean, self.y_mean, self.w_mean, self.r_mean = x_mean, y_mean, w_mean, r_mean
+        self.batch_size, self.max_length, self.hidden_size = batch_size, max_len, hidden_size
+        self.gmm_comp_num, self.n_layers, self.bidirectional_encoder = gmm_comp_num, n_layers, bidirectional
+        self.input_dropout_p, self.dropout_p, self.use_attention = input_dropout_p, dropout_p, use_attention
+        self.aug_size = 50
+        nl, h, aug = self.l_output_size, hidden_size, self.aug_size
+        self.l_embedding = _EmbeddingP(nl, h)
+        self.xy_embedding = _LinearP(2, aug)
+        self.wh_embedding = _LinearP(2, aug)
+        self.next_xy_embedding = _LinearP(2, aug)
+        self.rnn = _LSTMP(h + 2 * aug, h)
+        self.l_out = _LinearP(h, nl)
+        self.xy_out = _LinearP(h + nl, 6 * gmm_comp_num)
+        self.wh_out = _LinearP(h + nl + aug, 6 * gmm_comp_num)
+        self._derived_key = None
+        self._packed = None
+
+    def _params_key(self):
+        ps = list(self.parameters())
+        return tuple((p.data_ptr(), p._version) for p in ps) + (ops._epoch_of(ps[0]),)
+
+    def packed_weights(self) -> dict:
+        """The kernel-native copies og_box_decode reads (ops.BOX_PACKED), rebuilt in place when a parameter changes:
+        the label table (og_box_label_table), the transposed [xy | wh] columns of W_ih with W_hh, and the transposed
+        heads."""
+        key = self._params_key()
+        if key != self._derived_key:
+            r = self.rnn
+            w = {"wt": torch.cat([r.weight_ih_l0[:, :2 * self.aug_size], r.weight_hh_l0], 1).t(),
+                 "lout_t": self.l_out.weight.t(), "xyo_t": self.xy_out.weight.t(), "who_t": self.wh_out.weight.t(),
+                 "lout_b": self.l_out.bias, "xyo_b": self.xy_out.bias, "who_b": self.wh_out.bias}
+            for k, m in (("xy", self.xy_embedding), ("wh", self.wh_embedding), ("nxy", self.next_xy_embedding)):
+                w[k + "_w"], w[k + "_b"] = m.weight, m.bias
+            if self._packed is None or self._packed["wt"].device != r.weight_hh_l0.device:
+                self._packed = {k: torch.empty(v.shape, device=v.device, dtype=torch.float32) for k, v in w.items()}
+                self._packed["table"] = torch.empty((self.l_output_size, 4 * self.hidden_size),
+                                                    device=r.weight_hh_l0.device, dtype=torch.float32)
+            with torch.no_grad():
+                for k, v in w.items():
+                    self._packed[k].copy_(v)
+                self._packed["table"].copy_(ops.box_label_table(self.l_embedding.weight, r.weight_ih_l0, r.bias_ih_l0,
+                                                                r.bias_hh_l0))
+            self._derived_key = self._params_key()
+        return self._packed
+
+    def _check_inference(self, *inputs):
+        if self.training:
+            raise RuntimeError("DecoderRNN is inference only and has no dropout: call .eval() first")
+        ops.inference_only("DecoderRNN", *inputs, *self.parameters())
+
+    def sample_state(self, h0, c0, noise, early_stop_len, debug=False):
+        """``sample`` on the concatenated state h0 / c0 (B, 256)."""
+        self._check_inference(h0, c0)
+        return ops.box_decode(h0, c0, self.packed_weights(), noise, int(early_stop_len), self.l_sos_id, self.l_eos_id,
+                              (self.x_mean, self.y_mean, self.w_mean, self.r_mean), debug)
+
+    def sample(self, encoder_hidden, noise, early_stop_len=10, debug=False):
+        """The inference branch for every sample of the batch at once, each stopping after its own <eos> step or after
+        early_stop_len steps.  encoder_hidden: (h_n, c_n), each (2, B, 128) (PreEncoderRNN's); noise (B, >=
+        early_stop_len, 6): per step (u_xy, n1, n2, u_wh, n3, n4), two uniforms in [0, 1) for the component choices and
+        four standard normals.  Returns labels (B, S) int64 (-1 after the end), the normalised samples (B, S, 4) (x, y,
+        w, r), the steps taken (B,) and, with debug, (B, S, n_labels + 60): each step's p and both mixture parameter
+        sets (pi, mu_x, mu_y, sigma_x, sigma_y, rho)."""
+        h_n, c_n = encoder_hidden
+        b = h_n.shape[1]
+        cat = lambda t: t.transpose(0, 1).reshape(b, 2 * t.shape[2])     # _cat_directions
+        return self.sample_state(cat(h_n), cat(c_n), noise, early_stop_len, debug)
 
 
 # --------------------------------------------------------------------------------------------------

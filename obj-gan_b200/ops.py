@@ -1800,3 +1800,87 @@ def class_label_emb(glove_weight, cat_labels, cat_label_lens, order):
     _call("og_class_label_emb", _p(glove_weight.detach().contiguous()), e, _p(lab), lab.shape[1], _p(lens), _p(order),
           n, _p(out))
     return out
+
+
+# --------------------------------------------------------------------------------------------------
+# Box stage (the box generator's encoder state, decoder and layout post-processing).  Inference only.
+# --------------------------------------------------------------------------------------------------
+BOX_NOISE = 6           # per sample and step: u_xy, n1, n2, u_wh, n3, n4
+
+
+def lstm_bidir_state(gx, whh_f, whh_b, cap_lens, max_len):
+    """lstm_bidir that also returns the final cell state: (words_emb (B, 2H, max_len), h (B, 2H), c (B, 2H)), h and c
+    with the directions concatenated (forward state after token cap_lens[b]-1, backward state after token 0)."""
+    _chk(gx, whh_f, whh_b, cap_lens)
+    inference_only("lstm_bidir_state", gx, whh_f, whh_b)
+    h = whh_f.shape[1]
+    b = cap_lens.shape[0]
+    assert gx.shape == (b * max_len, 8 * h) and whh_f.shape == whh_b.shape == (4 * h, h)
+    words = torch.empty((b, 2 * h, max_len), device=gx.device, dtype=torch.float32)
+    sent = torch.empty((b, 2 * h), device=gx.device, dtype=torch.float32)
+    cell = torch.empty((b, 2 * h), device=gx.device, dtype=torch.float32)
+    _call("og_lstm_bidir_state", _p(gx.contiguous()), _p(whh_f.detach().contiguous()),
+          _p(whh_b.detach().contiguous()), _p(_i64(cap_lens)), b, max_len, h, _p(words), _p(sent), _p(cell))
+    return words, sent, cell
+
+
+def box_label_table(emb, w_ih, b_ih, b_hh):
+    """(n_labels, 1024) = b_ih + b_hh + W_ih[:, 100:] emb[l] for every label l (og_box_label_table)."""
+    _chk(emb, w_ih, b_ih, b_hh)
+    nl = emb.shape[0]
+    assert emb.shape[1] == 256 and w_ih.shape == (1024, 356)
+    table = torch.empty((nl, 1024), device=emb.device, dtype=torch.float32)
+    _call("og_box_label_table", _p(emb.detach().contiguous()), _p(w_ih.detach().contiguous()),
+          _p(b_ih.detach().contiguous()), _p(b_hh.detach().contiguous()), nl, _p(table))
+    return table
+
+
+BOX_PACKED = ("table", "wt", "xy_w", "xy_b", "wh_w", "wh_b", "nxy_w", "nxy_b", "lout_t", "lout_b", "xyo_t", "xyo_b",
+              "who_t", "who_b")
+
+
+def box_decode(h0, c0, packed, noise, steps, sos, eos, means, debug=False):
+    """Every decoding step of the box decoder in one launch (og_box_decode).  h0 / c0 (B, 256) the encoder state with
+    its directions concatenated, ``packed`` the decoder's derived weights (DecoderRNN.packed_weights), noise (B, >=
+    steps, 6), ``means`` the first step's (x, y, w, r).  Returns labels (B, steps) int64 (-1 after the end), samples
+    (B, steps, 4), steps taken (B,) int64 and, with ``debug``, (B, steps, n_labels + 60): each step's p and both
+    mixture parameter sets."""
+    nz = noise[:, :steps]
+    nz = nz if nz.is_contiguous() else nz.contiguous()
+    _chk(h0, c0, nz, *(packed[k] for k in BOX_PACKED))
+    inference_only("box_decode", h0, c0)
+    b, nl = h0.shape[0], packed["table"].shape[0]
+    assert h0.shape == c0.shape == (b, 256) and nz.shape == (b, steps, BOX_NOISE)
+    dev = h0.device
+    labels = torch.empty((b, steps), device=dev, dtype=torch.int64)
+    samples = torch.empty((b, steps, 4), device=dev, dtype=torch.float32)
+    taken = torch.empty((b,), device=dev, dtype=torch.int64)
+    dbg = torch.empty((b, steps, nl + 60), device=dev, dtype=torch.float32) if debug else None
+    _call("og_box_decode", _p(h0.contiguous()), _p(c0.contiguous()), *(_p(packed[k]) for k in BOX_PACKED), _p(nz), b,
+          steps, nl, int(sos), int(eos), *(float(m) for m in means), _p(labels), _p(samples), _p(taken), _p(dbg))
+    return labels, samples, taken, dbg
+
+
+def boxes_to_layout(labels, samples, steps, mean_std, label_to_class, count_stats, noise_cnt, boxes_num=10,
+                    min_size=10):
+    """The evaluator's post-processing of decoder samples and the loader's reading of boxes.txt (ref:
+    box_generation/seq2seq/evaluator/evaluator.py:74-139, image_generation/miscc/load.py:653-776) on the device
+    (og_box_layout): labels (B, S) int64, samples (B, S, 4) normalised, steps (B,), mean_std (4, 2) float64 (mean, std of
+    x, y, w, r), label_to_class (n_labels,) int64 (class row, -1 for the special tokens), count_stats (C, 2) float64
+    (mu, sigma of the per-class box count), noise_cnt (B, C) standard normals.  Returns rois (a list of three (B,
+    boxes_num, 6) float64 tables at 64, 128 and 256 pixels), fm_rois (B, boxes_num, 6), roi_cls (B, boxes_num) int64 and
+    num_rois (B,) int64, zero-padded to boxes_num slots."""
+    ms, cs = mean_std.to(torch.float64).contiguous(), count_stats.to(torch.float64).contiguous()
+    ncnt = noise_cnt.to(torch.float32).contiguous()
+    _chk(labels, samples, steps, ms, label_to_class, cs, ncnt)
+    b, s = labels.shape
+    nl, c = label_to_class.shape[0], cs.shape[0]
+    assert samples.shape == (b, s, 4) and ms.shape == (4, 2) and cs.shape == (c, 2) and ncnt.shape == (b, c)
+    dev = labels.device
+    rois = torch.empty((3, b, boxes_num, 6), device=dev, dtype=torch.float64)
+    fm_rois = torch.empty((b, boxes_num, 6), device=dev, dtype=torch.float64)
+    roi_cls = torch.empty((b, boxes_num), device=dev, dtype=torch.int64)
+    num_rois = torch.empty((b,), device=dev, dtype=torch.int64)
+    _call("og_box_layout", _p(_i64(labels)), _p(samples.contiguous()), _p(_i64(steps)), _p(ms), _p(_i64(label_to_class)),
+          _p(cs), _p(ncnt), b, s, nl, c, boxes_num, int(min_size), _p(rois), _p(fm_rois), _p(roi_cls), _p(num_rois))
+    return list(rois.unbind(0)), fm_rois, roi_cls, num_rois

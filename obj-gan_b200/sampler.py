@@ -9,6 +9,12 @@ With a text encoder (``RNN_ENCODER``) and the GloVe table (ref: evaluator.py:90-
 ``captions``, ``cap_lens`` and ``glove_captions`` instead of ``words_embs`` is encoded on the device inside the same
 graph: token ids -> text encoder + GloVe lookups + padding mask -> (shape generator) -> G_NET.
 
+With a box generator (``BoxGenerator``: PreEncoderRNN + DecoderRNN, ref: box_generation/sample.py, Evaluator.evaluate
+and load_gen_insanns), a caption batch that brings no ``rois`` gets its layout on the device first: box captions ->
+encoder state -> og_box_decode -> og_box_layout.  The roi count decides the shape of the image graph (Rmax, below), so
+the box stage is a CUDA graph of its own, keyed by (B, box caption length); one device -> host read of ``num_rois``
+follows it, and then the text + generated-shape graph runs.
+
 ``GSampler`` holds its own G_NET in eval mode, so BatchNorm normalises with the running statistics and never updates
 them.  A forward pass is ~200 library calls, which cost far more host time than the kernels take at small batch, so
 every input shape is captured once into a CUDA graph and replayed after that:
@@ -34,6 +40,8 @@ from . import model, ops
 from .config import cfg
 from .synth import IMG_SIZES
 from .trainer import prepare_data
+
+NOISE_BOX = ops.BOX_NOISE
 
 # what G_NET.forward reads, in its argument order (ref: model.py:747)
 G_ARGS = ("z", "sent_emb", "words_embs", "glove_words_embs", "slabels_feat", "mask", "hmaps", "rois", "fm_rois",
@@ -75,9 +83,10 @@ class GSampler:
     """Eval-mode G_NET forward with the reference's inputs and 6-tuple output, CUDA-graph replayed per input shape."""
 
     def __init__(self, netG: model.G_NET, netShpG: model.SHP_G_NET | None = None,
-                 text_encoder: model.RNN_ENCODER | None = None, glove=None, clabels_emb=None):
+                 text_encoder: model.RNN_ENCODER | None = None, glove=None, clabels_emb=None, box_generator=None):
         """``glove``: the GloVe table (V, 50) as a tensor or an nn.Embedding (the reference's ``glove_emb``);
-        ``clabels_emb``: (num_classes, 50) label embeddings (see ops.class_label_emb) used when a batch has none."""
+        ``clabels_emb``: (num_classes, 50) label embeddings (see ops.class_label_emb) used when a batch has none;
+        ``box_generator``: a boxgen.BoxGenerator that makes the layout of caption batches without ``rois``."""
         self.netG = netG.eval()
         self.netShpG = netShpG.eval() if netShpG is not None else None
         self.text_encoder = text_encoder.eval() if text_encoder is not None else None
@@ -88,19 +97,24 @@ class GSampler:
         glove = getattr(glove, "weight", glove)
         self.glove = glove.detach().to(self.device).float().contiguous() if glove is not None else None
         self.clabels_emb = clabels_emb.detach().to(self.device).float().contiguous() if clabels_emb is not None else None
+        self.box_generator = box_generator.to(self.device) if box_generator is not None else None
         self._graphs = {}
+        self._box_graphs = {}
         self._pool = None
 
     @classmethod
     def from_snapshot(cls, path: str, num_classes: int = 80, device="cuda", shape_snapshot: str | None = None,
                       text_snapshot: str | None = None, glove=None, cat_labels=None, cat_label_lens=None,
-                      cat_label_order=None) -> "GSampler":
+                      cat_label_order=None, box_checkpoint: str | None = None, mean_std=None, gaussian_dict=None,
+                      cat_ids=None) -> "GSampler":
         """A reference-format generator snapshot (``netG_epoch_N.pth``, what StepBTrainer.save_model writes), and
         optionally a shape generator snapshot (the reference's ``cfg.TEST.NET_SHP_G``) and a text encoder snapshot
         (``cfg.TRAIN.NET_E``; ntoken is read from its ``encoder.weight``); keys with or without the ``module.`` prefix
         that nn.DataParallel adds.  ``glove``: the GloVe table; ``cat_labels`` / ``cat_label_lens`` /
         ``cat_label_order``: the length-sorted class labels, their lengths and the resort indices of the reference's
-        load_cat_label (load.py:305-355), from which the label embeddings are computed once (prepare_cat_emb)."""
+        load_cat_label (load.py:305-355), from which the label embeddings are computed once (prepare_cat_emb).
+        ``box_checkpoint``: the reference's box checkpoint directory, read with ``mean_std``, ``gaussian_dict`` and
+        ``cat_ids`` by BoxGenerator.from_reference (its encoder is the text snapshot's network)."""
         shp = _new_shp_g(num_classes, device) if shape_snapshot is not None else None
         enc = None
         if text_snapshot is not None:
@@ -113,7 +127,14 @@ class GSampler:
             gw = getattr(glove, "weight", glove).detach().to(device).float()
             clabels = ops.class_label_emb(gw, cat_labels.to(device), cat_label_lens.to(device),
                                           cat_label_order.to(device))
-        s = cls(_new_g(num_classes, device), shp, enc, glove, clabels)
+        box = None
+        if box_checkpoint is not None:
+            if text_snapshot is None:
+                raise ValueError("box_checkpoint needs the text encoder snapshot (text_snapshot=...)")
+            from .boxgen import BoxGenerator
+            box = BoxGenerator.from_reference(box_checkpoint, text_snapshot, mean_std, gaussian_dict, cat_ids,
+                                              device=device)
+        s = cls(_new_g(num_classes, device), shp, enc, glove, clabels, box)
         s.load_state_dict(torch.load(path, map_location="cpu"))
         if shape_snapshot is not None:
             s.load_shape_state_dict(torch.load(shape_snapshot, map_location="cpu"))
@@ -131,6 +152,7 @@ class GSampler:
     def load_state_dict(self, state_dict: dict) -> None:
         """Loads G weights (strict) and drops every captured graph."""
         self._graphs.clear()
+        self._box_graphs.clear()
         self.netG.load_state_dict({k: v.to(self.device) for k, v in state_dict.items()}, strict=True)
 
     def load_shape_state_dict(self, state_dict: dict) -> None:
@@ -150,12 +172,22 @@ class GSampler:
         self.text_encoder.load_state_dict(strip_module_prefix(state_dict), strict=True)
 
     # ------------------------------------------------------------------ inputs
-    def _prepare(self, inp: dict) -> dict:
+    def _prepare(self, inp: dict, eager: bool = False) -> dict:
         """Device copies of the inputs G_NET reads (+ the derived tensors of a compact batch), with z and the CA_NET
-        noise drawn here, outside any graph, when the batch does not bring them."""
+        noise drawn here, outside any graph, when the batch does not bring them.  The box stage of a caption batch
+        without ``rois`` runs here too: replayed from its graph, or without graphs when ``eager``."""
         dev = {}
         for k, v in inp.items():
             dev[k] = _map(v, lambda t: t.to(self.device, non_blocking=True))
+        if dev.get("rois") is None and dev.get("captions") is not None:
+            lay = self._layout(dev, eager)
+            n_host = lay.pop("num_rois_host")
+            empty = (n_host == 0).nonzero().view(-1).tolist()
+            if len(empty) == len(n_host):
+                raise ValueError(f"the box generator made no box for any sample (samples {empty}); sample_layout "
+                                 "returns the layouts")
+            dev.update(rois=lay["rois"], fm_rois=lay["fm_rois"], roi_cls=lay["roi_cls"], num_rois=lay["num_rois"],
+                       glb_max_num_roi=int(n_host.max()))
         text = self._text_mode(dev)
         if dev.get("clabels_emb") is None and self.clabels_emb is not None:
             dev["clabels_emb"] = self.clabels_emb
@@ -205,6 +237,88 @@ class GSampler:
         dev["max_len"] = int(hi_l)
         dev["captions"], dev["glove_captions"] = caps.contiguous(), gcaps.contiguous()
         return True
+
+    def _layout(self, dev: dict, eager: bool = False) -> dict:
+        """The box stage of a caption batch without ``rois``: checks its inputs (one device -> host read), draws
+        ``noise_box`` / ``noise_cnt`` unless the batch brings them, runs the box graph of (B, box caption length) (or,
+        with ``eager``, the same library calls without a graph) and reads ``num_rois`` to the host (the second and last
+        read)."""
+        box = self.box_generator
+        if box is None:
+            raise ValueError("the batch has captions but no rois, and this sampler has no box generator: build it with "
+                             "GSampler(..., box_generator=...) or GSampler.from_snapshot(..., box_checkpoint=...)")
+        if self.netShpG is None and dev.get("bt_masks") is None:
+            raise ValueError("a batch whose boxes are generated needs a shape generator: build it with "
+                             "GSampler(netG, netShpG, ...) or GSampler.from_snapshot(..., shape_snapshot=...)")
+        if ("box_captions" in dev) != ("box_cap_lens" in dev):
+            raise ValueError("box_captions and box_cap_lens come together: give both or neither")
+        caps = dev.get("box_captions", dev["captions"])
+        lens = dev.get("box_cap_lens", dev.get("cap_lens"))
+        b = caps.shape[0]
+        if caps.dim() != 2 or lens is None or lens.shape != (b,) or caps.dtype != torch.int64 or \
+                lens.dtype != torch.int64:
+            raise ValueError("box captions (B, T) and their lengths (B,) must be int64 and agree on B")
+        lo_c, hi_c, lo_l, hi_l = torch.stack([caps.min(), caps.max(), lens.min(), lens.max()]).tolist()
+        if lo_l < 1 or hi_l > caps.shape[1]:
+            raise ValueError(f"box caption lengths must lie in [1, {caps.shape[1]}] (the caption width), got "
+                             f"[{lo_l}, {hi_l}]")
+        if lo_c < 0 or hi_c >= box.encoder.ntoken:
+            raise ValueError(f"box caption token ids must lie in [0, {box.encoder.ntoken}), got [{lo_c}, {hi_c}]")
+        nb, nc = dev.get("noise_box"), dev.get("noise_cnt")
+        if nb is None or nc is None:
+            d_nb, d_nc = box.draw_noise(b)
+            nb, nc = (d_nb if nb is None else nb), (d_nc if nc is None else nc)
+        if nb.shape != (b, box.early_stop_len, NOISE_BOX) or nc.shape != (b, box.num_classes):
+            raise ValueError(f"noise_box must be ({b}, {box.early_stop_len}, {NOISE_BOX}) and noise_cnt "
+                             f"({b}, {box.num_classes})")
+        # the graph's static captions have the key's width, max(lengths), whatever width the batch brings
+        ins = dict(captions=caps[:, :int(hi_l)].contiguous(), cap_lens=lens, noise_box=nb.float().contiguous(),
+                   noise_cnt=nc.float().contiguous())
+        key = (b, int(hi_l))
+        entry = self._box_graphs.get(key)
+        if eager:
+            out = box.sample(ins["captions"], ins["cap_lens"], key[1], ins["noise_box"], ins["noise_cnt"])
+        elif entry is None:
+            out = box.sample(ins["captions"], ins["cap_lens"], key[1], ins["noise_box"], ins["noise_cnt"])
+            self._box_graphs[key] = self._capture_box(ins, key[1])
+        else:
+            for k, v in entry.static_in.items():
+                v.copy_(ins[k], non_blocking=True)
+            entry.graph.replay()
+            _lib.get().launches += entry.launches
+            out = {k: _map(v, lambda t: t.clone()) for k, v in entry.static_out.items()}
+        out["num_rois_host"] = out["num_rois"].cpu()
+        return out
+
+    def _capture_box(self, ins: dict, max_len: int) -> _Graph:
+        static_in = {k: v.clone() for k, v in ins.items()}
+        if self._pool is None:
+            self._pool = torch.cuda.graph_pool_handle()
+        graph = torch.cuda.CUDAGraph()
+        n0 = _lib.get().launches
+        box = self.box_generator
+        with torch.cuda.graph(graph, pool=self._pool):
+            static_out = box.sample(static_in["captions"], static_in["cap_lens"], max_len, static_in["noise_box"],
+                                    static_in["noise_cnt"])
+        launches = _lib.get().launches - n0
+        _lib.get().launches = n0
+        keep = [c for n in (box.encoder,) for c in _packed_copies(n)] + [box.decoder.packed_weights()]
+        return _Graph(graph, static_in, static_out, launches, keep)
+
+    def sample_layout(self, inp: dict) -> dict:
+        """The box stage of a caption batch (graph-replayed like ``sample``): ``rois`` (3 scales, (B, BOXES_NUM, 6)
+        float64), ``fm_rois``, ``num_rois``, ``roi_cls`` -- the layout tensors a box batch brings -- and the raw
+        trajectory ``labels`` (B, S), ``samples`` (B, S, 4) and ``steps`` (B,).  ``box_captions`` with ``box_cap_lens``
+        are read when present (the untruncated captions; both or neither), else ``captions`` / ``cap_lens``; ``noise_box`` /
+        ``noise_cnt`` are taken from the batch when present."""
+        with torch.no_grad():
+            dev = {k: _map(v, lambda t: t.to(self.device, non_blocking=True)) for k, v in inp.items()
+                   if k in ("captions", "cap_lens", "box_captions", "box_cap_lens", "noise_box", "noise_cnt")}
+            if dev.get("captions") is None:
+                raise ValueError("sample_layout needs captions")
+            out = self._layout(dev)
+            out.pop("num_rois_host")
+            return out
 
     def _generates(self, dev: dict) -> bool:
         """Whether the batch's masks come from the shape generator (the batch brings no ``bt_masks``)."""
@@ -264,7 +378,7 @@ class GSampler:
     def sample_eager(self, inp: dict):
         """The same forward pass without graphs."""
         with torch.no_grad():
-            return self._forward(self._prepare(inp))
+            return self._forward(self._prepare(inp, eager=True))
 
     def sample_shapes(self, inp: dict) -> dict:
         """The generated shapes of a batch without masks (eager): ``raw_masks`` (B, R, 64, 64), the SHP_G_NET output the
@@ -272,7 +386,8 @@ class GSampler:
         ``hmaps`` (3 scales), ``bt_masks`` (3 scales) and ``fm_bt_masks``, the per-roi ones zero-padded to BOXES_NUM
         slots.  ``noise_shp`` (B, BOXES_NUM, 4 * num_classes) is taken from the batch when present."""
         with torch.no_grad():
-            dev = self._prepare({k: v for k, v in inp.items() if k not in ("bt_masks", "fm_bt_masks", "hmaps")})
+            dev = self._prepare({k: v for k, v in inp.items() if k not in ("bt_masks", "fm_bt_masks", "hmaps")},
+                                eager=True)
             return self._shapes(dev)
 
     def encode_text(self, inp: dict) -> dict:
