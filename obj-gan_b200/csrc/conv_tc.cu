@@ -17,7 +17,7 @@
 // 2^-18 of the tensor maximum keep all 22 bits, smaller ones an absolute error <= 2^-39 of the maximum.
 // nsplit = 1 runs a single fp16 product (reported separately, never the parity mode).
 //
-// GEMM tiling: one CTA = 128 output pixels (a TN x TH x TW patch) x BN output channels (BN % 16 == 0,
+// GEMM tiling: one CTA = 128 output pixels (a TN x TH x TW patch) x BN output channels (BN % 8 == 0,
 // <= 128); K loop over taps x 64-channel chunks; STAGES-deep smem ring of {A_hi, A_lo, B_hi, B_lo}.
 // Warpgroup roles: warpgroup 0 = TMA producer (one elected thread), warpgroups 1 and 2 = MMA + epilogue, each
 // owning 64 of the 128 tile rows.  The forward kernel issues one wgmma over the whole N extent per product and
@@ -52,7 +52,6 @@ struct TcParams {
   const unsigned* amax_a; // float bits of max|x| of the two operand tensors (power-of-two operand scaling)
   const unsigned* amax_b;
   int K;                  // output channels actually stored (<= gridDim.y * BN)
-  int nsplit;             // 1 or 3
   float* y;
   long long ysn, ysh, ysw;  // output strides (elements) of the FULL-resolution output tensor
   int osy, osx, opy, opx;   // output pixel = (osy * h + opy, osx * w + opx)
@@ -149,8 +148,13 @@ struct TcAccWide {
   }
   __device__ __forceinline__ void hold() { wg_hold(d); }
   __device__ __forceinline__ void mma(uint64_t a, uint64_t b, int scale_d) {
+    static_assert(BN == 32 || BN == 48 || BN == 64 || BN == 96 || BN == 104 || BN == 112 || BN == 128,
+                  "no wgmma wrapper for this tile width");
     if constexpr (BN == 32) wg_mma_n32<0, 0>(d, a, b, scale_d);
+    if constexpr (BN == 48) wg_mma_n48<0, 0>(d, a, b, scale_d);
     if constexpr (BN == 64) wg_mma_n64<0, 0>(d, a, b, scale_d);
+    if constexpr (BN == 96) wg_mma_n96<0, 0>(d, a, b, scale_d);
+    if constexpr (BN == 104) wg_mma_n104<0, 0>(d, a, b, scale_d);
     if constexpr (BN == 112) wg_mma_n112<0, 0>(d, a, b, scale_d);
     if constexpr (BN == 128) wg_mma_n128<0, 0>(d, a, b, scale_d);
   }
@@ -175,24 +179,59 @@ struct TcAccWide {
   }
 };
 
+// One stage's MMAs into a fresh partial sum: KS k-steps of 16, KSTEP bytes apart in the operand tiles, as ONE
+// straight-line issue window (fence, the MMAs, commit), then the wait for them.  Nothing in the window branches or
+// touches the accumulator registers; otherwise ptxas waits for every wgmma before issuing the next (C7520 / C7519 /
+// C7514 warnings).  The wait sits in here too, so that a caller choosing KS at run time (a switch) merges the
+// accumulators only after it (C7517 otherwise).
+// NSPLIT = 3: al*bh, ah*bl, ah*bh (small terms first); 1: ah*bh.  STACKED: al*[bh_hi | bh_lo], ah*[bh_hi | bh_lo].
+template <int KS, uint32_t KSTEP, int NSPLIT, bool STACKED, class Acc>
+__device__ __forceinline__ void tc_stage_mma(Acc& part, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl) {
+  wg_fence();
+#pragma unroll
+  for (int k = 0; k < KS; ++k) {
+    const uint64_t koff = (uint64_t)((k * KSTEP) >> 4);
+    if constexpr (STACKED) {
+      part.mma(al + koff, bh + koff, k > 0);
+      part.mma(ah + koff, bh + koff, 1);
+    } else if constexpr (NSPLIT == 3) {
+      part.mma(al + koff, bh + koff, k > 0);
+      part.mma(ah + koff, bl + koff, 1);
+      part.mma(ah + koff, bh + koff, 1);
+    } else {
+      part.mma(ah + koff, bh + koff, k > 0);
+    }
+  }
+  wg_commit();
+  wg_wait<0>();
+  part.hold();
+}
+
+// Warp index as a value ptxas knows to be warp-uniform (threadIdx.x >> 5 is, but the compiler cannot prove it, and
+// a role branch it takes for divergent serializes every wgmma behind it)
+__device__ __forceinline__ int tc_warp_uniform() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
+
 // ------------------------------------------------------------------------------------------------
 // STACKED (3xFP16 only, <= 32 output channels): B is [w_hi | w_lo] of the same BN / 2 output channels stacked along
 // N, so a k-step is two MMAs, a_lo [w_hi | w_lo] and a_hi [w_hi | w_lo], and the epilogue adds the two column halves
 // (the extra a_lo w_lo term is below the rounding of the others).  Each A copy is read from shared memory once per
 // k-step instead of 1.5 times -- narrow layers are bound by those reads, not by the MMA rate.
-template <int BN, int STAGES, bool STACKED>
+// NSPLIT: products per k-step (3 = 3xFP16, 1 = one fp16 product), a template parameter so that the issue window
+// holds no branch.
+template <int BN, int STAGES, bool STACKED, int NSPLIT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant__ CUtensorMap map_al,
                const __grid_constant__ CUtensorMap map_bh, const __grid_constant__ CUtensorMap map_bl,
                const TcParams p) {
+  static_assert(BN % 8 == 0 && BN <= 128 && (NSPLIT == 1 || NSPLIT == 3) && (!STACKED || NSPLIT == 3), "");
   constexpr uint32_t A_BYTES = TC_BM * 128;         // 128 rows of 128 bytes = 16 KB
-  constexpr uint32_t B_BYTES = BN * 128;
+  constexpr uint32_t B_BYTES = BN * 128;            // BN % 8 == 0: a whole number of 1024-byte swizzle atoms
   constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + (STACKED ? 1 : 2) * B_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = tc_warp_uniform(), lane = threadIdx.x & 31;
   // tile coordinates
   int t = blockIdx.x;
   const int tw_i = t % p.tiles_w;
@@ -205,13 +244,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
   const int per_split = (nk_total + p.ksplit - 1) / p.ksplit;
   const int it_beg = blockIdx.z * per_split;
   const int nk = min(nk_total, it_beg + per_split) - it_beg;
-  const uint32_t tx_bytes = (p.nsplit == 3) ? STAGE_BYTES : (A_BYTES + B_BYTES);
+  constexpr uint32_t tx_bytes = (NSPLIT == 3) ? STAGE_BYTES : (A_BYTES + B_BYTES);
   if (nk <= 0) return;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&map_ah);
     prefetch_tmap(&map_bh);
-    if (p.nsplit == 3) {
+    if (NSPLIT == 3) {
       prefetch_tmap(&map_al);
       prefetch_tmap(&map_bl);
     }
@@ -237,7 +276,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
         const int ns = n0 + p.taps.dn[tap];   // image offset: selects a space-to-depth phase block of the source
         tma_load_4d(sa, &map_ah, &full_bar[stage], c0, ws, hs, ns);
         tma_load_3d(sa + 2 * A_BYTES, &map_bh, &full_bar[stage], c0, col0, widx);
-        if (p.nsplit == 3) {
+        if (NSPLIT == 3) {
           tma_load_4d(sa + A_BYTES, &map_al, &full_bar[stage], c0, ws, hs, ns);
           // stacked: the lo rows follow the hi rows inside the same N extent (maps with a box of BN / 2 rows)
           tma_load_3d(sa + 2 * A_BYTES + (STACKED ? B_BYTES / 2 : B_BYTES), &map_bl, &full_bar[stage], c0, col0, widx);
@@ -266,27 +305,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
       const uint32_t sa = smem_u32(smem + (size_t)stage * STAGE_BYTES);
       const uint64_t ah = wg_desc_k(sa + cg * 64 * 128), al = wg_desc_k(sa + A_BYTES + cg * 64 * 128);
       const uint64_t bh = wg_desc_k(sa + 2 * A_BYTES), bl = wg_desc_k(sa + 2 * A_BYTES + B_BYTES);
-      // the last channel chunk may hold fewer than 64 real channels: skip the k-steps that would multiply zeros
+      // the last channel chunk may hold fewer than 64 real channels: skip the k-steps that would multiply zeros.
+      // A k-step advances 32 bytes (16 fp16) inside the swizzle row; stacked, bh addresses [w_hi | w_lo].
       const int ks = ((it_beg + it + 1) % p.cchunks == 0) ? p.klast : 4;
-      wg_fence();
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        if (k >= ks) break;
-        const uint64_t koff = (uint64_t)((k * 32) >> 4);      // advance 32 bytes (16 fp16) inside the swizzle row
-        if (STACKED) {
-          part.mma(al + koff, bh + koff, k > 0);   // bh addresses [w_hi | w_lo]
-          part.mma(ah + koff, bh + koff, 1);
-        } else if (p.nsplit == 3) {
-          part.mma(al + koff, bh + koff, k > 0);   // small terms first
-          part.mma(ah + koff, bl + koff, 1);
-          part.mma(ah + koff, bh + koff, 1);
-        } else {
-          part.mma(ah + koff, bh + koff, k > 0);
-        }
+      switch (ks) {
+        case 1: tc_stage_mma<1, 32, NSPLIT, STACKED>(part, ah, al, bh, bl); break;
+        case 2: tc_stage_mma<2, 32, NSPLIT, STACKED>(part, ah, al, bh, bl); break;
+        case 3: tc_stage_mma<3, 32, NSPLIT, STACKED>(part, ah, al, bh, bl); break;
+        default: tc_stage_mma<4, 32, NSPLIT, STACKED>(part, ah, al, bh, bl); break;
       }
-      wg_commit();
-      wg_wait<0>();
-      part.hold();
       if (lane == 0) mbar_arrive(&empty_bar[stage]);   // this stage's MMAs have completed: free its slot
       acc.add(part);
       if (++stage == STAGES) {
@@ -371,7 +398,7 @@ constexpr int tc_stages(size_t stage_bytes) {
   return TC_SMEM_BUDGET / stage_bytes >= 4 ? 4 : (int)(TC_SMEM_BUDGET / stage_bytes);
 }
 
-template <int BN, bool STACKED = false>
+template <int BN, int NSPLIT, bool STACKED = false>
 int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
               const TcParams& p, dim3 grid, cudaStream_t stream) {
   constexpr size_t stage = 2 * TC_BM * 128 + (STACKED ? 1 : 2) * BN * 128;
@@ -379,13 +406,37 @@ int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
   constexpr size_t smem = (size_t)STAGES * stage + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES, STACKED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES, STACKED, NSPLIT>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     configured = true;
   }
-  conv_tc_kernel<BN, STAGES, STACKED><<<grid, TC_THREADS, smem, stream>>>(ah, al, bh, bl, p);
+  conv_tc_kernel<BN, STAGES, STACKED, NSPLIT><<<grid, TC_THREADS, smem, stream>>>(ah, al, bh, bl, p);
   return (int)cudaGetLastError();
+}
+
+// N tile widths with an instantiated kernel: the layers of the hot path (K = 400 -> 4 x 104, 200 -> 2 x 104,
+// 96, 48, ...) each run within 8 columns of their real width
+constexpr int TC_BN_SET[] = {32, 48, 64, 96, 104, 112, 128};
+
+template <int NSPLIT>
+int launch_tc_bn(int bn, bool stacked, int stk_rows, const CUtensorMap& ah, const CUtensorMap& al,
+                 const CUtensorMap& bh, const CUtensorMap& bl, const TcParams& p, dim3 grid, cudaStream_t stream) {
+  if constexpr (NSPLIT == 3) {
+    if (stacked)
+      return stk_rows == 16 ? launch_tc<32, 3, true>(ah, al, bh, bl, p, grid, stream)
+                            : launch_tc<64, 3, true>(ah, al, bh, bl, p, grid, stream);
+  }
+  switch (bn) {
+    case 32:  return launch_tc<32, NSPLIT>(ah, al, bh, bl, p, grid, stream);
+    case 48:  return launch_tc<48, NSPLIT>(ah, al, bh, bl, p, grid, stream);
+    case 64:  return launch_tc<64, NSPLIT>(ah, al, bh, bl, p, grid, stream);
+    case 96:  return launch_tc<96, NSPLIT>(ah, al, bh, bl, p, grid, stream);
+    case 104: return launch_tc<104, NSPLIT>(ah, al, bh, bl, p, grid, stream);
+    case 112: return launch_tc<112, NSPLIT>(ah, al, bh, bl, p, grid, stream);
+    case 128: return launch_tc<128, NSPLIT>(ah, al, bh, bl, p, grid, stream);
+    default:  return (int)cudaErrorInvalidValue;
+  }
 }
 
 
@@ -409,7 +460,6 @@ struct TcWgradParams {
   int chunks_per_cta;
   int Kp, C;            // rows (co) and columns (ci) of each dW[t]
   int cotiles;          // blockIdx.x = citile * cotiles + cotile
-  int nsplit;
   float* dw;            // [ntaps_out][Kp][C]; or, when work is set, work[(z * nentries + e) * Kp * C] per (split, entry)
   float* work;
   const unsigned* amax_g; // operand scales (see TcParams)
@@ -425,7 +475,7 @@ static_assert(WG_SLAB == TC_NBLK_BYTES, "a 64-wide column block of the MN-major 
 
 __device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr) { return wg_desc(saddr, WG_SLAB, 1024); }
 
-template <int BNW, int STAGES>
+template <int BNW, int STAGES, int NSPLIT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap map_gh, const __grid_constant__ CUtensorMap map_gl,
                      const __grid_constant__ CUtensorMap map_xh, const __grid_constant__ CUtensorMap map_xl,
@@ -438,12 +488,12 @@ conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap map_gh, const __grid_co
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = tc_warp_uniform(), lane = threadIdx.x & 31;
   const int cotile = blockIdx.x % p.cotiles, citile = blockIdx.x / p.cotiles, tap = blockIdx.y;
   const int ch_beg = blockIdx.z * p.chunks_per_cta;
   const int ch_end = min(p.total_chunks, ch_beg + p.chunks_per_cta);
   const int nk = ch_end - ch_beg;
-  const uint32_t tx_bytes = (p.nsplit == 3) ? STAGE_BYTES : (A_BYTES + B_BYTES);
+  constexpr uint32_t tx_bytes = (NSPLIT == 3) ? STAGE_BYTES : (A_BYTES + B_BYTES);
   if (nk <= 0) return;
 
   if (threadIdx.x == 0) {
@@ -474,7 +524,7 @@ conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap map_gh, const __grid_co
         mbar_expect_tx(&full_bar[stage], tx_bytes);
         tma_load_5d(sa, &map_gh, &full_bar[stage], 0, w0, h, n + gdn, aslab);
         tma_load_5d(sa + 2 * A_BYTES, &map_xh, &full_bar[stage], 0, w0 + xdw, h + xdh, n + xdn, bslab);
-        if (p.nsplit == 3) {
+        if (NSPLIT == 3) {
           tma_load_5d(sa + A_BYTES, &map_gl, &full_bar[stage], 0, w0, h, n + gdn, aslab);
           tma_load_5d(sa + 2 * A_BYTES + B_BYTES, &map_xl, &full_bar[stage], 0, w0 + xdw, h + xdh, n + xdn, bslab);
         }
@@ -498,21 +548,7 @@ conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap map_gh, const __grid_co
       const uint32_t sa = smem_u32(smem + (size_t)stage * STAGE_BYTES);
       const uint64_t ah = make_desc_mn(sa + cg * WG_SLAB), al = make_desc_mn(sa + A_BYTES + cg * WG_SLAB);
       const uint64_t bh = make_desc_mn(sa + 2 * A_BYTES), bl = make_desc_mn(sa + 2 * A_BYTES + B_BYTES);
-      wg_fence();
-#pragma unroll
-      for (int k = 0; k < WG_PIX / 16; ++k) {
-        const uint64_t koff = (uint64_t)((k * 16 * 128) >> 4);    // 16 pixel rows of 128 bytes
-        if (p.nsplit == 3) {
-          part.mma(al + koff, bh + koff, k > 0);
-          part.mma(ah + koff, bl + koff, 1);
-          part.mma(ah + koff, bh + koff, 1);
-        } else {
-          part.mma(ah + koff, bh + koff, k > 0);
-        }
-      }
-      wg_commit();
-      wg_wait<0>();
-      part.hold();
+      tc_stage_mma<WG_PIX / 16, 16 * 128, NSPLIT, false>(part, ah, al, bh, bl);   // a k-step = 16 pixel rows
       if (lane == 0) mbar_arrive(&empty_bar[stage]);
       acc.add(part);
       if (++stage == STAGES) {
@@ -552,7 +588,7 @@ __global__ void __launch_bounds__(256) wgrad_sum_kernel(const float* __restrict_
   }
 }
 
-template <int BNW>
+template <int BNW, int NSPLIT>
 int launch_wgrad(const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap& xh, const CUtensorMap& xl,
                  const TcWgradParams& p, dim3 grid, cudaStream_t stream) {
   constexpr size_t stage = 2 * 2 * WG_SLAB + 2 * ((BNW + WG_CH - 1) / WG_CH) * WG_SLAB;
@@ -560,12 +596,24 @@ int launch_wgrad(const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap
   constexpr size_t smem = (size_t)STAGES * stage + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_wgrad_kernel<BNW, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_wgrad_kernel<BNW, STAGES, NSPLIT>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     configured = true;
   }
-  conv_tc_wgrad_kernel<BNW, STAGES><<<grid, TC_THREADS, smem, stream>>>(gh, gl, xh, xl, p);
+  conv_tc_wgrad_kernel<BNW, STAGES, NSPLIT><<<grid, TC_THREADS, smem, stream>>>(gh, gl, xh, xl, p);
   return (int)cudaGetLastError();
+}
+
+template <int NSPLIT>
+int launch_wgrad_bn(int bn, const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap& xh,
+                    const CUtensorMap& xl, const TcWgradParams& p, dim3 grid, cudaStream_t stream) {
+  switch (bn) {
+    case 32:  return launch_wgrad<32, NSPLIT>(gh, gl, xh, xl, p, grid, stream);
+    case 64:  return launch_wgrad<64, NSPLIT>(gh, gl, xh, xl, p, grid, stream);
+    case 112: return launch_wgrad<112, NSPLIT>(gh, gl, xh, xl, p, grid, stream);
+    default:  return launch_wgrad<128, NSPLIT>(gh, gl, xh, xl, p, grid, stream);
+  }
 }
 
 }  // namespace
@@ -612,7 +660,6 @@ OG_API int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, 
   p.klast = og_cdiv(C - (p.cchunks - 1) * TC_BK, 16);
   p.amax_a = amax_x; p.amax_b = amax_w;
   p.K = K;
-  p.nsplit = nsplit;
   p.y = y; p.ysn = ysn; p.ysh = ysh; p.ysw = ysw;
   p.osy = osy; p.osx = osx; p.opy = opy; p.opx = opx;
   p.OHfull = OHf; p.OWfull = OWf;
@@ -624,12 +671,16 @@ OG_API int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, 
     p.taps.widx[i] = taps_host[4 * i + 3];
   }
   // N tile: whole K if it fits 128 columns (a consumer thread holds two sets of BN / 2 accumulators), else the
-  // smallest number of equal tiles (multiple of 16)
-  const int Kr = (K + 15) / 16 * 16;
-  const int ntile = og_cdiv(Kr, 128);
-  int BN = (og_cdiv(Kr, ntile) + 15) / 16 * 16;
-  int BNsel = BN <= 64 ? 64 : BN <= 112 ? 112 : 128;
-  if (BN <= 32) BNsel = 32;
+  // smallest number of equal tiles; the width is rounded up to the wgmma N step of 8, then to the next instantiated
+  // width.  An output element's k-sum does not depend on the tile width, so neither do the results.
+  const int ntile = og_cdiv(K, 128);
+  const int bn8 = (og_cdiv(K, ntile) + 7) / 8 * 8;
+  int BNsel = 128;
+  for (int b : TC_BN_SET)
+    if (b >= bn8) {
+      BNsel = b;
+      break;
+    }
   dim3 grid(tiles_n * p.tiles_h * p.tiles_w, og_cdiv(K, BNsel), 1);
   // few output tiles (small feature maps): split the reduction over gridDim.z (about two CTAs per SM in all); the
   // slices' partial outputs are summed in a fixed order afterwards (og_split_sum)
@@ -675,14 +726,8 @@ OG_API int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, 
     mbl = mbh;
   }
   if (p.ksplit > 1) OG_CHECK(og_work_alloc(&p.work, (size_t)p.ksplit * p.work_plane, stream));
-  if (stacked) rc = stk_rows == 16 ? launch_tc<32, true>(mah, mal, mbh, mbl, p, grid, stream)
-                                     : launch_tc<64, true>(mah, mal, mbh, mbl, p, grid, stream);
-  else switch (BNsel) {
-    case 32:  rc = launch_tc<32>(mah, mal, mbh, mbl, p, grid, stream); break;
-    case 64:  rc = launch_tc<64>(mah, mal, mbh, mbl, p, grid, stream); break;
-    case 112: rc = launch_tc<112>(mah, mal, mbh, mbl, p, grid, stream); break;
-    default:  rc = launch_tc<128>(mah, mal, mbh, mbl, p, grid, stream); break;
-  }
+  rc = nsplit == 3 ? launch_tc_bn<3>(BNsel, stacked, stk_rows, mah, mal, mbh, mbl, p, grid, stream)
+                   : launch_tc_bn<1>(BNsel, stacked, stk_rows, mah, mal, mbh, mbl, p, grid, stream);
   if (p.ksplit > 1) {
     if (!rc) rc = og_split_sum(p.work, p.work_plane, p.ksplit, y, stream);
     const cudaError_t e = cudaFreeAsync(p.work, stream);
@@ -723,7 +768,7 @@ OG_API int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* am
   p.wchunks = OW / cw;
   p.hchunks = OH / chh;
   p.total_chunks = p.wchunks * p.hchunks * og_cdiv(N, cn);
-  p.Kp = Kp; p.C = C; p.nsplit = nsplit; p.dw = dw;
+  p.Kp = Kp; p.C = C; p.dw = dw;
   p.amax_g = amax_g; p.amax_x = amax_x;
   for (int i = 0; i < nentries; ++i) {
     p.gdn[i] = entries_host[5 * i];
@@ -777,12 +822,8 @@ OG_API int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* am
   p.work = nullptr;
   const long long plane = (long long)Kp * C;
   if (shared_out) OG_CHECK(og_work_alloc(&p.work, (size_t)splits * nentries * plane, stream));
-  switch (BNsel) {
-    case 32:  rc = launch_wgrad<32>(mgh, mgl, mxh, mxl, p, grid, stream); break;
-    case 64:  rc = launch_wgrad<64>(mgh, mgl, mxh, mxl, p, grid, stream); break;
-    case 112: rc = launch_wgrad<112>(mgh, mgl, mxh, mxl, p, grid, stream); break;
-    default:  rc = launch_wgrad<128>(mgh, mgl, mxh, mxl, p, grid, stream); break;
-  }
+  rc = nsplit == 3 ? launch_wgrad_bn<3>(BNsel, mgh, mgl, mxh, mxl, p, grid, stream)
+                   : launch_wgrad_bn<1>(BNsel, mgh, mgl, mxh, mxl, p, grid, stream);
   if (shared_out) {
     if (!rc) {
       WgradSum ws;
