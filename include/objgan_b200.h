@@ -235,7 +235,7 @@ int og_inc_i64(long long* counter, cudaStream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------
  * DAMSM matching losses around func_attention (ref: miscc/losses.py:13-159: cosine_similarity, sent_loss,
- * words_loss).  Dense row-major fp32; B <= 64 captions.
+ * words_loss).  Dense row-major fp32; B <= 128 captions (og_ce_pair: the R-precision pool of 100).
  *  og_cosine_cl_*     : out[b][l] = cos(word[:, l], wei[b, :, l]) over the D features (word [D][L] shared by all
  *                       images, wei [B][D][L]); backward w.r.t. wei (losses.py:101-108)
  *  og_expsumlog_*     : out[b] = log(sum_l exp(gamma * s[b][l]))            (Eq. 10, losses.py:112-115)
@@ -381,6 +381,37 @@ int og_box_layout(const long long* labels, const float* samples, const long long
 
 /* zero-fill (a memset node when captured in a CUDA graph; no kernel launch) */
 int og_zero_bytes(float* p, long long bytes, cudaStream_t stream);
+
+/* ----------------------------------------------------------------------------------------------------
+ * Inception-v3 image encoder (CNN_ENCODER, ref: model.py:182-287; csrc/inception.cu).  NHWC fp32, C % 8 == 0.
+ * og_conv2d_simt_pad2 is og_conv2d_simt with separate row / column padding (1x7, 7x1, 1x3, 3x1 kernels).
+ * Pooling: max_pool2d(3, 2) (output may be a channel slice: pixel stride ldy, offset yoff; the backward reads the
+ * gradient slice the same way), avg_pool2d(3, 1, 1, count_include_pad=True), the global average over P pixels; every
+ * backward is a deterministic gather.  og_bilinear_bwd_gather: adjoint of og_bilinear_fwd without atomics.
+ * og_bn_fold: eval BatchNorm folded into a bias-free conv (wout = w * s, bout = beta - mean * s, s = gamma /
+ * sqrt(var + eps), R = Ci * KH * KW).  og_prep_split_s2d: og_prep_split(s2d=1) for any H, W (phase blocks of
+ * ceil(H/2) x ceil(W/2), zero past an odd edge).  og_relu_grad_slice: out[p, ooff + c] = g[p, goff + c] masked by
+ * y[p, yoff + c] > 0 (relu = 1) or copied (relu = 0), c < nch.
+ * ---------------------------------------------------------------------------------------------------- */
+int og_conv2d_simt_pad2(const float* x, int N, int H, int W, int C, long long xsn, long long xsh, long long xsw,
+                        const float* wpacked, float* y, int OH, int OW, int K, long long ysn, long long ysh,
+                        long long ysw, int KH, int KW, int stride, int padh, int padw, int mode, const float* bias,
+                        int act, float slope, int allow_splitk, cudaStream_t stream);
+int og_maxpool3s2_fwd(const float* x, int N, int H, int W, int C, float* y, int ldy, int yoff, cudaStream_t stream);
+int og_maxpool3s2_bwd(const float* x, const float* g, int ldg, int goff, int N, int H, int W, int C, float* gx,
+                      cudaStream_t stream);
+int og_avgpool3s1_fwd(const float* x, int N, int H, int W, int C, float* y, cudaStream_t stream);
+int og_avgpool3s1_bwd(const float* g, int N, int H, int W, int C, float* gx, cudaStream_t stream);
+int og_global_avg_fwd(const float* x, int N, int P, int C, float* y, cudaStream_t stream);
+int og_global_avg_bwd(const float* g, int N, int P, int C, float* gx, cudaStream_t stream);
+int og_bilinear_bwd_gather(const float* g, int N, int IH, int IW, int C, int OH, int OW, float* gx,
+                           cudaStream_t stream);
+int og_bn_fold(const float* w, int Co, long long R, const float* gamma, const float* beta, const float* mean,
+               const float* var, float eps, float* wout, float* bout, cudaStream_t stream);
+int og_prep_split_s2d(const float* x, int N, int H, int W, int C, unsigned* amax, int amax_ready, void* xh, void* xl,
+                      cudaStream_t stream);
+int og_relu_grad_slice(const float* y, int ldy, int yoff, const float* g, int ldg, int goff, float* out, int ldo,
+                       int ooff, int nch, long long P, int relu, cudaStream_t stream);
 
 #ifdef __cplusplus
 }

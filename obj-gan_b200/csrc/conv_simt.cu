@@ -28,6 +28,7 @@ struct ConvArgs {
   float slope;
   float* work;       // split-K: slice z writes its partial result to work + z * work_plane (y's layout)
   long long work_plane;
+  int padw;          // column padding (pad is the row padding)
 };
 
 __device__ __forceinline__ int src_coord(int mode, int o, int k, int stride, int pad, int Hs) {
@@ -139,7 +140,7 @@ __global__ void __launch_bounds__(256) conv_gemm_kernel(ConvArgs a) {
     if (!am_ok) return;
     int kh = t / a.KW, kw = t - kh * a.KW;
     int ih = src_coord(a.mode, aoh, kh, a.stride, a.pad, a.H);
-    int iw = src_coord(a.mode, aow, kw, a.stride, a.pad, a.W);
+    int iw = src_coord(a.mode, aow, kw, a.stride, a.padw, a.W);
     if (ih < 0 || iw < 0) return;
     aptr = a.x + an * a.xsn + ih * a.xsh + iw * a.xsw + ah * 4;
   };
@@ -599,12 +600,13 @@ static int pick_splits(long long tiles, int nk, int want_ctas) {
   return s < 1 ? 1 : s;
 }
 
-OG_API int og_conv2d_simt(const float* x, int N, int H, int W, int C, long long xsn, long long xsh, long long xsw,
-                          const float* wpacked, float* y, int OH, int OW, int K, long long ysn, long long ysh,
-                          long long ysw, int KH, int KW, int stride, int pad, int mode, const float* bias, int act,
-                          float slope, int allow_splitk, cudaStream_t stream) {
+static int conv2d_simt(const float* x, int N, int H, int W, int C, long long xsn, long long xsh, long long xsw,
+                       const float* wpacked, float* y, int OH, int OW, int K, long long ysn, long long ysh,
+                       long long ysw, int KH, int KW, int stride, int pad, int padw, int mode, const float* bias,
+                       int act, float slope, int allow_splitk, cudaStream_t stream) {
   if (C % 8 || K % 4) return (int)cudaErrorInvalidValue;
   ConvArgs a{x, N, H, W, C, xsn, xsh, xsw, wpacked, y, OH, OW, K, ysn, ysh, ysw, KH, KW, stride, pad, mode, bias, act, slope};
+  a.padw = padw;
   long long M = (long long)N * OH * OW;
   if (M == 0) return 0;
   int TN = K > 64 ? 8 : (K > 32 ? 4 : 2);
@@ -636,6 +638,23 @@ OG_API int og_conv2d_simt(const float* x, int N, int H, int W, int C, long long 
     if (!rc) rc = (int)e;
   }
   return rc;
+}
+
+OG_API int og_conv2d_simt(const float* x, int N, int H, int W, int C, long long xsn, long long xsh, long long xsw,
+                          const float* wpacked, float* y, int OH, int OW, int K, long long ysn, long long ysh,
+                          long long ysw, int KH, int KW, int stride, int pad, int mode, const float* bias, int act,
+                          float slope, int allow_splitk, cudaStream_t stream) {
+  return conv2d_simt(x, N, H, W, C, xsn, xsh, xsw, wpacked, y, OH, OW, K, ysn, ysh, ysw, KH, KW, stride, pad, pad, mode,
+                     bias, act, slope, allow_splitk, stream);
+}
+
+// og_conv2d_simt with separate row / column padding (the 1x7 / 7x1 / 1x3 / 3x1 convolutions of Inception-v3)
+OG_API int og_conv2d_simt_pad2(const float* x, int N, int H, int W, int C, long long xsn, long long xsh, long long xsw,
+                               const float* wpacked, float* y, int OH, int OW, int K, long long ysn, long long ysh,
+                               long long ysw, int KH, int KW, int stride, int padh, int padw, int mode,
+                               const float* bias, int act, float slope, int allow_splitk, cudaStream_t stream) {
+  return conv2d_simt(x, N, H, W, C, xsn, xsh, xsw, wpacked, y, OH, OW, K, ysn, ysh, ysw, KH, KW, stride, padh, padw,
+                     mode, bias, act, slope, allow_splitk, stream);
 }
 
 OG_API int og_conv2d_wgrad_simt(const float* x, int N, int H, int W, int C, long long xsn, long long xsh,

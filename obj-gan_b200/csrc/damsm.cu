@@ -5,7 +5,8 @@
 #include "common.cuh"
 
 namespace {
-constexpr int DM_MAXB = 64;
+// largest B of og_ce_pair (one thread per row / column): the evaluator's R-precision pool is 100 (RP_POOL_SIZE)
+constexpr int DM_MAXB = 128;
 
 // ---- cosine_similarity(word, weiContext) over the feature axis (losses.py:13-19, 101-108) ----------------------
 // word [D][L] (one caption, shared by all images), wei [B][D][L]  ->  out[b][l]

@@ -322,3 +322,78 @@ def G_loss(netsPatD, netsShpD, netObjSSD, netObjLSD, image_encoder, fake_imgs, s
         add(ls)
         logs["objls_g_loss"] = ls.detach()
     return total, logs
+
+
+class RPrecision:
+    """R-precision of generated images (ref: evaluator.py:370-411, cfg.TEST.RP_POOL_SIZE = 100), restated with the
+    reference's pooling:
+
+      * batches of (region_features, cnn_code, words_embs, sent_emb, cap_lens) are appended until the pooled count
+        reaches ``pool_size``;
+      * the batch that arrives when the pool is full scores the pool and is itself NOT added (the reference drops it;
+        reproduced on purpose, so that the numbers compare);
+      * the pool's sets are cut to ``pool_size`` and its words_embs zero-padded to the longest of its captions;
+      * words_loss / sent_loss run with labels 0..pool_size-1 and the pool's class ids, like the reference: its losses
+        mask same-class pairs whatever ``is_training`` is (miscc/losses.py:27-54, 88-140); on COCO the class ids are
+        distinct (load.py:429-435), so the mask is empty there;
+      * ``result()`` gives (mean, std) of the word and of the sentence accuracy (percent) over the scored pools."""
+
+    def __init__(self, pool_size=100):
+        self.pool_size = pool_size
+        self.w_accuracy, self.s_accuracy = [], []
+        self._reset()
+
+    def _reset(self):
+        self.count = 0
+        self.sets = {"region_features": [], "cnn_code": [], "words_embs": [], "sent_emb": [], "cap_lens": []}
+        self.class_ids = []
+
+    def add(self, region_features, cnn_code, words_embs, sent_emb, cap_lens, class_ids=None):
+        """One batch; ``class_ids``: its class ids (a host sequence; None: every sample its own class)."""
+        if self.count >= self.pool_size:
+            self._score()
+            self._reset()
+            return
+        dev = cnn_code.device
+        lens = cap_lens.to(dev, torch.int64) if torch.is_tensor(cap_lens) else ops.h2d([int(v) for v in cap_lens], dev,
+                                                                                      torch.int64)
+        for k, v in (("region_features", region_features), ("cnn_code", cnn_code), ("words_embs", words_embs),
+                     ("sent_emb", sent_emb), ("cap_lens", lens)):
+            self.sets[k].append(v.detach())
+        import numpy as np
+        b = cnn_code.shape[0]
+        self.class_ids.append(np.asarray(class_ids).reshape(-1) if class_ids is not None
+                              else -1 - np.arange(self.count, self.count + b))     # distinct: no pair masked
+        self.count += b
+
+    def _pool(self):
+        """The pooled sets, cut to pool_size, words_embs padded to the pool's longest caption."""
+        p = self.pool_size
+        cat = {k: torch.cat(v, 0)[:p] for k, v in self.sets.items() if k != "words_embs"}
+        max_len = int(cat["cap_lens"].max())
+        we = self.sets["words_embs"]
+        words = torch.zeros((self.count, we[0].shape[1], max(max_len, *[w.shape[2] for w in we])),
+                            device=we[0].device, dtype=torch.float32)
+        acc = 0
+        for w in we:
+            words[acc:acc + w.shape[0], :, :w.shape[2]] = w
+            acc += w.shape[0]
+        cat["words_embs"] = words[:p, :, :max_len].contiguous()
+        import numpy as np
+        cat["class_ids"] = np.concatenate(self.class_ids, 0)[:p]
+        return cat
+
+    def _score(self):
+        s = self._pool()
+        p = self.pool_size
+        labels = torch.arange(p, device=s["cnn_code"].device)
+        _, _, _, w_acc = words_loss(s["region_features"], s["words_embs"], labels, s["cap_lens"], s["class_ids"], p,
+                                    is_training=False, need_att_maps=False)
+        _, _, s_acc = sent_loss(s["cnn_code"], s["sent_emb"], labels, s["class_ids"], p, is_training=False)
+        self.w_accuracy.append(float(w_acc))
+        self.s_accuracy.append(float(s_acc))
+
+    def result(self):
+        import numpy as np
+        w, s = np.asarray(self.w_accuracy), np.asarray(self.s_accuracy)
+        return float(w.mean()), float(w.std()), float(s.mean()), float(s.std())

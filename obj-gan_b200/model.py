@@ -1100,3 +1100,259 @@ def _get_rois_blob(im_rois, im_scale_factors):
     levels = np.repeat(np.arange(im_rois.shape[0] // n), n).reshape(-1, 1)
     rois = im_rois * np.asarray(im_scale_factors, dtype=np.float64)[levels]
     return np.hstack((levels.astype(np.float64), rois)).astype(np.float32, copy=False)
+
+
+# --------------------------------------------------------------------------------------------------
+# DAMSM image encoder (ref: model.py:182-287): torchvision's Inception-v3 trunk from Conv2d_1a_3x3 to Mixed_7c,
+# emb_features (1x1, 768 -> nef) on the Mixed_6e map and emb_cnn_code (Linear 2048 -> nef) on the 8x8 average.
+# --------------------------------------------------------------------------------------------------
+class _ConvWeight(nn.Module):
+    """nn.Conv2d(bias=False) parameter holder (key ``weight``)."""
+
+    def __init__(self, cin, cout, kh, kw):
+        super().__init__()
+        self.weight = nn.Parameter(torch.empty(cout, cin, kh, kw))
+        nn.init.normal_(self.weight.data, 0.0, (1.0 / (cin * kh * kw)) ** 0.5)
+
+
+class _BN(nn.Module):
+    """nn.BatchNorm2d(eps=0.001) parameters and buffers (used in eval mode only)."""
+
+    def __init__(self, c):
+        super().__init__()
+        self.weight = nn.Parameter(torch.ones(c))
+        self.bias = nn.Parameter(torch.zeros(c))
+        self.register_buffer("running_mean", torch.zeros(c))
+        self.register_buffer("running_var", torch.ones(c))
+        self.register_buffer("num_batches_tracked", torch.tensor(0, dtype=torch.long))
+
+
+class BasicConv2d(nn.Module):
+    """torchvision's BasicConv2d: conv (no bias) -> BatchNorm2d(eps=0.001) -> ReLU; keys ``conv.weight``, ``bn.*``."""
+
+    def __init__(self, cin, cout, k, stride=1, pad=(0, 0)):
+        super().__init__()
+        kh, kw = (k, k) if isinstance(k, int) else k
+        self.conv = _ConvWeight(cin, cout, kh, kw)
+        self.bn = _BN(cout)
+        self.kh, self.kw, self.stride, self.pad = kh, kw, stride, pad
+
+    def bn_tensors(self):
+        return (self.bn.weight, self.bn.bias, self.bn.running_mean, self.bn.running_var)
+
+
+# Inception-v3 blocks (torchvision.models.inception): per block kind, its BasicConv2d children as
+# (name, cin, cout, kernel, stride, padding) with "IN" the block's input width and "C7" the InceptionC width.
+_INCEPTION_CONVS = {
+    "A": [("branch1x1", "IN", 64, 1, 1, 0), ("branch5x5_1", "IN", 48, 1, 1, 0), ("branch5x5_2", 48, 64, 5, 1, 2),
+          ("branch3x3dbl_1", "IN", 64, 1, 1, 0), ("branch3x3dbl_2", 64, 96, 3, 1, 1),
+          ("branch3x3dbl_3", 96, 96, 3, 1, 1), ("branch_pool", "IN", "PF", 1, 1, 0)],
+    "B": [("branch3x3", "IN", 384, 3, 2, 0), ("branch3x3dbl_1", "IN", 64, 1, 1, 0), ("branch3x3dbl_2", 64, 96, 3, 1, 1),
+          ("branch3x3dbl_3", 96, 96, 3, 2, 0)],
+    "C": [("branch1x1", "IN", 192, 1, 1, 0), ("branch7x7_1", "IN", "C7", 1, 1, 0),
+          ("branch7x7_2", "C7", "C7", (1, 7), 1, (0, 3)), ("branch7x7_3", "C7", 192, (7, 1), 1, (3, 0)),
+          ("branch7x7dbl_1", "IN", "C7", 1, 1, 0), ("branch7x7dbl_2", "C7", "C7", (7, 1), 1, (3, 0)),
+          ("branch7x7dbl_3", "C7", "C7", (1, 7), 1, (0, 3)), ("branch7x7dbl_4", "C7", "C7", (7, 1), 1, (3, 0)),
+          ("branch7x7dbl_5", "C7", 192, (1, 7), 1, (0, 3)), ("branch_pool", "IN", 192, 1, 1, 0)],
+    "D": [("branch3x3_1", "IN", 192, 1, 1, 0), ("branch3x3_2", 192, 320, 3, 2, 0),
+          ("branch7x7x3_1", "IN", 192, 1, 1, 0), ("branch7x7x3_2", 192, 192, (1, 7), 1, (0, 3)),
+          ("branch7x7x3_3", 192, 192, (7, 1), 1, (3, 0)), ("branch7x7x3_4", 192, 192, 3, 2, 0)],
+    "E": [("branch1x1", "IN", 320, 1, 1, 0), ("branch3x3_1", "IN", 384, 1, 1, 0),
+          ("branch3x3_2a", 384, 384, (1, 3), 1, (0, 1)), ("branch3x3_2b", 384, 384, (3, 1), 1, (1, 0)),
+          ("branch3x3dbl_1", "IN", 448, 1, 1, 0), ("branch3x3dbl_2", 448, 384, 3, 1, 1),
+          ("branch3x3dbl_3a", 384, 384, (1, 3), 1, (0, 1)), ("branch3x3dbl_3b", 384, 384, (3, 1), 1, (1, 0)),
+          ("branch_pool", "IN", 192, 1, 1, 0)],
+}
+# (name, kind, input width, pool_features or c7)
+_INCEPTION_BLOCKS = [("Mixed_5b", "A", 192, 32), ("Mixed_5c", "A", 256, 64), ("Mixed_5d", "A", 288, 64),
+                     ("Mixed_6a", "B", 288, 0), ("Mixed_6b", "C", 768, 128), ("Mixed_6c", "C", 768, 160),
+                     ("Mixed_6d", "C", 768, 160), ("Mixed_6e", "C", 768, 192), ("Mixed_7a", "D", 768, 0),
+                     ("Mixed_7b", "E", 1280, 0), ("Mixed_7c", "E", 2048, 0)]
+_STEM = [("Conv2d_1a_3x3", 3, 32, 3, 2, 0), ("Conv2d_2a_3x3", 32, 32, 3, 1, 0), ("Conv2d_2b_3x3", 32, 64, 3, 1, 1),
+         ("Conv2d_3b_1x1", 64, 80, 1, 1, 0), ("Conv2d_4a_3x3", 80, 192, 3, 1, 0)]
+
+
+def _pair(v):
+    return (v, v) if isinstance(v, int) else tuple(v)
+
+
+class _InceptionBlock(nn.Module):
+    def __init__(self, kind, cin, param):
+        super().__init__()
+        self.kind = kind
+        sub = {"IN": cin, "PF": param, "C7": param}
+        for name, ci, co, k, s, p in _INCEPTION_CONVS[kind]:
+            self.add_module(name, BasicConv2d(sub.get(ci, ci), sub.get(co, co), _pair(k), s, _pair(p)))
+
+
+def _enc_layer(convs, relu=True):
+    c0 = convs[0]
+    return ops.EncConv([c.conv.weight for c in convs], [c.bn_tensors() for c in convs], c0.kh, c0.kw, c0.stride,
+                       c0.pad[0], c0.pad[1], eps=1e-3, relu=relu)
+
+
+def _block_steps(blk, name, src, dst, chans):
+    """Program steps of one Inception block: sibling 1x1 convolutions run as one GEMM (their weights concatenated
+    along N); final branch outputs go into their channel slice of the block output."""
+    s, L = [], lambda *n: _enc_layer([getattr(blk, m) for m in n])
+    t = lambda x: f"{name}.{x}"
+
+    def fused(names, outs):
+        """siblings -> fused buffer, then each part to outs[i] = (buffer, channel offset)"""
+        layer = L(*names)
+        chans[t("fused")] = layer.cout
+        s.append(("conv", layer, src, t("fused"), 0))
+        off = 0
+        for n, (d, doff) in zip(names, outs):
+            co = getattr(blk, n).conv.weight.shape[0]
+            if d != dst:
+                chans[d] = co
+            s.append(("copy", t("fused"), off, d, doff, co))
+            off += co
+
+    def conv(n, a, b, off=0, width=None):
+        layer = L(n)
+        if b != dst:
+            chans[b] = layer.cout
+        s.append(("conv", layer, a, b, off))
+        return layer.cout
+
+    def pool_branch(off):
+        s.append(("avgpool", src, t("pool")))
+        conv("branch_pool", t("pool"), dst, off)
+
+    if blk.kind == "A":
+        fused(["branch1x1", "branch5x5_1", "branch3x3dbl_1"], [(dst, 0), (t("b5"), 0), (t("d1"), 0)])
+        conv("branch5x5_2", t("b5"), dst, 64)
+        conv("branch3x3dbl_2", t("d1"), t("d2"))
+        conv("branch3x3dbl_3", t("d2"), dst, 128)
+        pool_branch(224)
+        chans[dst] = 224 + blk.branch_pool.conv.weight.shape[0]
+    elif blk.kind == "B":
+        conv("branch3x3", src, dst, 0)
+        conv("branch3x3dbl_1", src, t("d1"))
+        conv("branch3x3dbl_2", t("d1"), t("d2"))
+        conv("branch3x3dbl_3", t("d2"), dst, 384)
+        s.append(("maxpool", src, dst, 480))
+        chans[dst] = 480 + blk.branch3x3dbl_1.conv.weight.shape[1]
+    elif blk.kind == "C":
+        fused(["branch1x1", "branch7x7_1", "branch7x7dbl_1"], [(dst, 0), (t("a1"), 0), (t("d1"), 0)])
+        conv("branch7x7_2", t("a1"), t("a2"))
+        conv("branch7x7_3", t("a2"), dst, 192)
+        conv("branch7x7dbl_2", t("d1"), t("d2"))
+        conv("branch7x7dbl_3", t("d2"), t("d3"))
+        conv("branch7x7dbl_4", t("d3"), t("d4"))
+        conv("branch7x7dbl_5", t("d4"), dst, 384)
+        pool_branch(576)
+        chans[dst] = 768
+    elif blk.kind == "D":
+        fused(["branch3x3_1", "branch7x7x3_1"], [(t("a1"), 0), (t("b1"), 0)])
+        conv("branch3x3_2", t("a1"), dst, 0)
+        conv("branch7x7x3_2", t("b1"), t("b2"))
+        conv("branch7x7x3_3", t("b2"), t("b3"))
+        conv("branch7x7x3_4", t("b3"), dst, 320)
+        s.append(("maxpool", src, dst, 512))
+        chans[dst] = 512 + blk.branch3x3_1.conv.weight.shape[1]
+    else:  # E
+        fused(["branch1x1", "branch3x3_1", "branch3x3dbl_1"], [(dst, 0), (t("a1"), 0), (t("d1"), 0)])
+        conv("branch3x3_2a", t("a1"), dst, 320)
+        conv("branch3x3_2b", t("a1"), dst, 704)
+        conv("branch3x3dbl_2", t("d1"), t("d2"))
+        conv("branch3x3dbl_3a", t("d2"), dst, 1088)
+        conv("branch3x3dbl_3b", t("d2"), dst, 1472)
+        pool_branch(1856)
+        chans[dst] = 2048
+    return s
+
+
+class CNN_ENCODER(_Base):
+    """The DAMSM image encoder (ref: model.py:182-287) with the reference's state_dict keys and shapes.  It is frozen
+    and eval-only, as the reference uses it (trainer.py:75-89, evaluator.py:97-105): the forward computes the input
+    gradient (when the input requires grad) and never a weight gradient.  Construction reads no file; the trunk's
+    weights start as fan-in-scaled normal draws until a snapshot is loaded.
+
+    forward(x): x (B, 3, H, W) NCHW in [-1, 1] -> (features (B, nef, 17, 17), cnn_code (B, nef)).
+    forward_nhwc(x): x (B, H, W, 8) NHWC with the channel pad lanes zero, same outputs."""
+
+    def __init__(self, nef=256):
+        super().__init__()
+        self.nef = nef
+        for name, ci, co, k, s, p in _STEM:
+            self.add_module(name, BasicConv2d(ci, co, k, s, _pair(p)))
+        for name, kind, cin, param in _INCEPTION_BLOCKS:
+            self.add_module(name, _InceptionBlock(kind, cin, param))
+        self.emb_features = _ConvWeight(768, nef, 1, 1)
+        self.emb_cnn_code = LinearP(2048, nef)
+        # ref: model.py:231-234 init_trainable_weights
+        self.emb_features.weight.data.uniform_(-0.1, 0.1)
+        self.emb_cnn_code.weight.data.uniform_(-0.1, 0.1)
+        nn.init.uniform_(self.emb_cnn_code.bias.data, -(1 / 2048) ** 0.5, (1 / 2048) ** 0.5)
+        self.requires_grad_(False)
+        self.eval()
+        self._prog = None
+
+    def _apply(self, fn, *a, **k):
+        # .to() / .cuda() replace the BatchNorm buffers with new tensors: the program must fold from the new ones
+        self._prog = None
+        return super()._apply(fn, *a, **k)
+
+    @classmethod
+    def from_snapshot(cls, path, device="cuda", nef=256):
+        """The reference's ``image_encoder100.pth`` (keys with or without ``module.``)."""
+        enc = cls(nef).to(device)
+        enc.load_state_dict(torch.load(path, map_location="cpu"))
+        return enc
+
+    def load_state_dict(self, state_dict, strict=True, **kw):
+        """Also takes keys with the ``module.`` prefix nn.DataParallel adds, and snapshots without the
+        ``num_batches_tracked`` buffers (torch <= 0.4.0 did not write them)."""
+        sd = {(k[len("module."):] if k.startswith("module.") else k): v for k, v in state_dict.items()}
+        for k, v in self.state_dict().items():
+            if k.endswith(".num_batches_tracked") and k not in sd:
+                sd[k] = v.clone()
+        return super().load_state_dict(sd, strict=strict, **kw)
+
+    def program(self):
+        """The forward as an ops.InceptionProgram (built once; it holds the parameters, not copies)."""
+        if self._prog is None:
+            steps, chans = [("interp", "x", "x299", 299)], {}
+            src = "x299"
+            for i, (name, ci, co, k, s, p) in enumerate(_STEM):
+                dst = f"stem{i}"
+                chans[dst] = co
+                steps.append(("conv", _enc_layer([getattr(self, name)]), src, dst, 0))
+                src = dst
+                if name in ("Conv2d_2b_3x3", "Conv2d_4a_3x3"):     # max_pool2d(3, 2) after these two
+                    chans[dst + "p"] = co
+                    steps.append(("maxpool", src, dst + "p", 0))
+                    src = dst + "p"
+            for name, kind, cin, param in _INCEPTION_BLOCKS:
+                steps += _block_steps(getattr(self, name), name, src, name, chans)
+                src = name
+                if name == "Mixed_6e":
+                    chans["features"] = self.nef
+                    steps.append(("conv", ops.EncConv([self.emb_features.weight], None, 1, 1, relu=False),
+                                  "Mixed_6e", "features", 0))
+            steps.append(("gap", "Mixed_7c", "pooled"))
+            self._prog = ops.InceptionProgram(steps, chans, ("features", "pooled"))
+        return self._prog
+
+    def _check(self):
+        if self.training:
+            raise RuntimeError("CNN_ENCODER runs in eval mode only (BatchNorm uses the running statistics); call "
+                               ".eval() -- training the image encoder (DAMSM pretraining) is not supported")
+        for n, p in self.named_parameters():
+            if p.requires_grad:
+                raise RuntimeError(f"CNN_ENCODER is frozen and computes no weight gradient, but {n} requires grad; "
+                                   "call .requires_grad_(False)")
+
+    def forward_nhwc(self, x):
+        self._check()
+        feat, pooled = ops.inception_trunk(x, self.program())
+        cnn_code = self.emb_cnn_code(pooled)
+        return ops.to_nchw(feat, self.nef), cnn_code
+
+    def forward(self, x):
+        assert x.dim() == 4 and x.shape[1] == 3, "CNN_ENCODER takes (B, 3, H, W) images"
+        self._check()
+        return self.forward_nhwc(ops.to_nhwc(x))

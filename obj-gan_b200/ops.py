@@ -1884,3 +1884,300 @@ def boxes_to_layout(labels, samples, steps, mean_std, label_to_class, count_stat
     _call("og_box_layout", _p(_i64(labels)), _p(samples.contiguous()), _p(_i64(steps)), _p(ms), _p(_i64(label_to_class)),
           _p(cs), _p(ncnt), b, s, nl, c, boxes_num, int(min_size), _p(rois), _p(fm_rois), _p(roi_cls), _p(num_rois))
     return list(rois.unbind(0)), fm_rois, roi_cls, num_rois
+
+
+# --------------------------------------------------------------------------------------------------
+# Inception-v3 image encoder (CNN_ENCODER, ref: model.py:182-287).  Its convolutions have their own dispatch: the
+# tap-list tensor-core launcher for every kernel shape (1x1, 1xN, Nx1, 3x3, 5x5, valid 3x3 stride 2), the exact-fp32
+# SIMT kernel under TC_MIN_PIXELS output pixels or with CONV_ENGINE = "simt".  _tc_kind and the routes of the other
+# layers are not involved.  Eval BatchNorm is folded into the weights and the bias (og_bn_fold), ReLU is the LeakyReLU
+# epilogue with slope 0.  The backward computes the input gradient only; the encoder is frozen.
+# --------------------------------------------------------------------------------------------------
+class EncConv:
+    """One BasicConv2d (conv without bias -> BatchNorm2d(eps=0.001) in eval mode -> ReLU), or several that read the
+    same input fused along N (their weights concatenated), or a plain bias-free conv (``bns`` None, no ReLU).
+    ``weights``: OIHW parameters; ``bns``: (gamma, beta, running_mean, running_var) per weight."""
+
+    def __init__(self, weights, bns, kh, kw, stride=1, padh=0, padw=0, eps=1e-3, relu=True):
+        self.weights, self.bns = list(weights), (list(bns) if bns is not None else None)
+        self.kh, self.kw, self.stride, self.padh, self.padw, self.eps = kh, kw, stride, padh, padw, eps
+        self.act = ACT_LRELU if relu else ACT_NONE
+        self.cin = self.weights[0].shape[1]
+        self.couts = [w.shape[0] for w in self.weights]
+        self.cout = sum(self.couts)
+        assert self.cout % 8 == 0
+        self._key = None
+        self.wf = self.bias = self.cache = None
+
+    def folded(self):
+        """(folded OIHW weight, folded bias, PackedWeights); recomputed when any source tensor changed."""
+        srcs = list(self.weights) + [t for bn in (self.bns or ()) for t in bn]
+        key = (_param_epoch[0],) + tuple((t.data_ptr(), t._version) for t in srcs)
+        if key != self._key:
+            w0 = self.weights[0]
+            if self.bns is None and len(self.weights) == 1:
+                self.wf, self.bias = w0.detach(), None
+            else:
+                r = self.cin * self.kh * self.kw
+                self.wf = torch.empty((self.cout, self.cin, self.kh, self.kw), device=w0.device, dtype=torch.float32)
+                self.bias = torch.empty(self.cout, device=w0.device, dtype=torch.float32)
+                off = 0
+                for w, (g, b, m, v) in zip(self.weights, self.bns):
+                    _chk(w, g, b, m, v)
+                    co = w.shape[0]
+                    _call("og_bn_fold", _p(w.detach().contiguous()), co, r, _p(g), _p(b), _p(m), _p(v), self.eps,
+                          self.wf.data_ptr() + off * r * 4, self.bias.data_ptr() + off * 4)
+                    off += co
+            self.cache = PackedWeights()          # a new fold is a new operand: its packed copies start empty
+            self._key = key
+        return self.wf, self.bias, self.cache
+
+    def out_hw(self, h, w):
+        return ((h + 2 * self.padh - self.kh) // self.stride + 1, (w + 2 * self.padw - self.kw) // self.stride + 1)
+
+    def on_tc(self, n, h, w):
+        oh, ow = self.out_hw(h, w)
+        return CONV_ENGINE in ("f16x3", "f16") and n * oh * ow >= TC_MIN_PIXELS
+
+    def macs(self, h, w):
+        oh, ow = self.out_hw(h, w)
+        return oh * ow * self.cout * self.cin * self.kh * self.kw
+
+
+def _enc_tc(xs, n, ws, ntaps_w, kw_rows, yptr, oh, ow, k, ystr, ohf, owf, osy, op, taps, bias, act):
+    import ctypes
+    xh = xs[0]
+    sn, sh, sw, c = xh.shape
+    arr = _int_array(taps)
+    _call("og_conv2d_tc", _p(xh), _p(xs[1]), _p(xs[2]), n, sn, sh, sw, c, _p(ws[0]), _p(ws[1]), _p(ws[2]), ntaps_w,
+          kw_rows, yptr, oh, ow, k, ystr[0], ystr[1], ystr[2], ohf, owf, osy, osy, op[0], op[1], ctypes.addressof(arr),
+          len(taps), 0, _nsplit(), _p(bias), act, 0.0)
+
+
+def _split_s2d_odd(x):
+    n, h, w, c = x.shape
+    shape = (4 * n, (h + 1) // 2, (w + 1) // 2, c)
+    xh = _empty_slack(shape, x.device)
+    xl = _empty_slack(shape, x.device) if CONV_ENGINE == "f16x3" else None
+    amax = torch.empty(1, device=x.device, dtype=torch.int32)
+    _call("og_prep_split_s2d", _p(x), n, h, w, c, _p(amax), 0, _p(xh), _p(xl))
+    return xh, xl, amax
+
+
+def enc_conv_fwd(layer, x, y, yoff=0):
+    """y[..., yoff:yoff + layer.cout] = act(conv(x) * s + b): x (N, H, W, cpad(cin)) contiguous, y (N, OH, OW, Cy)."""
+    n, h, w, c = x.shape
+    assert c == cpad(layer.cin) and y.is_contiguous()
+    oh, ow = layer.out_hw(h, w)
+    cy = y.shape[3]
+    assert y.shape[1:3] == (oh, ow) and yoff + layer.cout <= cy
+    wf, bias, cache = layer.folded()
+    k = layer.cout
+    yptr = y.data_ptr() + yoff * 4
+    ystr = (oh * ow * cy, ow * cy, cy)
+    if layer.on_tc(n, h, w):
+        ws = cache.get_hilo(wf, c, k, 0, 0, 1)                    # [tap][co][ci]
+        kk = layer.kh * layer.kw
+        if layer.stride == 2:                                     # valid 3x3 stride 2 on the phase blocks
+            xs = _split_s2d_odd(x)
+            taps = []
+            for i in range(layer.kh):
+                dh, a = divmod(i, 2)
+                for j in range(layer.kw):
+                    dw, b = divmod(j, 2)
+                    taps.append((dh, dw, (a * 2 + b) * n, i * layer.kw + j))
+        else:
+            xs = _split(x, 0)
+            taps = [(i - layer.padh, j - layer.padw, 0, i * layer.kw + j) for i in range(layer.kh) for j in range(layer.kw)]
+        _enc_tc(xs, n, ws, kk, k, yptr, oh, ow, k, ystr, oh, ow, 1, (0, 0), taps, bias, layer.act)
+    else:
+        wp, _ = cache.get(wf, c, k, 0, 0, False)
+        _call("og_conv2d_simt_pad2", _p(x), n, h, w, c, h * w * c, w * c, c, _p(wp), yptr, oh, ow, k, ystr[0], ystr[1],
+              ystr[2], layer.kh, layer.kw, layer.stride, layer.padh, layer.padw, PAD_ZERO, _p(bias), layer.act, 0.0,
+              1 if (bias is None and layer.act == ACT_NONE and yoff == 0 and cy == k) else 0)
+
+
+def enc_conv_dgrad(layer, gp, h, w):
+    """Input gradient of the convolution (the epilogue's ReLU already applied to gp (N, OH, OW, cout)); (N, h, w, cpad(cin))."""
+    n, oh, ow, k = gp.shape
+    c = cpad(layer.cin)
+    wf, _, cache = layer.folded()
+    gx = torch.empty((n, h, w, c), device=gp.device, dtype=torch.float32)
+    if layer.on_tc(n, h, w):
+        ws = cache.get_hilo(wf, c, k, 0, 0, 0)                    # [tap][ci][co]
+        gs = _split(gp, 0)
+        ystr = (h * w * c, w * c, c)
+        if layer.stride == 2:     # input pixel (2i + a, 2j + b) <- kernel taps with kh = a, kw = b (mod 2)
+            for a in range(2):
+                for b in range(2):
+                    taps = [(-((i - a) // 2), -((j - b) // 2), 0, i * layer.kw + j)
+                            for i in range(layer.kh) if (i - a) % 2 == 0 for j in range(layer.kw) if (j - b) % 2 == 0]
+                    _enc_tc(gs, n, ws, layer.kh * layer.kw, c, gx.data_ptr(), (h + 1) // 2, (w + 1) // 2, c, ystr,
+                            h, w, 2, (a, b), taps, None, ACT_NONE)
+        else:
+            taps = [(layer.padh - i, layer.padw - j, 0, i * layer.kw + j) for i in range(layer.kh) for j in range(layer.kw)]
+            _enc_tc(gs, n, ws, layer.kh * layer.kw, c, gx.data_ptr(), h, w, c, ystr, h, w, 1, (0, 0), taps, None,
+                    ACT_NONE)
+    else:
+        _, wt = cache.get(wf, c, k, 0, 0, True)
+        _call("og_conv2d_simt_pad2", _p(gp), n, oh, ow, k, oh * ow * k, ow * k, k, _p(wt), _p(gx), h, w, c, h * w * c,
+              w * c, c, layer.kh, layer.kw, layer.stride, layer.padh, layer.padw, TRANSPOSED, 0, ACT_NONE, 0.0, 1)
+    return gx
+
+
+class InceptionProgram:
+    """The encoder as a list of steps over named NHWC buffers, run forward and, for the input gradient, backward.
+
+    Steps: ("interp", src, dst, size), ("conv", layer, src, dst, off), ("copy", src, soff, dst, doff, nch),
+    ("maxpool", src, dst, off), ("avgpool", src, dst), ("gap", src, dst).  ``chans[name]`` is a buffer's channel
+    count (its concatenated width for a block output)."""
+
+    def __init__(self, steps, chans, outputs):
+        self.steps, self.chans, self.outputs = steps, chans, outputs
+
+    def forward(self, x):
+        bufs = {"x": x}
+        for st in self.steps:
+            op = st[0]
+            if op == "interp":
+                _, s, d, size = st
+                src = bufs[s]
+                n, h, w, c = src.shape
+                y = torch.empty((n, size, size, c), device=src.device, dtype=torch.float32)
+                _call("og_bilinear_fwd", _p(src), n, h, w, c, size, size, _p(y))
+                bufs[d] = y
+            elif op == "conv":
+                _, layer, s, d, off = st
+                src = bufs[s]
+                if d not in bufs:
+                    oh, ow = layer.out_hw(src.shape[1], src.shape[2])
+                    bufs[d] = torch.empty((src.shape[0], oh, ow, self.chans[d]), device=src.device, dtype=torch.float32)
+                enc_conv_fwd(layer, src, bufs[d], off)
+            elif op == "copy":
+                _, s, soff, d, doff, nch = st
+                src = bufs[s]
+                n, h, w, cs = src.shape
+                if d not in bufs:
+                    bufs[d] = torch.empty((n, h, w, self.chans[d]), device=src.device, dtype=torch.float32)
+                _call("og_copy_channels", _p(src), cs, soff, _p(bufs[d]), self.chans[d], doff, nch, n * h * w, 0)
+            elif op == "maxpool":
+                _, s, d, off = st
+                src = bufs[s]
+                n, h, w, c = src.shape
+                if d not in bufs:
+                    bufs[d] = torch.empty((n, (h - 3) // 2 + 1, (w - 3) // 2 + 1, self.chans[d]), device=src.device,
+                                          dtype=torch.float32)
+                _call("og_maxpool3s2_fwd", _p(src), n, h, w, c, _p(bufs[d]), self.chans[d], off)
+            elif op == "avgpool":
+                _, s, d = st
+                src = bufs[s]
+                bufs[d] = torch.empty_like(src)
+                n, h, w, c = src.shape
+                _call("og_avgpool3s1_fwd", _p(src), n, h, w, c, _p(bufs[d]))
+            elif op == "gap":
+                _, s, d = st
+                src = bufs[s]
+                n, h, w, c = src.shape
+                bufs[d] = torch.empty((n, c), device=src.device, dtype=torch.float32)
+                _call("og_global_avg_fwd", _p(src), n, h * w, c, _p(bufs[d]))
+        return bufs
+
+    def backward(self, bufs, grads):
+        """grads: {output name: gradient}; returns the gradient of "x".  Each step adds its input gradients in the
+        fixed reverse order of the steps."""
+        grads = dict(grads)
+
+        def acc(name, t):
+            if name in grads:
+                _call("og_add", _p(grads[name]), _p(t), _p(grads[name]), t.numel())
+            else:
+                grads[name] = t
+
+        def acc_slice(name, src_t, src_ld, src_off, nch, doff):
+            if name not in grads:
+                grads[name] = torch.empty_like(bufs[name])
+                zeros_into(grads[name])
+            d = grads[name]
+            _call("og_copy_channels", _p(src_t), src_ld, src_off, _p(d), d.shape[-1], doff, nch, d.numel() // d.shape[-1],
+                  1)
+
+        for st in reversed(self.steps):
+            op = st[0]
+            if op == "conv":
+                _, layer, s, d, off = st
+                if d not in grads:
+                    continue
+                y, g = bufs[d], grads[d]
+                n, oh, ow, cy = y.shape
+                gp = torch.empty((n, oh, ow, layer.cout), device=y.device, dtype=torch.float32)
+                _call("og_relu_grad_slice", _p(y), cy, off, _p(g), cy, off, _p(gp), layer.cout, 0, layer.cout,
+                      n * oh * ow, 1 if layer.act == ACT_LRELU else 0)
+                src = bufs[s]
+                acc(s, enc_conv_dgrad(layer, gp, src.shape[1], src.shape[2]))
+            elif op == "copy":
+                _, s, soff, d, doff, nch = st
+                if d in grads:
+                    acc_slice(s, grads[d], self.chans[d], doff, nch, soff)
+            elif op == "maxpool":
+                _, s, d, off = st
+                if d not in grads:
+                    continue
+                src = bufs[s]
+                n, h, w, c = src.shape
+                gx = torch.empty_like(src)
+                _call("og_maxpool3s2_bwd", _p(src), _p(grads[d]), self.chans[d], off, n, h, w, c, _p(gx))
+                acc(s, gx)
+            elif op == "avgpool":
+                _, s, d = st
+                if d not in grads:
+                    continue
+                n, h, w, c = bufs[s].shape
+                gx = torch.empty_like(bufs[s])
+                _call("og_avgpool3s1_bwd", _p(grads[d]), n, h, w, c, _p(gx))
+                acc(s, gx)
+            elif op == "gap":
+                _, s, d = st
+                if d not in grads:
+                    continue
+                n, h, w, c = bufs[s].shape
+                gx = torch.empty_like(bufs[s])
+                _call("og_global_avg_bwd", _p(grads[d].contiguous()), n, h * w, c, _p(gx))
+                acc(s, gx)
+            elif op == "interp":
+                _, s, d, size = st
+                if d not in grads:
+                    continue
+                n, h, w, c = bufs[s].shape
+                gx = torch.empty_like(bufs[s])
+                _call("og_bilinear_bwd_gather", _p(grads[d]), n, h, w, c, size, size, _p(gx))
+                acc(s, gx)
+        return grads.get("x")
+
+
+class _InceptionTrunk(torch.autograd.Function):
+    """(x NHWC (N, H, W, 8)) -> the program's outputs; the backward gives the input gradient only, and the forward
+    keeps its buffers only when x requires grad."""
+
+    @staticmethod
+    def forward(ctx, x, prog):
+        _chk(x)
+        bufs = prog.forward(x.contiguous())
+        ctx.prog = prog
+        ctx.bufs = bufs if ctx.needs_input_grad[0] else None
+        return tuple(bufs[o] for o in prog.outputs)
+
+    @staticmethod
+    def backward(ctx, *gs):
+        bufs, prog = ctx.bufs, ctx.prog
+        ctx.bufs = None
+        grads = {}
+        for name, g in zip(prog.outputs, gs):
+            if g is not None:
+                grads[name] = g.contiguous()
+        if not grads:
+            return None, None
+        return prog.backward(bufs, grads), None
+
+
+def inception_trunk(x, prog):
+    return _InceptionTrunk.apply(x, prog)

@@ -83,10 +83,12 @@ class GSampler:
     """Eval-mode G_NET forward with the reference's inputs and 6-tuple output, CUDA-graph replayed per input shape."""
 
     def __init__(self, netG: model.G_NET, netShpG: model.SHP_G_NET | None = None,
-                 text_encoder: model.RNN_ENCODER | None = None, glove=None, clabels_emb=None, box_generator=None):
+                 text_encoder: model.RNN_ENCODER | None = None, glove=None, clabels_emb=None, box_generator=None,
+                 image_encoder: model.CNN_ENCODER | None = None):
         """``glove``: the GloVe table (V, 50) as a tensor or an nn.Embedding (the reference's ``glove_emb``);
         ``clabels_emb``: (num_classes, 50) label embeddings (see ops.class_label_emb) used when a batch has none;
-        ``box_generator``: a boxgen.BoxGenerator that makes the layout of caption batches without ``rois``."""
+        ``box_generator``: a boxgen.BoxGenerator that makes the layout of caption batches without ``rois``;
+        ``image_encoder``: the DAMSM CNN_ENCODER that ``encode_image`` runs (R-precision, losses.RPrecision)."""
         self.netG = netG.eval()
         self.netShpG = netShpG.eval() if netShpG is not None else None
         self.text_encoder = text_encoder.eval() if text_encoder is not None else None
@@ -98,6 +100,8 @@ class GSampler:
         self.glove = glove.detach().to(self.device).float().contiguous() if glove is not None else None
         self.clabels_emb = clabels_emb.detach().to(self.device).float().contiguous() if clabels_emb is not None else None
         self.box_generator = box_generator.to(self.device) if box_generator is not None else None
+        self.image_encoder = image_encoder.to(self.device).eval().requires_grad_(False) if image_encoder is not None \
+            else None
         self._graphs = {}
         self._box_graphs = {}
         self._pool = None
@@ -106,7 +110,7 @@ class GSampler:
     def from_snapshot(cls, path: str, num_classes: int = 80, device="cuda", shape_snapshot: str | None = None,
                       text_snapshot: str | None = None, glove=None, cat_labels=None, cat_label_lens=None,
                       cat_label_order=None, box_checkpoint: str | None = None, mean_std=None, gaussian_dict=None,
-                      cat_ids=None) -> "GSampler":
+                      cat_ids=None, image_snapshot: str | None = None) -> "GSampler":
         """A reference-format generator snapshot (``netG_epoch_N.pth``, what StepBTrainer.save_model writes), and
         optionally a shape generator snapshot (the reference's ``cfg.TEST.NET_SHP_G``) and a text encoder snapshot
         (``cfg.TRAIN.NET_E``; ntoken is read from its ``encoder.weight``); keys with or without the ``module.`` prefix
@@ -114,7 +118,8 @@ class GSampler:
         ``cat_label_order``: the length-sorted class labels, their lengths and the resort indices of the reference's
         load_cat_label (load.py:305-355), from which the label embeddings are computed once (prepare_cat_emb).
         ``box_checkpoint``: the reference's box checkpoint directory, read with ``mean_std``, ``gaussian_dict`` and
-        ``cat_ids`` by BoxGenerator.from_reference (its encoder is the text snapshot's network)."""
+        ``cat_ids`` by BoxGenerator.from_reference (its encoder is the text snapshot's network).  ``image_snapshot``:
+        the DAMSM image encoder (``image_encoder100.pth``) for ``encode_image``."""
         shp = _new_shp_g(num_classes, device) if shape_snapshot is not None else None
         enc = None
         if text_snapshot is not None:
@@ -134,7 +139,8 @@ class GSampler:
             from .boxgen import BoxGenerator
             box = BoxGenerator.from_reference(box_checkpoint, text_snapshot, mean_std, gaussian_dict, cat_ids,
                                               device=device)
-        s = cls(_new_g(num_classes, device), shp, enc, glove, clabels, box)
+        img = model.CNN_ENCODER.from_snapshot(image_snapshot, device) if image_snapshot is not None else None
+        s = cls(_new_g(num_classes, device), shp, enc, glove, clabels, box, img)
         s.load_state_dict(torch.load(path, map_location="cpu"))
         if shape_snapshot is not None:
             s.load_shape_state_dict(torch.load(shape_snapshot, map_location="cpu"))
@@ -148,6 +154,17 @@ class GSampler:
         s = cls(_new_g(trainer.netG.num_classes, trainer.device))
         s.load_state_dict(trainer.bG.ema_state_dict())
         return s
+
+    def encode_image(self, fake_imgs):
+        """(region_features (B, nef, 17, 17), cnn_code (B, nef)) of generated images through the image encoder (ref:
+        evaluator.py:375-376); ``fake_imgs``: the 256x256 images (B, 3, H, W) or the sampler's list of scales (the last
+        one is encoded).  Eager, no gradient."""
+        if self.image_encoder is None:
+            raise ValueError("this sampler has no image encoder: build it with GSampler(netG, image_encoder=...)")
+        if isinstance(fake_imgs, (list, tuple)):
+            fake_imgs = fake_imgs[-1]
+        with torch.no_grad():
+            return self.image_encoder(fake_imgs.detach())
 
     def load_state_dict(self, state_dict: dict) -> None:
         """Loads G weights (strict) and drops every captured graph."""
