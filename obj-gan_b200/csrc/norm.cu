@@ -67,7 +67,14 @@ __global__ void __launch_bounds__(256) norm_stats_kernel(const float* __restrict
 }
 
 // mean / rstd from (sum, sumsq); optional BatchNorm running-stat update.
-__global__ void norm_finalize_kernel(const double* __restrict__ stats, int groups, int C, double count, float eps,
+// The one-pass variance sumsq / count - mean^2 carries the rounding of the fp32 squares in the 4-row pre-sum: an error of
+// up to ~3 * 2^-24 * sumsq / count.  Where that could exceed 2^-10 of var + eps -- a large offset over a small spread, or
+// a constant channel (a dead filter plus its bias), which would get var = O(2^-24 mean^2) instead of 0 and an rstd far
+// below 1 / sqrt(eps), wrong by the same factor in the input gradient -- the channel is marked for
+// norm_stats_exact_kernel (stats[2 i] = 1, else 0), which recomputes it from shifted fp64 sums and does its running-stat
+// update.  Every other channel keeps the one-pass result.
+constexpr double OG_NORM_CANCEL = 1024.0;
+__global__ void norm_finalize_kernel(double* __restrict__ stats, int groups, int C, double count, float eps,
                                      float* __restrict__ mean, float* __restrict__ rstd, float* running_mean,
                                      float* running_var, float momentum, int real_c,
                                      long long* num_batches_tracked) {
@@ -75,14 +82,65 @@ __global__ void norm_finalize_kernel(const double* __restrict__ stats, int group
   if (i >= groups * C) return;
   if (i == 0 && num_batches_tracked) *num_batches_tracked += 1;
   double m = stats[i * 2] / count;
-  double var = stats[i * 2 + 1] / count - m * m;
+  const double ms = stats[i * 2 + 1] / count;
+  double var = ms - m * m;
   if (var < 0) var = 0;
+  const bool redo = ms > OG_NORM_CANCEL * (var + (double)eps);
+  stats[i * 2] = redo ? 1.0 : 0.0;
+  if (redo) return;
   mean[i] = (float)m;
   rstd[i] = (float)(1.0 / sqrt(var + (double)eps));
   if (running_mean && groups == 1 && i < real_c) {
     double unbiased = count > 1 ? var * count / (count - 1.0) : var;
     running_mean[i] = (1.f - momentum) * running_mean[i] + momentum * (float)m;
     running_var[i] = (1.f - momentum) * running_var[i] + momentum * (float)unbiased;
+  }
+}
+
+// The channels norm_finalize_kernel marked: mean and variance from fp64 sums of x - k, k = the group's first row of the
+// channel, so the squares are of deviations and nothing cancels.  grid: (C / 4, groups), block 256: one block per channel
+// quad; blocks whose four channels are all unmarked return at once.  The block sum is taken in a fixed order.
+__global__ void __launch_bounds__(256) norm_stats_exact_kernel(const float* __restrict__ x, int C, long long P,
+                                                               double count, float eps, const double* __restrict__ stats,
+                                                               float* __restrict__ mean, float* __restrict__ rstd,
+                                                               float* running_mean, float* running_var, float momentum,
+                                                               int real_c) {
+  const long long g = blockIdx.y;
+  const long long i0 = g * C + blockIdx.x * 4;
+  if (stats[i0 * 2] == 0 && stats[i0 * 2 + 2] == 0 && stats[i0 * 2 + 4] == 0 && stats[i0 * 2 + 6] == 0) return;
+  const float* base = x + g * P * C + blockIdx.x * 4;
+  const float4 k = ldg4(base);
+  double a[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (long long p = threadIdx.x; p < P; p += blockDim.x) {
+    const float4 v = ldg4(base + p * C);
+    const double d0 = (double)v.x - k.x, d1 = (double)v.y - k.y, d2 = (double)v.z - k.z, d3 = (double)v.w - k.w;
+    a[0] += d0; a[1] += d1; a[2] += d2; a[3] += d3;
+    a[4] += d0 * d0; a[5] += d1 * d1; a[6] += d2 * d2; a[7] += d3 * d3;
+  }
+  __shared__ double sh[8][8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const double t = warp_sum_d(a[j]);
+    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5][j] = t;
+  }
+  __syncthreads();
+  if (threadIdx.x >= 4) return;
+  const int j = threadIdx.x;
+  const long long i = i0 + j;
+  if (stats[i * 2] == 0) return;
+  double s = 0, q = 0;
+  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { s += sh[w][j]; q += sh[w][4 + j]; }
+  const double d = s / count;
+  double var = q / count - d * d;
+  if (var < 0) var = 0;
+  const double m = (double)(j == 0 ? k.x : j == 1 ? k.y : j == 2 ? k.z : k.w) + d;
+  mean[i] = (float)m;
+  rstd[i] = (float)(1.0 / sqrt(var + (double)eps));
+  const int c = (int)(i - g * C);
+  if (running_mean && gridDim.y == 1 && c < real_c) {
+    double unbiased = count > 1 ? var * count / (count - 1.0) : var;
+    running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * (float)m;
+    running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)unbiased;
   }
 }
 
@@ -624,6 +682,8 @@ OG_API int og_norm_stats(const float* x, int groups, long long P, int C, float e
   norm_finalize_kernel<<<og_cdiv((long long)groups * C, 256), 256, 0, stream>>>(stats, groups, C, (double)P, eps, mean, rstd,
                                                                      running_mean, running_var, momentum, real_c,
                                                                      num_batches_tracked);
+  norm_stats_exact_kernel<<<dim3(C / 4, groups), 256, 0, stream>>>(x, C, P, (double)P, eps, stats, mean, rstd,
+                                                                   running_mean, running_var, momentum, real_c);
   OG_RETURN_LAST_ERROR();
 }
 
