@@ -410,6 +410,15 @@ int og_bn_fold(const float* w, int Co, long long R, const float* gamma, const fl
                const float* var, float eps, float* wout, float* bout, cudaStream_t stream);
 int og_prep_split_s2d(const float* x, int N, int H, int W, int C, unsigned* amax, int amax_ready, void* xh, void* xl,
                       cudaStream_t stream);
+/* Scoring networks (INCEPTION_V3 / INCEPTION_V3_FID, ref: model.py:290-451; csrc/inception.cu).
+ * og_inception_input: NCHW (N, 3, H, W) images in [-1, 1] -> NHWC (N, OS, OS, 8), pad lanes zero; mode 0 (IS): the
+ * affine x * 0.5 + 0.5, (v - mean) / std, then the align_corners=True resize; mode 1 (FID): the half-pixel resize, then
+ * x * 0.5 + 0.5, v * (std / 0.5) + (mean - 0.5) / 0.5.  og_softmax_rows: softmax over the C columns of each row,
+ * deterministic.  og_moments_f64: adds one batch x (n, d) fp32 to the fp64 sums s1 = sum (x - k) and s2 = sum (x - k)
+ * (x - k)^T (tiles on or above the diagonal); init = 1 sets k to the batch's first row and starts the sums. */
+int og_inception_input(const float* x, int N, int H, int W, int OS, int mode, float* y, cudaStream_t stream);
+int og_softmax_rows(const float* x, int rows, int C, float* y, cudaStream_t stream);
+int og_moments_f64(const float* x, int n, int d, int init, double* k, double* s1, double* s2, cudaStream_t stream);
 int og_relu_grad_slice(const float* y, int ldy, int yoff, const float* g, int ldg, int goff, float* out, int ldo,
                        int ooff, int nch, long long P, int relu, cudaStream_t stream);
 

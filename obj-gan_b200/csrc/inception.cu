@@ -287,6 +287,149 @@ __global__ void __launch_bounds__(256) relu_grad_slice_kernel(const float* __res
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// The scoring networks' input (INCEPTION_V3 / INCEPTION_V3_FID, ref: model.py:301-315, 416-451): NCHW fp32 images
+// in [-1, 1] -> the trunk's NHWC (N, 299, 299, 8) input, pad lanes zero, in one pass.
+//   mode 0 (IS):  v = x * 0.5 + 0.5, v = (v - mean_c) / std_c, then bilinear resize with align_corners=True;
+//   mode 1 (FID): bilinear resize with half-pixel centres (align_corners=False), then v = x * 0.5 + 0.5,
+//                 v = v * a_c + b_c with a_c = std_c / 0.5, b_c = (mean_c - 0.5) / 0.5 (the reference's inverse of
+//                 the usual normalisation, kept).
+// Every step rounds to fp32 on its own as the reference's separate tensor ops do (no contraction into an FMA); the
+// constants are the Python doubles rounded to fp32.  Mode 0 applies the affine to the four taps before they are
+// blended, which is what affine-then-resize computes.
+// ---------------------------------------------------------------------------------------------------------------
+struct InceptionAffine {
+  float m[3], s[3];      // mode 0: (v - m) / s;  mode 1: v * s + m
+};
+
+__device__ __forceinline__ float half_affine(float x) { return __fadd_rn(__fmul_rn(x, 0.5f), 0.5f); }
+
+__device__ __forceinline__ void resize_coord(int o, int in, float r, int align, int& i0, int& i1, float& l) {
+  float f = align ? r * o : fmaxf(__fsub_rn(__fmul_rn(r, o + 0.5f), 0.5f), 0.f);
+  i0 = min((int)f, in - 1);
+  i1 = i0 + (i0 < in - 1);
+  l = fminf(f - i0, 1.f);
+}
+
+__global__ void __launch_bounds__(256) inception_input_kernel(const float* __restrict__ x, int H, int W, int OS,
+                                                              int mode, float rh, float rw, InceptionAffine af,
+                                                              long long total, float* __restrict__ y) {
+  GRID_STRIDE(i, total) {
+    const int ow = (int)(i % OS);
+    long long t = i / OS;
+    const int oh = (int)(t % OS);
+    const long long n = t / OS;
+    int h0, h1, w0, w1;
+    float lh, lw;
+    resize_coord(oh, H, rh, mode == 0, h0, h1, lh);
+    resize_coord(ow, W, rw, mode == 0, w0, w1, lw);
+    const float hh = 1.f - lh, hw = 1.f - lw;
+    float v[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float* p = x + (n * 3 + c) * (long long)H * W;
+      float a = __ldg(p + (long long)h0 * W + w0), b = __ldg(p + (long long)h0 * W + w1);
+      float d = __ldg(p + (long long)h1 * W + w0), e = __ldg(p + (long long)h1 * W + w1);
+      if (mode == 0) {
+        a = __fdiv_rn(__fsub_rn(half_affine(a), af.m[c]), af.s[c]);
+        b = __fdiv_rn(__fsub_rn(half_affine(b), af.m[c]), af.s[c]);
+        d = __fdiv_rn(__fsub_rn(half_affine(d), af.m[c]), af.s[c]);
+        e = __fdiv_rn(__fsub_rn(half_affine(e), af.m[c]), af.s[c]);
+      }
+      float r = hh * (hw * a + lw * b) + lh * (hw * d + lw * e);
+      if (mode == 1) r = __fadd_rn(__fmul_rn(half_affine(r), af.s[c]), af.m[c]);
+      v[c] = r;
+    }
+    st4(y + i * 8, make_float4(v[0], v[1], v[2], 0.f));
+    st4(y + i * 8 + 4, make_float4(0.f, 0.f, 0.f, 0.f));
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Row softmax y = exp(x - max) / sum exp(x - max) over C columns, one CTA per row.  Accurate expf; the per-thread
+// partials (columns tid, tid + 256, ...) and the shared-memory tree combine in a fixed order, so results are
+// deterministic.
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ x, int C, float* __restrict__ y) {
+  __shared__ float red[256];
+  const float* xr = x + (long long)blockIdx.x * C;
+  float* yr = y + (long long)blockIdx.x * C;
+  const int tid = threadIdx.x;
+  float m = -INFINITY;
+  for (int c = tid; c < C; c += 256) m = fmaxf(m, __ldg(xr + c));
+  red[tid] = m;
+  __syncthreads();
+  for (int s = 128; s > 0; s >>= 1) {
+    if (tid < s) red[tid] = fmaxf(red[tid], red[tid + s]);
+    __syncthreads();
+  }
+  m = red[0];
+  __syncthreads();
+  float sum = 0.f;
+  for (int c = tid; c < C; c += 256) {
+    const float e = expf(__ldg(xr + c) - m);
+    yr[c] = e;
+    sum += e;
+  }
+  red[tid] = sum;
+  __syncthreads();
+  for (int s = 128; s > 0; s >>= 1) {
+    if (tid < s) red[tid] += red[tid + s];
+    __syncthreads();
+  }
+  const float total = red[0];
+  for (int c = tid; c < C; c += 256) yr[c] = yr[c] / total;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Streaming FID moments in fp64: for a batch x (n, d) fp32, s1[j] += sum_r (x[r, j] - k[j]) and
+// s2[i, j] += sum_r (x[r, i] - k[i]) (x[r, j] - k[j]) for the tiles on or above the diagonal (tile row <= tile
+// column; the caller mirrors the rest).  init = 1 starts the sums (s1, s2 are written, not added to).  k is the first row of the first batch (init = 1 also writes it): a sum of
+// squares about a shift near the data does not cancel the way one about zero does.  Each element is summed by one
+// thread over the rows in order, then added to the running total: deterministic.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int MT = 32;   // moment tile (MT x MT elements, 256 threads, 4 per thread)
+
+__global__ void __launch_bounds__(256) moments_f64_kernel(const float* __restrict__ x, int n, int d, int init,
+                                                          double* __restrict__ k, double* __restrict__ s1,
+                                                          double* __restrict__ s2) {
+  const int ti = blockIdx.y, tj = blockIdx.x;
+  if (ti > tj) return;
+  __shared__ double a[MT][MT + 1], b[MT][MT + 1];   // [row][column within the tile]
+  const int tx = threadIdx.x % MT, ty = threadIdx.x / MT;
+  const int i0 = ti * MT, j0 = tj * MT;
+  const double ki = i0 + tx < d ? (init ? (double)__ldg(x + i0 + tx) : k[i0 + tx]) : 0.0;
+  const double kj = j0 + tx < d ? (init ? (double)__ldg(x + j0 + tx) : k[j0 + tx]) : 0.0;
+  double acc[4] = {0.0, 0.0, 0.0, 0.0}, acc1 = 0.0;
+  for (int r0 = 0; r0 < n; r0 += MT) {
+    __syncthreads();
+    for (int r = ty; r < MT; r += 256 / MT) {
+      const bool row = r0 + r < n;
+      a[r][tx] = row && i0 + tx < d ? (double)__ldg(x + (long long)(r0 + r) * d + i0 + tx) - ki : 0.0;
+      b[r][tx] = row && j0 + tx < d ? (double)__ldg(x + (long long)(r0 + r) * d + j0 + tx) - kj : 0.0;
+    }
+    __syncthreads();
+    const int rn = min(MT, n - r0);
+    for (int r = 0; r < rn; ++r) {
+      const double bj = b[r][tx];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[q] = fma(a[r][ty + 8 * q], bj, acc[q]);
+      if (ti == tj && ty == 0) acc1 += bj;
+    }
+  }
+  if (j0 + tx >= d) return;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int i = i0 + ty + 8 * q;
+    double* o = s2 + (long long)i * d + j0 + tx;
+    if (i < d) *o = init ? acc[q] : *o + acc[q];
+  }
+  if (ti == tj && ty == 0) {
+    s1[j0 + tx] = init ? acc1 : s1[j0 + tx] + acc1;
+    if (init) k[j0 + tx] = kj;
+  }
+}
+
 }  // namespace
 
 OG_API int og_maxpool3s2_fwd(const float* x, int N, int H, int W, int C, float* y, int ldy, int yoff,
@@ -378,5 +521,44 @@ OG_API int og_relu_grad_slice(const float* y, int ldy, int yoff, const float* g,
   if (total == 0) return 0;
   relu_grad_slice_kernel<<<grid_for(total), 256, 0, stream>>>(y, ldy, yoff, g, ldg, goff, out, ldo, ooff, nch / 4, relu,
                                                               total);
+  OG_RETURN_LAST_ERROR();
+}
+
+// x: (N, 3, H, W) NCHW fp32 contiguous; y: (N, 299, 299, 8) -- OS x OS in general.  mode 0: IS, 1: FID (see above)
+OG_API int og_inception_input(const float* x, int N, int H, int W, int OS, int mode, float* y, cudaStream_t stream) {
+  if (H < 1 || W < 1 || OS < 1 || (mode != 0 && mode != 1)) return (int)cudaErrorInvalidValue;
+  const long long total = (long long)N * OS * OS;
+  if (total == 0) return 0;
+  const double mean[3] = {0.485, 0.456, 0.406}, std_[3] = {0.229, 0.224, 0.225};
+  InceptionAffine af;
+  for (int c = 0; c < 3; ++c) {
+    af.m[c] = mode == 0 ? (float)mean[c] : (float)((mean[c] - 0.5) / 0.5);
+    af.s[c] = mode == 0 ? (float)std_[c] : (float)(std_[c] / 0.5);
+  }
+  float rh, rw;
+  if (mode == 0) {
+    rh = OS > 1 ? (float)(H - 1) / (float)(OS - 1) : 0.f;
+    rw = OS > 1 ? (float)(W - 1) / (float)(OS - 1) : 0.f;
+  } else {
+    rh = (float)H / (float)OS;
+    rw = (float)W / (float)OS;
+  }
+  inception_input_kernel<<<grid_for(total), 256, 0, stream>>>(x, H, W, OS, mode, rh, rw, af, total, y);
+  OG_RETURN_LAST_ERROR();
+}
+
+OG_API int og_softmax_rows(const float* x, int rows, int C, float* y, cudaStream_t stream) {
+  if (rows == 0 || C == 0) return 0;
+  if (rows < 0 || C < 0) return (int)cudaErrorInvalidValue;
+  softmax_rows_kernel<<<rows, 256, 0, stream>>>(x, C, y);
+  OG_RETURN_LAST_ERROR();
+}
+
+// k, s1: (d) fp64, s2: (d, d) fp64 (only the tiles on or above the diagonal are written)
+OG_API int og_moments_f64(const float* x, int n, int d, int init, double* k, double* s1, double* s2,
+                          cudaStream_t stream) {
+  if (n < 1 || d < 1 || (init != 0 && init != 1)) return (int)cudaErrorInvalidValue;
+  const int t = (d + MT - 1) / MT;
+  moments_f64_kernel<<<dim3(t, t), 256, 0, stream>>>(x, n, d, init, k, s1, s2);
   OG_RETURN_LAST_ERROR();
 }

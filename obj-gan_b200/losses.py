@@ -397,3 +397,126 @@ class RPrecision:
         import numpy as np
         w, s = np.asarray(self.w_accuracy), np.asarray(self.s_accuracy)
         return float(w.mean()), float(w.std()), float(s.mean()), float(s.std())
+
+
+def _split_parts(p, num_splits):
+    n = p.shape[0]
+    return [p[i * n // num_splits:(i + 1) * n // num_splits] for i in range(num_splits)]
+
+
+def inception_score(p, num_splits):
+    """(mean, std) over ``num_splits`` contiguous splits of exp(E_x KL(p(y|x) || p(y))) on the float32 predictions p
+    (N, 1000), in numpy with the reference's arithmetic (utils.py:417-428).  A probability of exactly 0 gives nan,
+    as it does there."""
+    import numpy as np
+    scores = []
+    for part in _split_parts(p, num_splits):
+        kl = part * (np.log(part) - np.log(np.expand_dims(np.mean(part, 0), 0)))
+        scores.append(np.exp(np.mean(np.sum(kl, 1))))
+    return np.mean(scores), np.std(scores)
+
+
+def negative_log_posterior(p, num_splits):
+    """(mean, std) over the splits of the mean of -log max_y p(y|x) (utils.py:431-441)."""
+    import numpy as np
+    scores = [np.mean(-1. * np.log(np.max(part, 1))) for part in _split_parts(p, num_splits)]
+    return np.mean(scores), np.std(scores)
+
+
+class InceptionScore:
+    """The evaluator's Inception score and confidence (ref: evaluator.py:421-450) over the INCEPTION_V3 predictions
+    of every added batch.  ``add`` keeps the predictions on the device; ``result()`` reads them once and returns
+    (mean, std, mean_conf, std_conf).  The evaluator uses min(10, batch_size) splits.  Each data-parallel rank
+    scores the predictions it was given."""
+
+    def __init__(self, num_splits=10):
+        self.num_splits = num_splits
+        self.predictions = []
+
+    def add(self, predictions):
+        self.predictions.append(predictions.detach())
+
+    def result(self):
+        p = torch.cat(self.predictions, 0).float().cpu().numpy()
+        mean, std = inception_score(p, self.num_splits)
+        mean_conf, std_conf = negative_log_posterior(p, self.num_splits)
+        return float(mean), float(std), float(mean_conf), float(std_conf)
+
+
+def frechet_distance(mu1, sigma1, mu2, sigma2, eps=1e-6):
+    """d^2 = |mu1 - mu2|^2 + Tr(sigma1 + sigma2 - 2 sqrt(sigma1 sigma2)) in float64 with scipy's sqrtm (utils.py:
+    660-714): when the square root is not finite it is retried with eps added to both diagonals, and an imaginary
+    part larger than 1e-3 on its diagonal raises ValueError.  (sqrtm is called without ``disp``, which scipy 1.18
+    removed; the value is the same.)"""
+    import numpy as np
+    from scipy import linalg
+    mu1, mu2 = np.atleast_1d(mu1), np.atleast_1d(mu2)
+    sigma1, sigma2 = np.atleast_2d(sigma1), np.atleast_2d(sigma2)
+    if mu1.shape != mu2.shape or sigma1.shape != sigma2.shape:
+        raise ValueError("the two sets of statistics have different dimensions")
+    diff = mu1 - mu2
+    covmean = linalg.sqrtm(sigma1.dot(sigma2))
+    if not np.isfinite(covmean).all():
+        offset = np.eye(sigma1.shape[0]) * eps
+        covmean = linalg.sqrtm((sigma1 + offset).dot(sigma2 + offset))
+    if np.iscomplexobj(covmean):
+        if not np.allclose(np.diagonal(covmean).imag, 0, atol=1e-3):
+            raise ValueError(f"Imaginary component {np.max(np.abs(covmean.imag))}")
+        covmean = covmean.real
+    return diff.dot(diff) + np.trace(sigma1) + np.trace(sigma2) - 2 * np.trace(covmean)
+
+
+class _Moments:
+    """Streaming fp64 mean and covariance of (n, d) fp32 rows on the device (og_moments_f64): O(d^2) memory however
+    many rows are added."""
+
+    def __init__(self, dims):
+        self.dims, self.n, self.k = dims, 0, None
+
+    def add(self, x):
+        if x.dim() != 2 or x.shape[1] != self.dims:
+            raise ValueError(f"activations must be (N, {self.dims}), got {tuple(x.shape)}")
+        if self.k is None:
+            d = self.dims
+            self.k, self.s1 = (torch.empty(d, device=x.device, dtype=torch.float64) for _ in range(2))
+            self.s2 = torch.empty((d, d), device=x.device, dtype=torch.float64)
+        ops.moments_f64(x, self.k, self.s1, self.s2, self.n == 0)
+        self.n += x.shape[0]
+
+    def statistics(self):
+        """(mu (d,), sigma (d, d)) float64; sigma as np.cov(rowvar=False), with n - 1."""
+        import numpy as np
+        if self.n < 2:
+            raise ValueError("the covariance needs at least two samples")
+        k, s1, s2 = (t.cpu().numpy() for t in (self.k, self.s1, self.s2))
+        t = np.arange(self.dims) // 32                 # og_moments_f64 writes the tiles on or above the diagonal
+        s2 = np.where(t[:, None] <= t[None, :], s2, s2.T)
+        m = s1 / self.n
+        return k + m, (s2 - np.outer(s1, m)) / (self.n - 1)
+
+
+class FrechetDistance:
+    """The evaluator's FID (ref: evaluator.py:429-457) from streamed activation moments.  ``add(fake_acts,
+    real_acts)`` takes (B, dims) activations of generated and of real images (INCEPTION_V3_FID.activations, or the
+    reference's dump_fid_acts arrays as tensors); either may be None.  ``statistics()`` returns ((mu, sigma) of the
+    real set, (mu, sigma) of the generated set) in float64; ``result()`` the distance between them."""
+
+    def __init__(self, dims=2048):
+        self.dims = dims
+        self.fake, self.real = _Moments(dims), _Moments(dims)
+
+    def add(self, fake_acts, real_acts=None):
+        if fake_acts is not None:
+            self.fake.add(fake_acts)
+        if real_acts is not None:
+            if not torch.is_tensor(real_acts):
+                import numpy as np
+                real_acts = torch.from_numpy(np.asarray(real_acts, dtype=np.float32))
+            self.real.add(real_acts.to(self.fake.k.device if self.fake.k is not None else "cuda"))
+
+    def statistics(self):
+        return self.real.statistics(), self.fake.statistics()
+
+    def result(self):
+        (mu1, sigma1), (mu2, sigma2) = self.statistics()
+        return float(frechet_distance(mu1, sigma1, mu2, sigma2))

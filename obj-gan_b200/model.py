@@ -1265,7 +1265,84 @@ def _block_steps(blk, name, src, dst, chans):
     return s
 
 
-class CNN_ENCODER(_Base):
+# stage outputs of the trunk: the two stem max-pools, then the blocks
+_STAGES = ("stem2p", "stem4p") + tuple(b[0] for b in _INCEPTION_BLOCKS)
+
+
+def _trunk_program(get, input_step, last, outputs, after=None):
+    """torchvision's Inception-v3 trunk as an ops.InceptionProgram: ``input_step`` writes "x299" from "x", then the
+    stem and the blocks run up to the stage ``last`` (a _STAGES name; "stem2p" / "stem4p" are the outputs of the
+    first / second max-pool, the others the block outputs).  ``get(name)``: the BasicConv2d or _InceptionBlock of
+    that torchvision name.  ``after``: {stage: (step, channels)} -- one more step that reads the stage's output
+    (its destination has that many channels).  ``outputs``: the buffers the program returns; "pooled" adds the
+    global average of the last stage."""
+    if last not in _STAGES:
+        raise ValueError(f"the trunk has no stage {last!r}; stages: {_STAGES}")
+    after = after or {}
+    steps, chans = [input_step], {}
+    src = "x299"
+
+    def staged(name):
+        if name in after:
+            step, c = after[name]
+            chans[step[3]] = c
+            steps.append(step)
+        return name == last
+
+    for i, (name, ci, co, k, s, p) in enumerate(_STEM):
+        dst = f"stem{i}"
+        chans[dst] = co
+        steps.append(("conv", _enc_layer([get(name)]), src, dst, 0))
+        src = dst
+        if name in ("Conv2d_2b_3x3", "Conv2d_4a_3x3"):     # max_pool2d(3, 2) after these two
+            chans[dst + "p"] = co
+            steps.append(("maxpool", src, dst + "p", 0))
+            src = dst + "p"
+            if staged(src):
+                break
+    else:
+        for name, kind, cin, param in _INCEPTION_BLOCKS:
+            steps += _block_steps(get(name), name, src, name, chans)
+            src = name
+            if staged(name):
+                break
+    if "pooled" in outputs:
+        steps.append(("gap", src, "pooled"))
+    return ops.InceptionProgram(steps, chans, tuple(outputs))
+
+
+class _FrozenInception(_Base):
+    """Shared behaviour of the Inception-v3 networks: frozen and eval-only, a program rebuilt after .to() (the
+    BatchNorm fold then reads the new buffers; loads are caught by the fold's version check), and state_dict loads
+    that accept the ``module.`` prefix and snapshots without ``num_batches_tracked``."""
+    _TRAIN_HINT = ""
+
+    def _apply(self, fn, *a, **k):
+        # .to() / .cuda() replace the BatchNorm buffers with new tensors: the program must fold from the new ones
+        self._prog = None
+        return super()._apply(fn, *a, **k)
+
+    def load_state_dict(self, state_dict, strict=True, **kw):
+        """Also takes keys with the ``module.`` prefix nn.DataParallel adds, and snapshots without the
+        ``num_batches_tracked`` buffers (torch <= 0.4.0 did not write them)."""
+        sd = {(k[len("module."):] if k.startswith("module.") else k): v for k, v in state_dict.items()}
+        for k, v in self.state_dict().items():
+            if k.endswith(".num_batches_tracked") and k not in sd:
+                sd[k] = v.clone()
+        return super().load_state_dict(sd, strict=strict, **kw)
+
+    def _check(self):
+        name = type(self).__name__
+        if self.training:
+            raise RuntimeError(f"{name} runs in eval mode only (BatchNorm uses the running statistics); call "
+                               f".eval(){self._TRAIN_HINT}")
+        for n, p in self.named_parameters():
+            if p.requires_grad:
+                raise RuntimeError(f"{name} is frozen and computes no weight gradient, but {n} requires grad; "
+                                   "call .requires_grad_(False)")
+
+
+class CNN_ENCODER(_FrozenInception):
     """The DAMSM image encoder (ref: model.py:182-287) with the reference's state_dict keys and shapes.  It is frozen
     and eval-only, as the reference uses it (trainer.py:75-89, evaluator.py:97-105): the forward computes the input
     gradient (when the input requires grad) and never a weight gradient.  Construction reads no file; the trunk's
@@ -1273,6 +1350,7 @@ class CNN_ENCODER(_Base):
 
     forward(x): x (B, 3, H, W) NCHW in [-1, 1] -> (features (B, nef, 17, 17), cnn_code (B, nef)).
     forward_nhwc(x): x (B, H, W, 8) NHWC with the channel pad lanes zero, same outputs."""
+    _TRAIN_HINT = " -- training the image encoder (DAMSM pretraining) is not supported"
 
     def __init__(self, nef=256):
         super().__init__()
@@ -1291,11 +1369,6 @@ class CNN_ENCODER(_Base):
         self.eval()
         self._prog = None
 
-    def _apply(self, fn, *a, **k):
-        # .to() / .cuda() replace the BatchNorm buffers with new tensors: the program must fold from the new ones
-        self._prog = None
-        return super()._apply(fn, *a, **k)
-
     @classmethod
     def from_snapshot(cls, path, device="cuda", nef=256):
         """The reference's ``image_encoder100.pth`` (keys with or without ``module.``)."""
@@ -1303,48 +1376,13 @@ class CNN_ENCODER(_Base):
         enc.load_state_dict(torch.load(path, map_location="cpu"))
         return enc
 
-    def load_state_dict(self, state_dict, strict=True, **kw):
-        """Also takes keys with the ``module.`` prefix nn.DataParallel adds, and snapshots without the
-        ``num_batches_tracked`` buffers (torch <= 0.4.0 did not write them)."""
-        sd = {(k[len("module."):] if k.startswith("module.") else k): v for k, v in state_dict.items()}
-        for k, v in self.state_dict().items():
-            if k.endswith(".num_batches_tracked") and k not in sd:
-                sd[k] = v.clone()
-        return super().load_state_dict(sd, strict=strict, **kw)
-
     def program(self):
         """The forward as an ops.InceptionProgram (built once; it holds the parameters, not copies)."""
         if self._prog is None:
-            steps, chans = [("interp", "x", "x299", 299)], {}
-            src = "x299"
-            for i, (name, ci, co, k, s, p) in enumerate(_STEM):
-                dst = f"stem{i}"
-                chans[dst] = co
-                steps.append(("conv", _enc_layer([getattr(self, name)]), src, dst, 0))
-                src = dst
-                if name in ("Conv2d_2b_3x3", "Conv2d_4a_3x3"):     # max_pool2d(3, 2) after these two
-                    chans[dst + "p"] = co
-                    steps.append(("maxpool", src, dst + "p", 0))
-                    src = dst + "p"
-            for name, kind, cin, param in _INCEPTION_BLOCKS:
-                steps += _block_steps(getattr(self, name), name, src, name, chans)
-                src = name
-                if name == "Mixed_6e":
-                    chans["features"] = self.nef
-                    steps.append(("conv", ops.EncConv([self.emb_features.weight], None, 1, 1, relu=False),
-                                  "Mixed_6e", "features", 0))
-            steps.append(("gap", "Mixed_7c", "pooled"))
-            self._prog = ops.InceptionProgram(steps, chans, ("features", "pooled"))
+            emb = ("conv", ops.EncConv([self.emb_features.weight], None, 1, 1, relu=False), "Mixed_6e", "features", 0)
+            self._prog = _trunk_program(lambda n: getattr(self, n), ("interp", "x", "x299", 299), "Mixed_7c",
+                                        ("features", "pooled"), {"Mixed_6e": (emb, self.nef)})
         return self._prog
-
-    def _check(self):
-        if self.training:
-            raise RuntimeError("CNN_ENCODER runs in eval mode only (BatchNorm uses the running statistics); call "
-                               ".eval() -- training the image encoder (DAMSM pretraining) is not supported")
-        for n, p in self.named_parameters():
-            if p.requires_grad:
-                raise RuntimeError(f"CNN_ENCODER is frozen and computes no weight gradient, but {n} requires grad; "
-                                   "call .requires_grad_(False)")
 
     def forward_nhwc(self, x):
         self._check()
@@ -1356,3 +1394,174 @@ class CNN_ENCODER(_Base):
         assert x.dim() == 4 and x.shape[1] == 3, "CNN_ENCODER takes (B, 3, H, W) images"
         self._check()
         return self.forward_nhwc(ops.to_nhwc(x))
+
+
+# --------------------------------------------------------------------------------------------------
+# Scoring networks (ref: model.py:290-451): the ImageNet Inception-v3 for the Inception score and for the FID
+# activations.  Same trunk as CNN_ENCODER, another input transform, and forward only.
+# --------------------------------------------------------------------------------------------------
+IS_INPUT, FID_INPUT = 0, 1      # og_inception_input modes
+# torchvision's Inception3 stem / block names in INCEPTION_V3_FID's blocks.<i>.<j> layout
+_FID_BLOCKS = (("Conv2d_1a_3x3", "Conv2d_2a_3x3", "Conv2d_2b_3x3"), ("Conv2d_3b_1x1", "Conv2d_4a_3x3"),
+               ("Mixed_5b", "Mixed_5c", "Mixed_5d", "Mixed_6a", "Mixed_6b", "Mixed_6c", "Mixed_6d", "Mixed_6e"),
+               ("Mixed_7a", "Mixed_7b", "Mixed_7c"))
+_FID_LAST = ("stem2p", "stem4p", "Mixed_6e", "Mixed_7c")      # the trunk stage that ends each block
+_FID_OUT = ("stem2p", "stem4p", "Mixed_6e", "pooled")
+
+
+def _imagenet_state_dict(src):
+    """torchvision's ``inception_v3_google-1a9a5a14.pth`` (keys as Inception3's, also with ``module.``), from its path
+    or as already loaded."""
+    sd = src if isinstance(src, dict) else torch.load(src, map_location="cpu")
+    return {(k[len("module."):] if k.startswith("module.") else k): v for k, v in sd.items()}
+
+
+class _InceptionAux(nn.Module):
+    """torchvision's InceptionAux parameters (held and loaded; the eval forward never runs it)."""
+
+    def __init__(self):
+        super().__init__()
+        self.conv0 = BasicConv2d(768, 128, 1)
+        self.conv1 = BasicConv2d(128, 768, 5)
+        self.fc = LinearP(768, 1000)
+
+
+class _Inception3(nn.Module):
+    """torchvision's Inception3(aux_logits=True, num_classes=1000) state_dict layout."""
+
+    def __init__(self):
+        super().__init__()
+        for name, ci, co, k, s, p in _STEM:
+            self.add_module(name, BasicConv2d(ci, co, k, s, _pair(p)))
+        for name, kind, cin, param in _INCEPTION_BLOCKS:
+            self.add_module(name, _InceptionBlock(kind, cin, param))
+            if name == "Mixed_6e":
+                self.AuxLogits = _InceptionAux()
+        self.fc = LinearP(2048, 1000)
+
+
+class INCEPTION_V3(_FrozenInception):
+    """The Inception-score network (ref: model.py:290-315) with the reference's state_dict keys (``model.`` plus
+    torchvision's Inception3 keys, AuxLogits included).  Frozen, eval-only, forward-only: the output carries no
+    gradient.  Each rank of a data-parallel run scores its own images; predictions are not gathered.
+
+    forward(x): x (B, 3, H, W) in [-1, 1] -> (B, 1000) class probabilities.  The input goes through x * 0.5 + 0.5,
+    the ImageNet normalisation and the align_corners=True resize to 299 (og_inception_input), the trunk to Mixed_7c,
+    the 8x8 average, ``fc`` and a row softmax (og_softmax_rows)."""
+
+    def __init__(self):
+        super().__init__()
+        self.model = _Inception3()
+        self.requires_grad_(False)
+        self.eval()
+        self._prog = None
+
+    @classmethod
+    def from_imagenet(cls, path, device="cuda"):
+        """torchvision's ImageNet file ``inception_v3_google-1a9a5a14.pth`` (its path, or its state_dict already
+        loaded), as the reference loads it."""
+        net = cls().to(device)
+        net.load_state_dict({"model." + k: v for k, v in _imagenet_state_dict(path).items()})
+        return net
+
+    def program(self):
+        if self._prog is None:
+            self._prog = _trunk_program(lambda n: getattr(self.model, n), ("input", "x", "x299", 299, IS_INPUT),
+                                        "Mixed_7c", ("pooled",))
+        return self._prog
+
+    def forward(self, x):
+        assert x.dim() == 4 and x.shape[1] == 3, "INCEPTION_V3 takes (B, 3, H, W) images"
+        self._check()
+        with torch.no_grad():
+            pooled = self.program().forward(x.detach().float().contiguous())["pooled"]
+            return ops.softmax_rows(self.model.fc(pooled))
+
+
+class INCEPTION_V3_FID(_FrozenInception):
+    """The FID network (ref: model.py:318-451) with the reference's ``blocks.<i>.<j>`` state_dict keys, holding only
+    the blocks up to the last one requested.  Frozen, eval-only, forward-only.
+
+    Blocks: 0 ends at the first max-pool (64 channels), 1 at the second (192), 2 at Mixed_6e (768), 3 at the Mixed_7c
+    average (2048).  The input goes through the half-pixel resize to 299, then x * 0.5 + 0.5 and the reference's
+    x * (std / 0.5) + (mean - 0.5) / 0.5 (og_inception_input); the trunk stops at the last requested block.
+
+    forward(x): x (B, 3, H, W) in [-1, 1] -> the list of the requested blocks' maps (B, C, h, w), by block index.
+    activations(x): the first requested block's map averaged over its pixels, (B, C) -- the reference's
+    get_activations (utils.py:587-641)."""
+    DEFAULT_BLOCK_INDEX = 3
+    BLOCK_INDEX_BY_DIM = {64: 0, 192: 1, 768: 2, 2048: 3}
+
+    def __init__(self, output_blocks=(DEFAULT_BLOCK_INDEX,)):
+        super().__init__()
+        self.output_blocks = sorted(output_blocks)
+        if not self.output_blocks or self.output_blocks[0] < 0 or self.output_blocks[-1] > 3:
+            raise ValueError(f"output_blocks must be block indices in 0..3, got {list(output_blocks)}")
+        self.last_needed_block = self.output_blocks[-1]
+        self.blocks = nn.ModuleList()
+        for b in range(self.last_needed_block + 1):
+            mods = nn.ModuleList()
+            for name in _FID_BLOCKS[b]:
+                kind = next((k for n, k, c, q in _INCEPTION_BLOCKS if n == name), None)
+                if kind is None:
+                    ci, co, k, s, p = next(r[1:] for r in _STEM if r[0] == name)
+                    mods.append(BasicConv2d(ci, co, k, s, _pair(p)))
+                else:
+                    cin, param = next((c, q) for n, k, c, q in _INCEPTION_BLOCKS if n == name)
+                    mods.append(_InceptionBlock(kind, cin, param))
+            self.blocks.append(mods)
+        self.requires_grad_(False)
+        self.eval()
+        self._prog = None
+
+    @classmethod
+    def from_imagenet(cls, path, device="cuda", output_blocks=(DEFAULT_BLOCK_INDEX,)):
+        """torchvision's ImageNet file ``inception_v3_google-1a9a5a14.pth`` (its path, or its state_dict already
+        loaded); only the needed blocks are read."""
+        net = cls(output_blocks).to(device)
+        net.load_state_dict(net.from_torchvision(_imagenet_state_dict(path)))
+        return net
+
+    def from_torchvision(self, sd):
+        """This module's state_dict from an Inception3 one (torchvision keys)."""
+        out = {}
+        for b, names in enumerate(_FID_BLOCKS[:self.last_needed_block + 1]):
+            for j, name in enumerate(names):
+                for k, v in sd.items():
+                    if k.startswith(name + "."):
+                        out[f"blocks.{b}.{j}.{k[len(name) + 1:]}"] = v
+        return out
+
+    def _module(self, name):
+        for b, names in enumerate(_FID_BLOCKS):
+            if name in names:
+                return self.blocks[b][names.index(name)]
+        raise KeyError(name)
+
+    def program(self):
+        if self._prog is None:
+            self._prog = _trunk_program(self._module, ("input", "x", "x299", 299, FID_INPUT),
+                                        _FID_LAST[self.last_needed_block],
+                                        tuple(_FID_OUT[b] for b in self.output_blocks))
+        return self._prog
+
+    def _outputs(self, x):
+        assert x.dim() == 4 and x.shape[1] == 3, "INCEPTION_V3_FID takes (B, 3, H, W) images"
+        self._check()
+        bufs = self.program().forward(x.detach().float().contiguous())
+        return [bufs[_FID_OUT[b]] for b in self.output_blocks]
+
+    def forward(self, x):
+        with torch.no_grad():
+            return [y.view(y.shape[0], -1, 1, 1) if y.dim() == 2 else ops.to_nchw(y, y.shape[-1])
+                    for y in self._outputs(x)]
+
+    def activations(self, x):
+        with torch.no_grad():
+            y = self._outputs(x)[0]
+            if y.dim() == 2:
+                return y
+            n, h, w, c = y.shape
+            out = torch.empty((n, c), device=y.device, dtype=torch.float32)
+            ops._call("og_global_avg_fwd", ops._p(y), n, h * w, c, ops._p(out))
+            return out

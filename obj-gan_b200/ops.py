@@ -2028,7 +2028,8 @@ def enc_conv_dgrad(layer, gp, h, w):
 class InceptionProgram:
     """The encoder as a list of steps over named NHWC buffers, run forward and, for the input gradient, backward.
 
-    Steps: ("interp", src, dst, size), ("conv", layer, src, dst, off), ("copy", src, soff, dst, doff, nch),
+    Steps: ("input", src, dst, size, mode) (og_inception_input: NCHW images to the trunk's NHWC input; forward
+    only), ("interp", src, dst, size), ("conv", layer, src, dst, off), ("copy", src, soff, dst, doff, nch),
     ("maxpool", src, dst, off), ("avgpool", src, dst), ("gap", src, dst).  ``chans[name]`` is a buffer's channel
     count (its concatenated width for a block output)."""
 
@@ -2039,7 +2040,15 @@ class InceptionProgram:
         bufs = {"x": x}
         for st in self.steps:
             op = st[0]
-            if op == "interp":
+            if op == "input":
+                _, s, d, size, mode = st
+                src = bufs[s]
+                _chk(src)
+                n, c, h, w = src.shape
+                assert c == 3 and src.is_contiguous()
+                bufs[d] = torch.empty((n, size, size, 8), device=src.device, dtype=torch.float32)
+                _call("og_inception_input", _p(src), n, h, w, size, mode, _p(bufs[d]))
+            elif op == "interp":
                 _, s, d, size = st
                 src = bufs[s]
                 n, h, w, c = src.shape
@@ -2181,3 +2190,19 @@ class _InceptionTrunk(torch.autograd.Function):
 
 def inception_trunk(x, prog):
     return _InceptionTrunk.apply(x, prog)
+
+
+def softmax_rows(x):
+    """Row softmax of a (rows, C) fp32 tensor (og_softmax_rows)."""
+    _chk(x)
+    x = x.contiguous()
+    y = torch.empty_like(x)
+    _call("og_softmax_rows", _p(x), x.shape[0], x.shape[1], _p(y))
+    return y
+
+
+def moments_f64(x, k, s1, s2, init):
+    """Adds the rows of x (n, d) fp32 to the fp64 shifted sums (k, s1, s2) of og_moments_f64."""
+    _chk(x, k, s1, s2)
+    x = x.detach().float().contiguous()
+    _call("og_moments_f64", _p(x), x.shape[0], x.shape[1], 1 if init else 0, _p(k), _p(s1), _p(s2))

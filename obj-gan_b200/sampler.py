@@ -84,11 +84,14 @@ class GSampler:
 
     def __init__(self, netG: model.G_NET, netShpG: model.SHP_G_NET | None = None,
                  text_encoder: model.RNN_ENCODER | None = None, glove=None, clabels_emb=None, box_generator=None,
-                 image_encoder: model.CNN_ENCODER | None = None):
+                 image_encoder: model.CNN_ENCODER | None = None, inception: model.INCEPTION_V3 | None = None,
+                 inception_fid: model.INCEPTION_V3_FID | None = None):
         """``glove``: the GloVe table (V, 50) as a tensor or an nn.Embedding (the reference's ``glove_emb``);
         ``clabels_emb``: (num_classes, 50) label embeddings (see ops.class_label_emb) used when a batch has none;
         ``box_generator``: a boxgen.BoxGenerator that makes the layout of caption batches without ``rois``;
-        ``image_encoder``: the DAMSM CNN_ENCODER that ``encode_image`` runs (R-precision, losses.RPrecision)."""
+        ``image_encoder``: the DAMSM CNN_ENCODER that ``encode_image`` runs (R-precision, losses.RPrecision);
+        ``inception`` / ``inception_fid``: the scoring networks that ``score_images`` runs (losses.InceptionScore,
+        losses.FrechetDistance)."""
         self.netG = netG.eval()
         self.netShpG = netShpG.eval() if netShpG is not None else None
         self.text_encoder = text_encoder.eval() if text_encoder is not None else None
@@ -102,6 +105,8 @@ class GSampler:
         self.box_generator = box_generator.to(self.device) if box_generator is not None else None
         self.image_encoder = image_encoder.to(self.device).eval().requires_grad_(False) if image_encoder is not None \
             else None
+        self.inception = inception.to(self.device).eval() if inception is not None else None
+        self.inception_fid = inception_fid.to(self.device).eval() if inception_fid is not None else None
         self._graphs = {}
         self._box_graphs = {}
         self._pool = None
@@ -110,7 +115,8 @@ class GSampler:
     def from_snapshot(cls, path: str, num_classes: int = 80, device="cuda", shape_snapshot: str | None = None,
                       text_snapshot: str | None = None, glove=None, cat_labels=None, cat_label_lens=None,
                       cat_label_order=None, box_checkpoint: str | None = None, mean_std=None, gaussian_dict=None,
-                      cat_ids=None, image_snapshot: str | None = None) -> "GSampler":
+                      cat_ids=None, image_snapshot: str | None = None, inception_weights: str | None = None,
+                      fid_dims: int = 2048) -> "GSampler":
         """A reference-format generator snapshot (``netG_epoch_N.pth``, what StepBTrainer.save_model writes), and
         optionally a shape generator snapshot (the reference's ``cfg.TEST.NET_SHP_G``) and a text encoder snapshot
         (``cfg.TRAIN.NET_E``; ntoken is read from its ``encoder.weight``); keys with or without the ``module.`` prefix
@@ -119,7 +125,9 @@ class GSampler:
         load_cat_label (load.py:305-355), from which the label embeddings are computed once (prepare_cat_emb).
         ``box_checkpoint``: the reference's box checkpoint directory, read with ``mean_std``, ``gaussian_dict`` and
         ``cat_ids`` by BoxGenerator.from_reference (its encoder is the text snapshot's network).  ``image_snapshot``:
-        the DAMSM image encoder (``image_encoder100.pth``) for ``encode_image``."""
+        the DAMSM image encoder (``image_encoder100.pth``) for ``encode_image``.  ``inception_weights``: torchvision's
+        ImageNet file (``inception_v3_google-1a9a5a14.pth``), from which both scoring networks of ``score_images``
+        are built, the FID one returning ``fid_dims`` activations (64, 192, 768 or 2048: cfg.TEST.FID_DIMS)."""
         shp = _new_shp_g(num_classes, device) if shape_snapshot is not None else None
         enc = None
         if text_snapshot is not None:
@@ -140,7 +148,13 @@ class GSampler:
             box = BoxGenerator.from_reference(box_checkpoint, text_snapshot, mean_std, gaussian_dict, cat_ids,
                                               device=device)
         img = model.CNN_ENCODER.from_snapshot(image_snapshot, device) if image_snapshot is not None else None
-        s = cls(_new_g(num_classes, device), shp, enc, glove, clabels, box, img)
+        inc = fid = None
+        if inception_weights is not None:
+            imagenet = model._imagenet_state_dict(inception_weights)        # one read of the ~100 MB file for both
+            inc = model.INCEPTION_V3.from_imagenet(imagenet, device)
+            fid = model.INCEPTION_V3_FID.from_imagenet(imagenet, device,
+                                                       [model.INCEPTION_V3_FID.BLOCK_INDEX_BY_DIM[fid_dims]])
+        s = cls(_new_g(num_classes, device), shp, enc, glove, clabels, box, img, inc, fid)
         s.load_state_dict(torch.load(path, map_location="cpu"))
         if shape_snapshot is not None:
             s.load_shape_state_dict(torch.load(shape_snapshot, map_location="cpu"))
@@ -165,6 +179,20 @@ class GSampler:
             fake_imgs = fake_imgs[-1]
         with torch.no_grad():
             return self.image_encoder(fake_imgs.detach())
+
+    def score_images(self, fake_imgs):
+        """(predictions (B, 1000), activations (B, dims)) of generated images through INCEPTION_V3 and
+        INCEPTION_V3_FID (ref: evaluator.py:421-434), for losses.InceptionScore and losses.FrechetDistance;
+        ``fake_imgs``: the 256x256 images (B, 3, H, W) or the sampler's list of scales (the last one is scored).
+        Eager, no gradient."""
+        if self.inception is None or self.inception_fid is None:
+            raise ValueError("this sampler has no scoring networks: build it with GSampler(netG, inception=..., "
+                             "inception_fid=...) or from_snapshot(..., inception_weights=...)")
+        if isinstance(fake_imgs, (list, tuple)):
+            fake_imgs = fake_imgs[-1]
+        with torch.no_grad():
+            x = fake_imgs.detach()
+            return self.inception(x), self.inception_fid.activations(x)
 
     def load_state_dict(self, state_dict: dict) -> None:
         """Loads G weights (strict) and drops every captured graph."""
