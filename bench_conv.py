@@ -3,6 +3,7 @@
 
     python bench_conv.py                         # fprop / dgrad / wgrad of each layer below (3xFP16)
     python bench_conv.py --step-profile DIR      # torch.profiler over eager Step-A steps (in a run of its own)
+    python bench_conv.py --cta-cost              # the conv1 forward's fixed cost per CTA (two channel counts)
 
 Per convolution and direction: ms per call (CUDA events around back-to-back calls, median of three windows, the
 spread beside it), algorithmic TFLOP/s (the layer as the model writes it: real channels, every tap of the kernel on
@@ -94,9 +95,10 @@ def issued_wgrad(n, oh, ow, kp, c, entries, nsplit=3):
         chh *= 2
     cn = 64 // (cw * chh)
     pix = (ow // cw) * (oh // chh) * math.ceil(n / cn) * 64
-    cr = (c + 15) // 16 * 16
-    bnw = 32 if cr <= 32 else 64 if cr <= 64 else 112 if cr <= 112 else 128
-    return nsplit * 2.0 * math.ceil(kp / 128) * 128 * math.ceil(c / bnw) * bnw * pix * entries
+    ntile = math.ceil(c / 128)                     # ci tiles fitted like the forward's N tile
+    bnw = next((b for b in BN_SET if b >= (math.ceil(c / ntile) + 7) // 8 * 8), 128)
+    rows = math.ceil(kp / 64) * 64                 # a 64-row co slab wholly past kp issues nothing
+    return nsplit * 2.0 * rows * ntile * bnw * pix * entries
 
 
 def layer_work(cin, cout, k, stride, mode, split, n, h, w):
@@ -137,7 +139,7 @@ def _time(fn, reps):
     return e0.elapsed_time(e1) / reps
 
 
-def bench_layer(spec, window_ms):
+def bench_layer(spec, window_ms, dirs=("fprop", "dgrad", "wgrad")):
     from objgan_b200 import model, ops
     from objgan_b200.lib import ACT_NONE, PAD_REFLECT, PAD_ZERO, UPSAMPLE2X
     name, cin, cout, k, stride, mode_s, split, n, h, w = spec
@@ -174,6 +176,8 @@ def bench_layer(spec, window_ms):
     out = {}
     with torch.no_grad():
         for d, fn in calls.items():
+            if d not in dirs:
+                continue
             for i in range(2 * nsets):
                 fn(i)
             torch.cuda.synchronize()
@@ -184,6 +188,22 @@ def bench_layer(spec, window_ms):
                       "alg_tflops": round(alg / (ms[1] * 1e-3) / 1e12, 2),
                       "issued_tflops": round(iss[d] / (ms[1] * 1e-3) / 1e12, 1), "reps": reps}
     return out
+
+
+# ---------------------------------------------------------------- fixed cost per CTA of the forward
+# The res-block conv1 forward with 192 and with 384 input channels: the same CTAs (pixel tiles x 4 N tiles of 104),
+# each with 27 resp. 54 stages of 4 k-steps.  With t = F + S (F: per-CTA set-up, fill and epilogue; S: the stages),
+# F = 2 t192 - t384.
+CTA_COST = [("conv1 fprop 192->388 @128", 192, 388, 3, 1, "reflect", 194, 16, 128, 128),
+            ("conv1 fprop 384->388 @128", 384, 388, 3, 1, "reflect", 194, 16, 128, 128)]
+
+
+def cta_cost(window_ms):
+    t1, t2 = (bench_layer(spec, window_ms, ("fprop",))["fprop"]["ms"] for spec in CTA_COST)
+    fixed = 2 * t1 - t2
+    print(f"conv1 fprop: {t1:.3f} ms at 192 channels, {t2:.3f} ms at 384; fixed per-CTA part {fixed:.3f} ms "
+          f"= {fixed / t1:.1%} of the 192-channel time")
+    return {"ms_192": t1, "ms_384": t2, "fixed_ms": round(fixed, 4), "fixed_share_192": round(fixed / t1, 4)}
 
 
 # ---------------------------------------------------------------- step profile
@@ -241,6 +261,7 @@ def main():
     ap.add_argument("--step-profile", metavar="DIR", help="profile whole Step-A steps instead; trace written to DIR")
     ap.add_argument("--window-ms", type=float, default=200.0, help="GPU time per timing window")
     ap.add_argument("--layers", default="", help="comma-separated substrings selecting layers (default: all)")
+    ap.add_argument("--cta-cost", action="store_true", help="split the conv1 forward into per-CTA and per-stage time")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_conv.py needs a CUDA device"
     torch.cuda.set_device(0)
@@ -249,6 +270,8 @@ def main():
     res = {"card": card()}
     if args.step_profile:
         res["step_profile"] = step_profile(args.step_profile)
+    elif args.cta_cost:
+        res["cta_cost"] = cta_cost(args.window_ms)
     else:
         sel = [s for s in args.layers.split(",") if s]
         res["layers"] = {}

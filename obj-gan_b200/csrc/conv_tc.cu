@@ -20,9 +20,9 @@
 // GEMM tiling: one CTA = 128 output pixels (a TN x TH x TW patch) x BN output channels (BN % 8 == 0,
 // <= 128); K loop over taps x 64-channel chunks; STAGES-deep smem ring of {A_hi, A_lo, B_hi, B_lo}.
 // Warpgroup roles: warpgroup 0 = TMA producer (one elected thread), warpgroups 1 and 2 = MMA + epilogue, each
-// owning 64 of the 128 tile rows.  The forward kernel issues one wgmma over the whole N extent per product and
-// k-step (the A tile is read from shared memory once); the weight-gradient kernel, whose B operand is MN-major,
-// issues 64-wide column blocks plus one narrower tail.
+// owning 64 of the 128 tile rows.  Both kernels issue one wgmma over the whole N extent per product and k-step (the A
+// tile is read from shared memory once); in the weight-gradient kernel that B operand is MN-major and spans several
+// 64-channel slabs.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include <cuda_fp16.h>
@@ -35,7 +35,6 @@ constexpr int TC_BK = 64;              // fp16 elements per k-chunk = one 128-by
 constexpr int TC_MAX_TAPS = 36;
 constexpr int TC_THREADS = 384;        // producer warpgroup + two consumer warpgroups
 constexpr int TC_CONSUMER_WARPS = 8;
-constexpr uint32_t TC_NBLK_BYTES = 64 * 128;   // one 64-wide block of B (64 K-major rows, or one MN-major slab)
 constexpr size_t TC_SMEM_BUDGET = 200 * 1024;  // operand ring per CTA (one CTA per SM; 227 KB is the sm_90 limit)
 
 struct TcTaps {
@@ -82,63 +81,9 @@ __device__ __forceinline__ TcScale tc_scale(const unsigned* amax_a, const unsign
   return s;
 }
 
-// 64 x BN fp32 accumulator of one consumer warpgroup: BN / 64 full 64-column blocks and a 0/32/48-column tail.
-// Column block j of the B operand starts TC_NBLK_BYTES * j bytes after the operand base.
-template <int BN, int TA, int TB>
-struct TcAcc {
-  static constexpr int NF = BN / 64, TAIL = BN % 64;
-  static_assert(TAIL == 0 || TAIL == 32 || TAIL == 48, "tile widths 32, 64, 112, 128");
-  float f[NF > 0 ? NF : 1][32];
-  float t[TAIL > 0 ? TAIL / 2 : 1];
-
-  __device__ __forceinline__ void zero() {
-#pragma unroll
-    for (int j = 0; j < NF; ++j)
-#pragma unroll
-      for (int i = 0; i < 32; ++i) f[j][i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < (TAIL > 0 ? TAIL / 2 : 1); ++i) t[i] = 0.f;
-  }
-  __device__ __forceinline__ void hold() {
-#pragma unroll
-    for (int j = 0; j < NF; ++j) wg_hold(f[j]);
-    wg_hold(t);
-  }
-  // scale_d = 0: D = A * B (the accumulator's previous contents are dropped)
-  __device__ __forceinline__ void mma(uint64_t a, uint64_t b, int scale_d) {
-#pragma unroll
-    for (int j = 0; j < NF; ++j) wg_mma_n64<TA, TB>(f[j], a, b + (uint64_t)((j * TC_NBLK_BYTES) >> 4), scale_d);
-    const uint64_t bt = b + (uint64_t)((NF * TC_NBLK_BYTES) >> 4);
-    if constexpr (TAIL == 32) wg_mma_n32<TA, TB>(t, a, bt, scale_d);
-    if constexpr (TAIL == 48) wg_mma_n48<TA, TB>(t, a, bt, scale_d);
-  }
-  __device__ __forceinline__ void add(const TcAcc& o) {
-#pragma unroll
-    for (int j = 0; j < NF; ++j)
-#pragma unroll
-      for (int i = 0; i < 32; ++i) f[j][i] += o.f[j][i];
-#pragma unroll
-    for (int i = 0; i < (TAIL > 0 ? TAIL / 2 : 1); ++i) t[i] += o.t[i];
-  }
-  // fn(column, row half h, value at column, value at column + 1) for every accumulator pair of this thread
-  template <class F>
-  __device__ __forceinline__ void each(int lane, F&& fn) const {
-    const int c2 = 2 * (lane & 3);
-#pragma unroll
-    for (int j = 0; j < NF; ++j)
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) fn(64 * j + 8 * i + c2, h, f[j][4 * i + 2 * h], f[j][4 * i + 2 * h + 1]);
-#pragma unroll
-    for (int i = 0; i < TAIL / 8; ++i)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) fn(64 * NF + 8 * i + c2, h, t[4 * i + 2 * h], t[4 * i + 2 * h + 1]);
-  }
-};
-
-// 64 x BN fp32 accumulator issued as ONE wgmma per call (both operands K-major)
-template <int BN>
+// 64 x BN fp32 accumulator of one consumer warpgroup, issued as ONE wgmma per call.  TA / TB = 1: that operand is
+// MN-major (the weight gradient's; an MN-major B wider than 64 spans several slabs, LBO apart in its descriptor).
+template <int BN, int TA = 0, int TB = 0>
 struct TcAccWide {
   float d[BN / 2];
 
@@ -147,16 +92,17 @@ struct TcAccWide {
     for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
   }
   __device__ __forceinline__ void hold() { wg_hold(d); }
+  // scale_d = 0: D = A * B (the accumulator's previous contents are dropped)
   __device__ __forceinline__ void mma(uint64_t a, uint64_t b, int scale_d) {
     static_assert(BN == 32 || BN == 48 || BN == 64 || BN == 96 || BN == 104 || BN == 112 || BN == 128,
                   "no wgmma wrapper for this tile width");
-    if constexpr (BN == 32) wg_mma_n32<0, 0>(d, a, b, scale_d);
-    if constexpr (BN == 48) wg_mma_n48<0, 0>(d, a, b, scale_d);
-    if constexpr (BN == 64) wg_mma_n64<0, 0>(d, a, b, scale_d);
-    if constexpr (BN == 96) wg_mma_n96<0, 0>(d, a, b, scale_d);
-    if constexpr (BN == 104) wg_mma_n104<0, 0>(d, a, b, scale_d);
-    if constexpr (BN == 112) wg_mma_n112<0, 0>(d, a, b, scale_d);
-    if constexpr (BN == 128) wg_mma_n128<0, 0>(d, a, b, scale_d);
+    if constexpr (BN == 32) wg_mma_n32<TA, TB>(d, a, b, scale_d);
+    if constexpr (BN == 48) wg_mma_n48<TA, TB>(d, a, b, scale_d);
+    if constexpr (BN == 64) wg_mma_n64<TA, TB>(d, a, b, scale_d);
+    if constexpr (BN == 96) wg_mma_n96<TA, TB>(d, a, b, scale_d);
+    if constexpr (BN == 104) wg_mma_n104<TA, TB>(d, a, b, scale_d);
+    if constexpr (BN == 112) wg_mma_n112<TA, TB>(d, a, b, scale_d);
+    if constexpr (BN == 128) wg_mma_n128<TA, TB>(d, a, b, scale_d);
   }
   __device__ __forceinline__ void add(const TcAccWide& o) {
 #pragma unroll
@@ -169,6 +115,7 @@ struct TcAccWide {
 #pragma unroll
       for (int q = 0; q < 4; ++q) d[4 * i + q] += d[4 * (i + BN / 16) + q];
   }
+  // fn(column, row half h, value at column, value at column + 1) for every accumulator pair of this thread
   template <class F>
   __device__ __forceinline__ void each(int lane, F&& fn) const {
     const int c2 = 2 * (lane & 3);
@@ -449,8 +396,12 @@ int launch_tc_bn(int bn, bool stacked, int stk_rows, const CUtensorMap& ah, cons
 // stack of "slabs" (64 channels x 64 pixels = 64 rows of 128 bytes, lbo = 8192 apart; 8-row groups sbo = 1024
 // apart); one 5-D TMA box (64 channels-in-slab, w, h, n, slab) fills all slabs of an operand, the tap shift is a
 // plain coordinate offset with out-of-bounds zero fill.  One MMA consumes 16 pixel rows (K = 16); consumer
-// warpgroup cg multiplies slab cg of the G operand (64 output channels).
-// Grid: (co tiles x ci tiles, taps, pixel splits); partial sums meet in a fixed order (wgrad_sum_kernel).
+// warpgroup cg multiplies slab cg of the G operand (64 output channels) by the whole BNW-wide X operand, one wgmma
+// per product and k-step.  A ci tile starts at any multiple of 8 channels (citile * BNW): the X map's channel
+// dimension is the whole pixel vector, the slab dimension steps 64 channels on from the tile's first one.  A
+// warpgroup whose G slab lies wholly past Kp issues nothing (it only releases the stages).  TAPS = 2: two entries
+// with the same G image offset share the CTA and its G tile, one accumulator each.
+// Grid: (co tiles x ci tiles, entries / TAPS, pixel splits); partial sums meet in a fixed order (wgrad_sum_kernel).
 // ------------------------------------------------------------------------------------------------
 struct TcWgradParams {
   int N, OH, OW;        // pixel grid of G
@@ -460,6 +411,7 @@ struct TcWgradParams {
   int chunks_per_cta;
   int Kp, C;            // rows (co) and columns (ci) of each dW[t]
   int cotiles;          // blockIdx.x = citile * cotiles + cotile
+  int nentries;         // blockIdx.y = group of TAPS consecutive entries sharing one G tile
   float* dw;            // [ntaps_out][Kp][C]; or, when work is set, work[(z * nentries + e) * Kp * C] per (split, entry)
   float* work;
   const unsigned* amax_g; // operand scales (see TcParams)
@@ -471,29 +423,30 @@ struct TcWgradParams {
 constexpr int WG_PIX = 64;                     // pixels per stage (4 MMA k-steps of 16)
 constexpr int WG_CH = 64;                      // channels per slab = one 128-byte row
 constexpr uint32_t WG_SLAB = WG_PIX * 128;     // bytes of one slab: 64 pixels x 64 channels
-static_assert(WG_SLAB == TC_NBLK_BYTES, "a 64-wide column block of the MN-major B operand is one slab");
 
 __device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr) { return wg_desc(saddr, WG_SLAB, 1024); }
 
-template <int BNW, int STAGES, int NSPLIT>
+template <int BNW, int STAGES, int NSPLIT, int TAPS>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap map_gh, const __grid_constant__ CUtensorMap map_gl,
-                     const __grid_constant__ CUtensorMap map_xh, const __grid_constant__ CUtensorMap map_xl,
-                     const TcWgradParams p) {
+conv_tc_wgrad_wide_kernel(const __grid_constant__ CUtensorMap map_gh, const __grid_constant__ CUtensorMap map_gl,
+                          const __grid_constant__ CUtensorMap map_xh, const __grid_constant__ CUtensorMap map_xl,
+                          const TcWgradParams p) {
   constexpr int NSB = (BNW + WG_CH - 1) / WG_CH;          // slabs of the X operand
   constexpr uint32_t A_BYTES = 2 * WG_SLAB;               // 128 co = 2 slabs = 16 KB
   constexpr uint32_t B_BYTES = NSB * WG_SLAB;
-  constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
+  constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + TAPS * 2 * B_BYTES;   // G hi, G lo, then X hi, X lo per entry
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
   const int warp = tc_warp_uniform(), lane = threadIdx.x & 31;
-  const int cotile = blockIdx.x % p.cotiles, citile = blockIdx.x / p.cotiles, tap = blockIdx.y;
+  const int cotile = blockIdx.x % p.cotiles, citile = blockIdx.x / p.cotiles;
+  const int e0 = blockIdx.y * TAPS;                       // this CTA's entries: e0 .. e0 + ne - 1
+  const int ne = min(TAPS, p.nentries - e0);
   const int ch_beg = blockIdx.z * p.chunks_per_cta;
   const int ch_end = min(p.total_chunks, ch_beg + p.chunks_per_cta);
   const int nk = ch_end - ch_beg;
-  constexpr uint32_t tx_bytes = (NSPLIT == 3) ? STAGE_BYTES : (A_BYTES + B_BYTES);
+  const uint32_t tx_bytes = (NSPLIT == 3) ? 2 * A_BYTES + ne * 2 * B_BYTES : A_BYTES + ne * B_BYTES;
   if (nk <= 0) return;
 
   if (threadIdx.x == 0) {
@@ -511,8 +464,8 @@ conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap map_gh, const __grid_co
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      const int gdn = p.gdn[tap], xdh = p.xdh[tap], xdw = p.xdw[tap], xdn = p.xdn[tap];
-      const int aslab = cotile * 2, bslab = citile * NSB;
+      const int gdn = p.gdn[e0];                          // the same for every entry of the CTA (host)
+      const int aslab = cotile * 2, ci0 = citile * BNW;
       for (int it = 0; it < nk; ++it) {
         const int ch = ch_beg + it;
         const int wc = ch % p.wchunks;
@@ -523,10 +476,13 @@ conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap map_gh, const __grid_co
         uint8_t* sa = smem + (size_t)stage * STAGE_BYTES;
         mbar_expect_tx(&full_bar[stage], tx_bytes);
         tma_load_5d(sa, &map_gh, &full_bar[stage], 0, w0, h, n + gdn, aslab);
-        tma_load_5d(sa + 2 * A_BYTES, &map_xh, &full_bar[stage], 0, w0 + xdw, h + xdh, n + xdn, bslab);
-        if (NSPLIT == 3) {
-          tma_load_5d(sa + A_BYTES, &map_gl, &full_bar[stage], 0, w0, h, n + gdn, aslab);
-          tma_load_5d(sa + 2 * A_BYTES + B_BYTES, &map_xl, &full_bar[stage], 0, w0 + xdw, h + xdh, n + xdn, bslab);
+        if (NSPLIT == 3) tma_load_5d(sa + A_BYTES, &map_gl, &full_bar[stage], 0, w0, h, n + gdn, aslab);
+        for (int t = 0; t < ne; ++t) {
+          const int e = e0 + t;
+          const int xw = w0 + p.xdw[e], xh = h + p.xdh[e], xn = n + p.xdn[e];
+          uint8_t* sb = sa + 2 * A_BYTES + t * 2 * B_BYTES;
+          tma_load_5d(sb, &map_xh, &full_bar[stage], ci0, xw, xh, xn, 0);
+          if (NSPLIT == 3) tma_load_5d(sb + B_BYTES, &map_xl, &full_bar[stage], ci0, xw, xh, xn, 0);
         }
         if (++stage == STAGES) {
           stage = 0;
@@ -538,8 +494,24 @@ conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap map_gh, const __grid_co
   }
 
   const int cg = (warp >> 2) - 1;
-  TcAcc<BNW, 1, 1> acc, part;            // per-stage partial sums, as in conv_tc_kernel
-  acc.zero();
+  if ((cotile * 2 + cg) * WG_CH >= p.Kp) {   // G slab past the last row: zero-filled, no product to issue
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int it = 0; it < nk; ++it) {
+      mbar_wait(&full_bar[stage], phase);
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    return;
+  }
+  // per-stage partial sums, as in conv_tc_kernel; one accumulator per entry, each entry's stages in the same order
+  // as with one entry per CTA
+  TcAccWide<BNW, 1, 1> acc[TAPS], part;
+#pragma unroll
+  for (int t = 0; t < TAPS; ++t) acc[t].zero();
   {
     int stage = 0;
     uint32_t phase = 0;
@@ -547,10 +519,18 @@ conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap map_gh, const __grid_co
       mbar_wait(&full_bar[stage], phase);
       const uint32_t sa = smem_u32(smem + (size_t)stage * STAGE_BYTES);
       const uint64_t ah = make_desc_mn(sa + cg * WG_SLAB), al = make_desc_mn(sa + A_BYTES + cg * WG_SLAB);
-      const uint64_t bh = make_desc_mn(sa + 2 * A_BYTES), bl = make_desc_mn(sa + 2 * A_BYTES + B_BYTES);
-      tc_stage_mma<WG_PIX / 16, 16 * 128, NSPLIT, false>(part, ah, al, bh, bl);   // a k-step = 16 pixel rows
-      if (lane == 0) mbar_arrive(&empty_bar[stage]);
-      acc.add(part);
+      const uint32_t sb = sa + 2 * A_BYTES;
+      tc_stage_mma<WG_PIX / 16, 16 * 128, NSPLIT, false>(part, ah, al, make_desc_mn(sb), make_desc_mn(sb + B_BYTES));
+      acc[0].add(part);
+      if constexpr (TAPS == 2) {
+        if (ne == 2) {
+          const uint32_t sb1 = sb + 2 * B_BYTES;
+          tc_stage_mma<WG_PIX / 16, 16 * 128, NSPLIT, false>(part, ah, al, make_desc_mn(sb1),
+                                                             make_desc_mn(sb1 + B_BYTES));
+          acc[1].add(part);
+        }
+      }
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);     // this stage's MMAs have completed: free its slot
       if (++stage == STAGES) {
         stage = 0;
         phase ^= 1;
@@ -561,12 +541,18 @@ conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap map_gh, const __grid_co
   const int co0 = cotile * TC_BM + cg * 64 + (warp & 3) * 16 + (lane >> 2);
   const int cleft = p.C - citile * BNW;          // a multiple of 8: the pair (c, c + 1) is in or out together
   const TcScale sc = tc_scale(p.amax_g, p.amax_x);
-  acc.each(lane, [&](int c, int h, float v0, float v1) {
-    const int co = co0 + 8 * h;
-    if (co >= p.Kp || c >= cleft) return;
-    float* base = p.work ? p.work + ((long long)blockIdx.z * gridDim.y + tap) * p.Kp * p.C : p.dw + (long long)p.out[tap] * p.Kp * p.C;
-    *reinterpret_cast<float2*>(base + (long long)co * p.C + citile * BNW + c) = make_float2(v0 * sc.fa * sc.fb, v1 * sc.fa * sc.fb);
-  });
+#pragma unroll
+  for (int t = 0; t < TAPS; ++t) {
+    if (t >= ne) break;
+    const int e = e0 + t;
+    float* base = p.work ? p.work + ((long long)blockIdx.z * p.nentries + e) * p.Kp * p.C
+                         : p.dw + (long long)p.out[e] * p.Kp * p.C;
+    acc[t].each(lane, [&](int c, int h, float v0, float v1) {
+      const int co = co0 + 8 * h;
+      if (co >= p.Kp || c >= cleft) return;
+      *reinterpret_cast<float2*>(base + (long long)co * p.C + citile * BNW + c) = make_float2(v0 * sc.fa * sc.fb, v1 * sc.fa * sc.fb);
+    });
+  }
 }
 
 // dw[t][j] = sum over the entries e with out[e] == t, then over the splits z, of work[(z * nentries + e) * plane + j]
@@ -588,32 +574,49 @@ __global__ void __launch_bounds__(256) wgrad_sum_kernel(const float* __restrict_
   }
 }
 
-template <int BNW, int NSPLIT>
+template <int BNW, int NSPLIT, int TAPS>
 int launch_wgrad(const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap& xh, const CUtensorMap& xl,
                  const TcWgradParams& p, dim3 grid, cudaStream_t stream) {
-  constexpr size_t stage = 2 * 2 * WG_SLAB + 2 * ((BNW + WG_CH - 1) / WG_CH) * WG_SLAB;
+  constexpr size_t stage = 2 * 2 * WG_SLAB + TAPS * 2 * ((BNW + WG_CH - 1) / WG_CH) * WG_SLAB;
   constexpr int STAGES = tc_stages(stage);
   constexpr size_t smem = (size_t)STAGES * stage + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_wgrad_kernel<BNW, STAGES, NSPLIT>,
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_wgrad_wide_kernel<BNW, STAGES, NSPLIT, TAPS>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     configured = true;
   }
-  conv_tc_wgrad_kernel<BNW, STAGES, NSPLIT><<<grid, TC_THREADS, smem, stream>>>(gh, gl, xh, xl, p);
+  conv_tc_wgrad_wide_kernel<BNW, STAGES, NSPLIT, TAPS><<<grid, TC_THREADS, smem, stream>>>(gh, gl, xh, xl, p);
   return (int)cudaGetLastError();
 }
 
+// widths up to 104 take two entries per CTA (three accumulator sets of BNW / 2 registers fit the 168 of a thread)
+constexpr int WG_PAIR_MAX_BN = 104;
+
 template <int NSPLIT>
-int launch_wgrad_bn(int bn, const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap& xh,
+int launch_wgrad_bn(int bn, bool pair, const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap& xh,
                     const CUtensorMap& xl, const TcWgradParams& p, dim3 grid, cudaStream_t stream) {
   switch (bn) {
-    case 32:  return launch_wgrad<32, NSPLIT>(gh, gl, xh, xl, p, grid, stream);
-    case 64:  return launch_wgrad<64, NSPLIT>(gh, gl, xh, xl, p, grid, stream);
-    case 112: return launch_wgrad<112, NSPLIT>(gh, gl, xh, xl, p, grid, stream);
-    default:  return launch_wgrad<128, NSPLIT>(gh, gl, xh, xl, p, grid, stream);
+    case 32:  return pair ? launch_wgrad<32, NSPLIT, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<32, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 48:  return pair ? launch_wgrad<48, NSPLIT, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<48, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 64:  return pair ? launch_wgrad<64, NSPLIT, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<64, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 96:  return pair ? launch_wgrad<96, NSPLIT, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<96, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 104: return pair ? launch_wgrad<104, NSPLIT, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<104, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 112: return launch_wgrad<112, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 128: return launch_wgrad<128, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
+    default:  return (int)cudaErrorInvalidValue;
   }
+}
+
+// ci tile: as the forward's N tile (og_conv2d_tc), the smallest number of equal tiles of <= 128 columns, rounded up
+// to the wgmma N step of 8, then to the next instantiated width
+int tc_fit_width(int cols) {
+  const int ntile = og_cdiv(cols, 128);
+  const int bn8 = (og_cdiv(cols, ntile) + 7) / 8 * 8;
+  for (int b : TC_BN_SET)
+    if (b >= bn8) return b;
+  return 128;
 }
 
 }  // namespace
@@ -673,14 +676,7 @@ OG_API int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, 
   // N tile: whole K if it fits 128 columns (a consumer thread holds two sets of BN / 2 accumulators), else the
   // smallest number of equal tiles; the width is rounded up to the wgmma N step of 8, then to the next instantiated
   // width.  An output element's k-sum does not depend on the tile width, so neither do the results.
-  const int ntile = og_cdiv(K, 128);
-  const int bn8 = (og_cdiv(K, ntile) + 7) / 8 * 8;
-  int BNsel = 128;
-  for (int b : TC_BN_SET)
-    if (b >= bn8) {
-      BNsel = b;
-      break;
-    }
+  const int BNsel = tc_fit_width(K);
   dim3 grid(tiles_n * p.tiles_h * p.tiles_w, og_cdiv(K, BNsel), 1);
   // few output tiles (small feature maps): split the reduction over gridDim.z (about two CTAs per SM in all); the
   // slices' partial outputs are summed in a fixed order afterwards (og_split_sum)
@@ -778,12 +774,13 @@ OG_API int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* am
     p.out[i] = entries_host[5 * i + 4];
   }
   const int cotiles = og_cdiv(Kp, TC_BM);
-  const int Cr = (C + 15) / 16 * 16;
-  const int BNsel = Cr <= 32 ? 32 : Cr <= 64 ? 64 : Cr <= 112 ? 112 : 128;
-  const int citiles = og_cdiv(C, BNsel);
+  const int BNsel = tc_fit_width(C);      // C = 200: 2 x 104 columns
+  const int citiles = og_cdiv(C, BNsel);  // = ceil(C / 128), as many as 128-wide tiles would take
   p.cotiles = cotiles;
   // pixel splits: the CTAs are equal-sized and run one per SM, so fill at most two full waves (one CTA more would
-  // cost a whole extra round); at least 8 chunks per CTA
+  // cost a whole extra round); at least 8 chunks per CTA.  The count depends on the number of tiles and entries only,
+  // not on the tile width or on how many entries a CTA shares, and an element's k-sum has the same stages and order
+  // in every form: results do not depend on BNsel or on the entry pairing below
   int splits = 2 * og_num_sms() / (cotiles * citiles * nentries);
   if (splits < 1) splits = 1;
   int maxs = p.total_chunks / 8;
@@ -791,7 +788,23 @@ OG_API int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* am
   if (splits > maxs) splits = maxs;
   p.chunks_per_cta = og_cdiv(p.total_chunks, splits);
   splits = og_cdiv(p.total_chunks, p.chunks_per_cta);
-  dim3 grid(cotiles * citiles, nentries, splits);
+  // entries 2j and 2j + 1 share one CTA when they read the same G tile (equal image offset: every entry of a stride-1
+  // or space-to-depth layer, the two column taps of an upsample phase): G is loaded once for both, a stage moves
+  // 96 KB instead of 2 x 64 KB at BNW = 104.  The kernel is bound by those bytes, so pair only where
+  // (waves) x (bytes per stage) drops: res-block conv1, 216 CTAs in 2 waves -> 120 in 1; not conv2 (252 -> 140, 2 waves)
+  bool pair = BNsel <= WG_PAIR_MAX_BN && nentries > 1;
+  for (int e = 0; e + 1 < nentries; e += 2) pair &= p.gdn[e] == p.gdn[e + 1];
+  // OG_WGRAD_PAIR=0 / 1: never / always pair where the entries allow it (the results are the same)
+  const char* pair_env = getenv("OG_WGRAD_PAIR");
+  if (pair_env && atoi(pair_env) == 0) pair = false;
+  if (pair && !pair_env) {
+    const int nsb = og_cdiv(BNsel, WG_CH), sms = og_num_sms();
+    const long long waves1 = og_cdiv((long long)cotiles * citiles * nentries * splits, sms);
+    const long long waves2 = og_cdiv((long long)cotiles * citiles * og_cdiv(nentries, 2) * splits, sms);
+    pair = waves2 * (4 + 4 * nsb) < waves1 * (4 + 2 * nsb);   // G: 2 slabs, X: nsb slabs per entry (hi and lo alike)
+  }
+  p.nentries = nentries;
+  dim3 grid(cotiles * citiles, pair ? og_cdiv(nentries, 2) : nentries, splits);
   CUtensorMap mgh, mgl, mxh, mxl;
   // [slab][n][h][w][64 channels of the slab]: the slab dimension strides by 64 halves inside a pixel's channel vector
   unsigned long long gd[5] = {(unsigned long long)WG_CH, (unsigned long long)OW, (unsigned long long)OH,
@@ -799,11 +812,15 @@ OG_API int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* am
   unsigned long long gs[4] = {(unsigned long long)Kp, (unsigned long long)OW * Kp, (unsigned long long)OH * OW * Kp,
                               (unsigned long long)WG_CH};
   unsigned gb[5] = {(unsigned)WG_CH, (unsigned)cw, (unsigned)chh, (unsigned)cn, 2u};
-  unsigned long long xd[5] = {(unsigned long long)WG_CH, (unsigned long long)SW, (unsigned long long)SH,
-                              (unsigned long long)XN, (unsigned long long)og_cdiv(C, WG_CH)};
+  // X: [slab of the tile][n][h][w][channel of the whole pixel vector]; a tile's box starts at channel citile * BNsel
+  // and its slab s holds channels from there + 64 s (those >= C are never stored: zero-filled in the first slab,
+  // read from the next pixel -- or the readable bytes after the tensor -- in the others)
+  const int xslabs = (BNsel + WG_CH - 1) / WG_CH;
+  unsigned long long xd[5] = {(unsigned long long)C, (unsigned long long)SW, (unsigned long long)SH,
+                              (unsigned long long)XN, (unsigned long long)xslabs};
   unsigned long long xs[4] = {(unsigned long long)C, (unsigned long long)SW * C, (unsigned long long)SH * SW * C,
                               (unsigned long long)WG_CH};
-  unsigned xb[5] = {(unsigned)WG_CH, (unsigned)cw, (unsigned)chh, (unsigned)cn, (unsigned)((BNsel + WG_CH - 1) / WG_CH)};
+  unsigned xb[5] = {(unsigned)WG_CH, (unsigned)cw, (unsigned)chh, (unsigned)cn, (unsigned)xslabs};
   int rc;
   if ((rc = make_map(&mgh, gh, 5, gd, gs, gb))) return rc;
   if ((rc = make_map(&mxh, xh, 5, xd, xs, xb))) return rc;
@@ -822,8 +839,8 @@ OG_API int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* am
   p.work = nullptr;
   const long long plane = (long long)Kp * C;
   if (shared_out) OG_CHECK(og_work_alloc(&p.work, (size_t)splits * nentries * plane, stream));
-  rc = nsplit == 3 ? launch_wgrad_bn<3>(BNsel, mgh, mgl, mxh, mxl, p, grid, stream)
-                   : launch_wgrad_bn<1>(BNsel, mgh, mgl, mxh, mxl, p, grid, stream);
+  rc = nsplit == 3 ? launch_wgrad_bn<3>(BNsel, pair, mgh, mgl, mxh, mxl, p, grid, stream)
+                   : launch_wgrad_bn<1>(BNsel, pair, mgh, mgl, mxh, mxl, p, grid, stream);
   if (shared_out) {
     if (!rc) {
       WgradSum ws;
