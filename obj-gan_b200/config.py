@@ -1,6 +1,6 @@
 """Configuration object with the same shape as the reference's global ``cfg``
-(reference: image_generation/miscc/config.py:9-87).  Only the keys the hot path reads
-are kept; values are the reference defaults except TEXT.WORDS_NUM, which BASELINE.json
+(reference: image_generation/miscc/config.py:9-87).  Only the keys the hot path and the
+training loop read are kept; values are the reference defaults except TEXT.WORDS_NUM, which BASELINE.json
 fixes at 18 tokens."""
 
 
@@ -25,6 +25,10 @@ def default_cfg():
     c.TREE = AttrDict(BRANCH_NUM=3, BASE_SIZE=64)
     c.TRAIN = AttrDict(
         BATCH_SIZE=16, DISCRIMINATOR_LR=2e-4, GENERATOR_LR=2e-4, BUATTN_NORM=True,
+        # the training loop (trainer.condGANTrainer): epochs, snapshot / log intervals, the pretrained DAMSM text
+        # encoder (the image encoder is the same path with text_encoder -> image_encoder) and a generator to resume
+        MAX_EPOCH=60, SNAPSHOT_INTERVAL=1, PRINT_INTERVAL=100, DISPLAY_INTERVAL=500, FLAG=True,
+        NET_E="/pretrained/text_encoder100.pth", NET_G="",
         SMOOTH=AttrDict(GAMMA1=4.0, GAMMA2=5.0, GAMMA3=10.0, DAMSM_LAMBDA=100.0,
                         TXT_LAMBDA=0.1, SHP_LAMBDA=1.0, OBJ_LAMBDA=0.1, UNCOND_LAMBDA=1.0))
     c.GAN = AttrDict(DF_DIM=96, GF_DIM=48, Z_DIM=100, CONDITION_DIM=100, R_NUM=1,

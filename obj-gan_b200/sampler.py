@@ -39,7 +39,7 @@ from . import lib as _lib
 from . import model, ops
 from .config import cfg
 from .synth import IMG_SIZES
-from .trainer import prepare_data
+from .trainer import prepare_data, text_stage
 
 NOISE_BOX = ops.BOX_NOISE
 
@@ -384,10 +384,8 @@ class GSampler:
 
     def _text(self, dev: dict) -> dict:
         """captions -> RNN_ENCODER (words_embs, sent_emb), GloVe lookups and mask (ref: evaluator.py:337-351)."""
-        n = dev["max_len"]
-        words, sent = self.text_encoder(dev["captions"], dev["cap_lens"], n)
-        glove_words, mask = ops.text_inputs(dev["captions"], dev["glove_captions"], self.glove, n)
-        return dict(words_embs=words, sent_emb=sent, mask=mask, glove_words_embs=glove_words)
+        return text_stage(self.text_encoder, self.glove, dev["captions"], dev["cap_lens"], dev["glove_captions"],
+                          dev["max_len"])
 
     def _shapes(self, dev: dict) -> dict:
         """Box maps -> SHP_G_NET -> form_hmaps (ref: evaluator.py:315-328): the raw masks (B, R, 64, 64) and the heat

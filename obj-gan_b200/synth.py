@@ -159,3 +159,59 @@ def shard(inp: dict, rank: int, world: int) -> dict:
     out["glb_max_num_roi"] = rmax
     out["slabels_feat"] = out["slabels_feat"][:, :, :rmax].contiguous()
     return out
+
+
+def reference_batch(batch: int, seed: int = 1234, *, lens=None, parity: bool = True, max_rois: int | None = None,
+                    n_words: int = 200, n_glove: int = 200, num_classes: int = 80):
+    """One batch in the format the reference's DataLoader collates from ``TrainDataset.__getitem__`` (ref:
+    trainDataset.py:56-74, miscc/load.py:112-191): (imgs, captions (B, 18, 1) int64, glove_captions (B, 18, 1),
+    cap_lens (B,) UNSORTED, hmaps (float64 per-class sums of the masks, unclamped), rois, fm_rois, num_rois, bt_masks
+    and fm_bt_masks (float64), class_ids (B,), keys (B strings)).  The boxes, masks and images are ``make_inputs``'s
+    (``parity``: ragged roi counts); ``lens``: the caption lengths (default: seeded draws in [5, 18]); token ids are
+    drawn in [1, n_words) / [1, n_glove) on the first cap_lens[b] positions and 0 after."""
+    inp = make_inputs(batch, seed, parity=parity, max_rois=max_rois, num_classes=num_classes)
+    g = torch.Generator().manual_seed(seed + 1)
+    L = cfg.TEXT.WORDS_NUM
+    lens = torch.randint(5, L + 1, (batch,), generator=g) if lens is None else torch.as_tensor(lens, dtype=torch.int64)
+    pos = torch.arange(L).view(1, L) < lens.view(-1, 1)
+    caps = (torch.randint(1, n_words, (batch, L), generator=g) * pos).view(batch, L, 1)
+    gcaps = (torch.randint(1, n_glove, (batch, L), generator=g) * pos).view(batch, L, 1)
+    cls = inp["rois"][0][..., 4].long()
+    hmaps = []
+    for m in inp["bt_masks"]:
+        s = m.shape[-1]
+        hm = torch.zeros(batch, num_classes, s, s, dtype=torch.float64)
+        hmaps.append(hm.scatter_add_(1, cls.view(batch, -1, 1, 1).expand(-1, -1, s, s), m.double()))
+    class_ids = torch.randint(0, 100000, (batch,), generator=g)
+    keys = [f"COCO_train2014_{seed:06d}{i:06d}" for i in range(batch)]
+    return (inp["imgs"], caps, gcaps, lens, hmaps, inp["rois"], inp["fm_rois"], inp["num_rois"],
+            [m.double() for m in inp["bt_masks"]], inp["fm_bt_masks"].double(), class_ids, keys)
+
+
+def reference_dataset(n_words: int = 200, n_glove: int = 200, num_classes: int = 80, seed: int = 0):
+    """An object with the attributes the reference's condGANTrainer reads from its ``TrainDataset`` (n_words,
+    cats_index_dict, cat_labels, cat_label_lens, sorted_cat_label_indices, glove_embed), seeded: labels of one or
+    two GloVe tokens, sorted by length as load_cat_label does (ref: miscc/load.py:305-355)."""
+    import types
+    g = torch.Generator().manual_seed(seed)
+    lens = torch.randint(1, 3, (num_classes,), generator=g)
+    order = torch.sort(lens, stable=True).indices
+    labels = torch.randint(1, n_glove, (num_classes, 2), generator=g) * (torch.arange(2).view(1, 2) < lens.view(-1, 1))
+    glove = torch.nn.Embedding(n_glove, cfg.TEXT.GLOVE_EMBEDDING_DIM)
+    with torch.no_grad():
+        glove.weight.copy_(0.5 * torch.randn(n_glove, cfg.TEXT.GLOVE_EMBEDDING_DIM, generator=g))
+    return types.SimpleNamespace(n_words=n_words, cats_index_dict={i: i for i in range(num_classes)},
+                                 cat_labels=labels[order], cat_label_lens=lens[order],
+                                 sorted_cat_label_indices=torch.argsort(order), glove_embed=glove)
+
+
+def reference_encoders(directory: str, n_words: int = 200, seed: int = 0) -> str:
+    """Writes seeded DAMSM encoder snapshots in the reference's layout, ``text_encoder100.pth`` and
+    ``image_encoder100.pth``, to ``directory``; returns the text encoder's path (what cfg.TRAIN.NET_E names)."""
+    import os
+    from . import model
+    torch.manual_seed(seed)
+    torch.save(model.RNN_ENCODER(n_words, nhidden=cfg.TEXT.EMBEDDING_DIM).state_dict(),
+               os.path.join(directory, "text_encoder100.pth"))
+    torch.save(model.CNN_ENCODER(cfg.TEXT.EMBEDDING_DIM).state_dict(), os.path.join(directory, "image_encoder100.pth"))
+    return os.path.join(directory, "text_encoder100.pth")

@@ -14,6 +14,7 @@ from __future__ import annotations
 
 import contextlib
 import os
+import time
 
 import torch
 import torch.distributed as dist
@@ -48,6 +49,63 @@ def prepare_data(dev: dict, num_classes: int | None = None, into: dict | None = 
                                out=(into["slabels_feat"] if into is not None and "slabels_feat" in into else None))
     dst["hmaps"], dst["slabels_feat"] = hm, sl
     return dst
+
+
+def text_stage(text_encoder, glove, captions, cap_lens, glove_captions, max_len: int) -> dict:
+    """The frozen text side of a caption batch (ref: trainer.py:365-380, evaluator.py:337-351): RNN_ENCODER ->
+    (words_embs (B, 256, max_len), sent_emb (B, 256)), then the GloVe lookups and padding mask (glove_words_embs
+    (B, 50, max_len), mask (B, max_len) bool).  ``captions`` / ``cap_lens`` / ``glove_captions`` are int64 device
+    tensors, ``glove`` the (V, 50) table on the device, ``max_len`` = max(cap_lens) as a host int.  The sampler and the
+    training loop both call this."""
+    words, sent = text_encoder(captions, cap_lens, max_len)
+    glove_words, mask = ops.text_inputs(captions, glove_captions, glove, max_len)
+    return dict(words_embs=words, sent_emb=sent, mask=mask, glove_words_embs=glove_words)
+
+
+def prepare_reference_batch(data):
+    """The reference's ``prepare_data`` (ref: trainDataset.py:79-128) on the host, producing the compact batch that
+    ``StepATrainer.to_device`` takes.  ``data`` is what the reference's DataLoader collates from
+    ``TrainDataset.__getitem__``: (imgs, captions, glove_captions, cap_lens, hmaps, rois, fm_rois, num_rois, bt_masks,
+    fm_bt_masks, class_ids, keys).
+
+    Every per-sample tensor is reordered by caption length, longest first.  The sort is stable: samples with equal
+    lengths keep their loader order (the reference's ``torch.sort(cap_lens, 0, True)`` leaves that order unspecified).
+    The masks become float32 like the reference's ``.float()`` calls; the box tables keep their float64, as there.
+    The loader's float64 ``hmaps`` are not read: ``to_device`` rebuilds them on the device from the masks and the roi
+    classes (column 4 of ``rois[0]``), unclamped like the loader's sums (``hmap_clamp`` 0).  The outputs are pinned
+    when CUDA is available, so the copies to the device do not block the host.
+
+    Returns (batch, class_ids, keys): the batch dict (with ``max_len`` = max(cap_lens) and ``host_boxes``, the box
+    tables the step reads on the host), the class ids as a numpy array and the keys as a list, both in the sorted
+    order."""
+    imgs, captions, glove_captions, cap_lens, _hmaps, rois, fm_rois, num_rois, bt_masks, fm_bt_masks, class_ids, \
+        keys = data
+    cap_lens = torch.as_tensor(cap_lens).to(torch.int64).view(-1)
+    b = cap_lens.shape[0]
+    order = torch.sort(cap_lens, dim=0, descending=True, stable=True).indices
+    pin = torch.cuda.is_available()          # a copy from pageable memory blocks the host until the GPU drains
+    idx = order.tolist()
+
+    def take(t, dtype=None):
+        t = torch.as_tensor(t)
+        out = torch.empty(t.shape, dtype=dtype or t.dtype, pin_memory=pin)
+        if out.dtype == t.dtype:
+            return torch.index_select(t, 0, order, out=out)
+        for j, i in enumerate(idx):          # gather and convert in one pass (the float64 masks: ~110 MB at batch 16)
+            out[j].copy_(t[i])
+        return out
+
+    rois = [take(r) for r in rois]
+    roi_cls = torch.empty(rois[0].shape[:2], dtype=torch.int64, pin_memory=pin).copy_(rois[0][..., 4])
+    batch = dict(imgs=[take(x) for x in imgs], captions=take(torch.as_tensor(captions).reshape(b, -1)),
+                 glove_captions=take(torch.as_tensor(glove_captions).reshape(b, -1)), cap_lens=take(cap_lens),
+                 rois=rois, fm_rois=take(fm_rois), num_rois=take(torch.as_tensor(num_rois).to(torch.int64).view(-1)),
+                 bt_masks=[take(m, torch.float32) for m in bt_masks], fm_bt_masks=take(fm_bt_masks, torch.float32),
+                 roi_cls=roi_cls, hmap_clamp=0.0)
+    batch["glb_max_num_roi"] = int(batch["num_rois"].max())
+    batch["max_len"] = int(cap_lens.max())
+    batch["host_boxes"] = {"rois": rois, "fm_rois": batch["fm_rois"], "num_rois": batch["num_rois"]}
+    return batch, torch.as_tensor(class_ids)[order].numpy(), [keys[i] for i in idx]
 
 
 class FlatBucket:
@@ -551,3 +609,194 @@ class StepBTrainer(StepATrainer):
         self.bG.adam(lr_g, gs)
         out.update(errG=err_g.detach(), kl=kl.detach(), logs=logs, fake_imgs=[f.detach() for f in fake_imgs])
         return out
+
+
+class condGANTrainer:
+    """The reference's training loop (ref: trainer.py:30-511, ``condGANTrainer``) on this library: the same constructor
+    and ``train()``, fed by the reference's own DataLoader.  Each step runs the intake (``prepare_reference_batch``),
+    the copies to the device and the heat-map rebuild, the frozen text encoder (``text_stage``), the complete step
+    (``StepBTrainer.step``, DAMSM terms included) and INCEPTION_V3 on the 256-pixel images; the predictions stay on the
+    device until the end of the epoch, when ``Score/scores_%d.txt`` is written in the reference's format.  Snapshots
+    are the reference's file set (``StepBTrainer.save_model``) under ``Model/``; ``cfg.TRAIN.NET_G`` resumes.
+
+    ``dataset`` provides what the reference reads from it: ``n_words``, ``cats_index_dict``, ``cat_labels``,
+    ``cat_label_lens``, ``sorted_cat_label_indices`` and ``glove_embed``.  ``inception_weights``: torchvision's
+    ImageNet file (``inception_v3_google-1a9a5a14.pth``, its path or its loaded state_dict) for INCEPTION_V3; the
+    reference downloads it, this library reads no network.
+
+    Under torchrun (one process per GPU, each with its own shard of the data): every rank trains on its own batches
+    and the ranks exchange gradients through ``process_group``; the epoch's Inception score covers every rank's
+    predictions, gathered to rank 0 once per epoch, and only rank 0 prints and writes files.
+
+    Not produced: the attention-map PNGs the reference saves every DISPLAY_INTERVAL steps (``save_img_results``);
+    ``Image/`` is created for the reference's directory layout and stays empty."""
+
+    def __init__(self, output_dir, data_loader, dataset, *, inception_weights, device=None, process_group=None):
+        self.pg = process_group
+        self.world = dist.get_world_size(process_group) if (dist.is_available() and dist.is_initialized()) else 1
+        self.rank = dist.get_rank(process_group) if self.world > 1 else 0
+        self.model_dir = os.path.join(output_dir, "Model")
+        self.image_dir = os.path.join(output_dir, "Image")
+        self.score_dir = os.path.join(output_dir, "Score")
+        if cfg.TRAIN.FLAG and self.rank == 0:
+            for d in (self.model_dir, self.image_dir, self.score_dir):
+                os.makedirs(d, exist_ok=True)
+        self.batch_size = cfg.TRAIN.BATCH_SIZE
+        self.max_epoch = cfg.TRAIN.MAX_EPOCH
+        self.snapshot_interval = cfg.TRAIN.SNAPSHOT_INTERVAL
+        self.print_interval = cfg.TRAIN.PRINT_INTERVAL
+        self.display_interval = cfg.TRAIN.DISPLAY_INTERVAL
+        self.n_words = dataset.n_words
+        self.cats_index_dict = dataset.cats_index_dict
+        self.cat_labels = dataset.cat_labels
+        self.cat_label_lens = dataset.cat_label_lens
+        self.sorted_cat_label_indices = dataset.sorted_cat_label_indices
+        self.glove_emb = dataset.glove_embed
+        self.data_loader = data_loader
+        self.num_batches = len(data_loader)
+        self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
+        self.inception_weights = inception_weights
+
+    def build_models(self):
+        """(text_encoder, image_encoder, StepBTrainer, INCEPTION_V3, start_epoch), like the reference's build_models
+        (ref: trainer.py:75-195): the DAMSM encoders from cfg.TRAIN.NET_E (the image encoder's path is NET_E with
+        ``text_encoder`` -> ``image_encoder``), fresh networks or the snapshot of cfg.TRAIN.NET_G, identical on every
+        rank."""
+        from .sampler import strip_module_prefix
+        if not cfg.TRAIN.NET_E:
+            raise ValueError("no pretrained text-image encoders: set cfg.TRAIN.NET_E")
+        dev = self.device
+        image_encoder = model.CNN_ENCODER.from_snapshot(cfg.TRAIN.NET_E.replace("text_encoder", "image_encoder"), dev,
+                                                        nef=cfg.TEXT.EMBEDDING_DIM)
+        text_encoder = model.RNN_ENCODER(self.n_words, nhidden=cfg.TEXT.EMBEDDING_DIM).to(dev)
+        text_encoder.load_state_dict(strip_module_prefix(torch.load(cfg.TRAIN.NET_E, map_location="cpu")), strict=True)
+        text_encoder.requires_grad_(False).eval()
+        net = StepBTrainer(len(self.cats_index_dict), dev, self.pg, image_encoder=image_encoder)
+        start_epoch = net.load_model(cfg.TRAIN.NET_G) if cfg.TRAIN.NET_G else 0
+        net.broadcast_parameters()
+        inception = model.INCEPTION_V3.from_imagenet(self.inception_weights, dev)
+        return text_encoder, image_encoder, net, inception, start_epoch
+
+    def prepare_cat_emb(self):
+        """(num_classes, 50) label embeddings on the device (ref: trainer.py:226-242)."""
+        as_i64 = lambda t: torch.as_tensor(t).to(self.device, torch.int64)
+        return ops.class_label_emb(self.glove, as_i64(self.cat_labels), as_i64(self.cat_label_lens),
+                                   as_i64(self.sorted_cat_label_indices))
+
+    def setup(self):
+        """Builds the networks, the GloVe table and the label embeddings; returns the epoch to start from."""
+        self.text_encoder, self.image_encoder, self.net, self.inception, start = self.build_models()
+        glove = getattr(self.glove_emb, "weight", self.glove_emb)
+        self.glove = glove.detach().to(self.device).float().contiguous()
+        self.clabels_emb = self.prepare_cat_emb()
+        return start
+
+    def train_step(self, data, score=None, z=None, eps=None) -> dict:
+        """One step of the loop body (ref: trainer.py:361-469) on one loader batch: intake, copies to the device, text stage, fresh noise (``z`` / the CA_NET
+        ``eps`` when given), the complete step, and the Inception predictions of ``fake_imgs[-1]`` added to ``score``
+        (a losses.InceptionScore).  Returns the step's outputs (device tensors) with the sorted ``class_ids``
+        and ``keys``."""
+        batch, class_ids, keys = prepare_reference_batch(data)
+        batch = dict(batch, clabels_emb=self.clabels_emb)
+        dev = self.net.to_device(batch)
+        with torch.no_grad():
+            dev.update(text_stage(self.text_encoder, self.glove, dev["captions"], dev["cap_lens"],
+                                  dev["glove_captions"], batch["max_len"]))
+        b = dev["num_rois"].shape[0]
+        dev["z"] = z if z is not None else torch.randn(b, cfg.GAN.Z_DIM, device=self.device)   # noise.normal_(0, 1)
+        if eps is not None:
+            dev["eps"] = eps
+        out = self.net.step(dev, class_ids)
+        pred = self.inception(out["fake_imgs"][-1])
+        if score is not None:
+            score.add(pred)
+        out.update(predictions=pred, class_ids=class_ids, keys=keys)
+        return out
+
+    @staticmethod
+    def host_losses(out) -> dict:
+        """The step's losses on the host, in one read (the loop reads them on print steps and at epoch ends only)."""
+        names = [k for k in out if k.startswith("err") or k == "kl"]
+        logs = list(out["logs"])
+        vals = [out[k] for k in names if out[k] is not None] + [out["logs"][k] for k in logs]
+        host = torch.stack([v.reshape(()).float() for v in vals]).tolist() if vals else []
+        it = iter(host)
+        res = {k: (next(it) if out[k] is not None else None) for k in names}
+        res["logs"] = {k: next(it) for k in logs}
+        return res
+
+    def _log(self, epoch, gen_iterations, h):
+        """The reference's per-step report (ref: trainer.py:474-476)."""
+        n = len(self.net.netsPatD)
+        pat = "".join("errPatD%d: %.2f " % (i, h[f"errPatD{i}"]) for i in range(n))
+        shp = "".join("errShpD%d: %.2f " % (i, h[f"errShpD{i}"]) for i in range(n))
+        ss = "errSSACD: %.2f " % h["errObjSSD"] if h["errObjSSD"] is not None else ""
+        ls = "errObjLSD: %.2f " % h["errObjLSD"] if h["errObjLSD"] is not None else ""
+        g = "".join("%s: %.2f " % (k, v) for k, v in h["logs"].items()) + "kl_loss: %.2f " % h["kl"]
+        print("[%d/%d][%d]" % (epoch, self.max_epoch, gen_iterations) + "\n" + pat + "\n" + shp + "\n" + ss + "\n" +
+              ls + "\n" + g)
+
+    def epoch_score(self, score):
+        """The epoch's InceptionScore over every rank's predictions: one gather to rank 0 (None on the other
+        ranks).  Rank r's predictions follow rank r-1's."""
+        if self.world == 1:
+            return score
+        local = torch.cat(score.predictions, 0)
+        n = torch.tensor([local.shape[0]], device=local.device, dtype=torch.int64)
+        counts = [torch.zeros_like(n) for _ in range(self.world)]
+        dist.all_gather(counts, n, group=self.pg)
+        counts = [int(c) for c in counts]
+        pad = local.new_zeros((max(counts), local.shape[1]))
+        pad[:local.shape[0]] = local
+        parts = [torch.empty_like(pad) for _ in range(self.world)]
+        dist.all_gather(parts, pad, group=self.pg)
+        if self.rank != 0:
+            return None
+        out = losses.InceptionScore(score.num_splits)
+        for p, c in zip(parts, counts):
+            out.add(p[:c])
+        return out
+
+    def write_score(self, epoch, score):
+        """Score/scores_%d.txt in the reference's format (ref: trainer.py:495-506)."""
+        mean, std, mean_conf, std_conf = score.result()
+        with open(os.path.join(self.score_dir, "scores_%d.txt" % epoch), "w") as fp:
+            fp.write("mean, std, mean_conf, std_conf \n")
+            fp.write("%f, %f, %f, %f" % (mean, std, mean_conf, std_conf))
+        print("inception_score: mean, std, mean_conf, std_conf")
+        print("inception_score: %f, %f, %f, %f" % (mean, std, mean_conf, std_conf))
+
+    def train(self):
+        """ref: trainer.py:331-511."""
+        start_epoch = self.setup()
+        gen_iterations = 0
+        lead = self.rank == 0
+        for epoch in range(start_epoch, self.max_epoch):
+            start_t = time.time()
+            score = losses.InceptionScore(min(10, self.batch_size))
+            data_iter = iter(self.data_loader)
+            out = None
+            for _ in range(self.num_batches):
+                out = self.train_step(next(data_iter), score)
+                gen_iterations += 1
+                if gen_iterations % self.print_interval == 0 and lead:
+                    self._log(epoch, gen_iterations, self.host_losses(out))
+            if out is None:
+                continue
+            h = self.host_losses(out)
+            end_t = time.time()
+            n = len(self.net.netsPatD)
+            zero = lambda v: 0.0 if v is None else v
+            if lead:
+                print("[%d/%d][%d]\n                  Loss_PatD: %.2f Loss_ShpD: %.2f Loss_ObjSSD: %.2f Loss_ObjLSD: %.2f "
+                      "Loss_G: %.2f Time: %.2fs"
+                      % (epoch, self.max_epoch, self.num_batches, sum(h[f"errPatD{i}"] for i in range(n)),
+                         sum(h[f"errShpD{i}"] for i in range(n)), zero(h["errObjSSD"]), zero(h["errObjLSD"]),
+                         h["errG"] + h["kl"], end_t - start_t))
+            score = self.epoch_score(score)
+            if lead:
+                self.write_score(epoch, score)
+                if epoch % self.snapshot_interval == 0:
+                    self.net.save_model(self.model_dir, epoch)
+        if lead:
+            self.net.save_model(self.model_dir, self.max_epoch)
