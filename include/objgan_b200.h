@@ -114,8 +114,8 @@ int og_prep_split(const float* x, int N, int H, int W, int C, int pad, int s2d, 
 int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, int N, int SN, int SH, int SW, int C,
                  const void* wh, const void* wl, const unsigned* amax_w, int ntaps_w, int Kw, float* y, int OH, int OW,
                  int K, long long ysn, long long ysh, long long ysw, int OHf, int OWf, int osy, int osx, int opy,
-                 int opx, const int* taps_host, int ntaps, int tap_layout, int nsplit, const float* bias, int act,
-                 float slope, cudaStream_t stream);
+                 int opx, const int* taps_host, int ntaps, int nsplit, const float* bias, int act, float slope,
+                 cudaStream_t stream);
 /* Weight gradient: dw[tap][co][ci] = sum_{n,h,w} G[n+gdn, h, w, co] * X[n+xdn, h+dh, w+dw, ci]  (X out of range = 0).
  * Both operands are the same NHWC fp16 hi/lo tensors og_prep_split writes for the forward / input-gradient kernels
  * (G: [GN][OH][OW][Kp], X: [XN][SH][SW][C]; GN / XN = N or 4N space-to-depth blocks), consumed MN-major by

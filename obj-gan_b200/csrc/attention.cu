@@ -10,7 +10,6 @@
 // The grid attention streams h_code once (4*C bytes / query), writes the context once and the
 // attention map once: algorithmic bytes 4*Q*(2C + L) per image (SURVEY.md 8d).
 #include "common.cuh"
-#include <stdlib.h>
 
 constexpr int LMAX = 32;   // max caption length handled in registers (reference uses 12..18)
 
@@ -206,138 +205,6 @@ att_general_fwd_kernel(const float* __restrict__ h, const float* __restrict__ sr
   }
 }
 
-// ---------------------------------------------------------------------------------------------
-// Register-resident variant for the large maps (Q >= 4096, L <= 20): NO shared-memory transposes.  A thread owns QPT
-// queries (rows q0 + t + u * 128); it streams each of its rows straight from global memory with 16-byte loads (the
-// 32 lanes of a warp walk 32 adjacent rows, so every byte of every cache line fetched is consumed by the following
-// loads of the same warp), keeps the QPT x 20 scores / probabilities in registers, and writes its context rows
-// with 16-byte stores.  The only shared memory is the 48 x 20 word-projection table, read with broadcast LDS.128 that
-// each feed 4 * QPT FMAs.
-// ---------------------------------------------------------------------------------------------
-template <int QPT>
-__global__ void __launch_bounds__(ATT_Q)
-att_general_fwd_reg_kernel(const float* __restrict__ h, const float* __restrict__ src,
-                           const unsigned char* __restrict__ mask, int B, int Q, int idf, int cs, int L,
-                           float* __restrict__ wc, float* __restrict__ attn) {
-  constexpr int LM = 20;
-  extern __shared__ __align__(16) float ssrc[];          // [idf][LM], zero padded beyond L
-  const int b = blockIdx.y, q0 = blockIdx.x * (ATT_Q * QPT), t = threadIdx.x;
-  for (int i = t; i < idf * LM; i += ATT_Q) {
-    const int c = i / LM, l = i - c * LM;
-    ssrc[i] = l < L ? src[((long long)b * idf + c) * L + l] : 0.f;
-  }
-  __syncthreads();
-  int q[QPT];
-  bool live[QPT];
-  const float* hrow[QPT];
-#pragma unroll
-  for (int u = 0; u < QPT; ++u) {
-    q[u] = q0 + t + u * ATT_Q;
-    live[u] = q[u] < Q;
-    hrow[u] = h + ((long long)b * Q + (live[u] ? q[u] : 0)) * cs;
-  }
-  float2 s2[QPT][LM / 2];
-#pragma unroll
-  for (int u = 0; u < QPT; ++u)
-#pragma unroll
-    for (int l = 0; l < LM / 2; ++l) s2[u][l] = make_float2(0.f, 0.f);
-  for (int c4 = 0; c4 < idf; c4 += 4) {
-    float4 hv[QPT];
-#pragma unroll
-    for (int u = 0; u < QPT; ++u) hv[u] = ldg4(hrow[u] + c4);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (c4 + k < idf) {
-        const float4* sr = reinterpret_cast<const float4*>(ssrc + (c4 + k) * LM);
-        float2 hv2[QPT];
-#pragma unroll
-        for (int u = 0; u < QPT; ++u) {
-          const float x = k == 0 ? hv[u].x : k == 1 ? hv[u].y : k == 2 ? hv[u].z : hv[u].w;
-          hv2[u] = make_float2(x, x);
-        }
-#pragma unroll
-        for (int l4 = 0; l4 < LM / 4; ++l4) {
-          const float4 w = sr[l4];
-#pragma unroll
-          for (int u = 0; u < QPT; ++u) {
-            s2[u][2 * l4] = ffma2(hv2[u], make_float2(w.x, w.y), s2[u][2 * l4]);
-            s2[u][2 * l4 + 1] = ffma2(hv2[u], make_float2(w.z, w.w), s2[u][2 * l4 + 1]);
-          }
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int u = 0; u < QPT; ++u) {
-    float sc[LM];
-#pragma unroll
-    for (int l = 0; l < LM / 2; ++l) {
-      sc[2 * l] = s2[u][l].x;
-      sc[2 * l + 1] = s2[u][l].y;
-    }
-    float mx = -INFINITY;
-    if (mask && live[u]) {
-      const unsigned char* mr = mask + (((long long)b * Q + q[u]) % B) * L;
-#pragma unroll
-      for (int l = 0; l < LM; ++l)
-        if (l < L && mr[l]) sc[l] = -INFINITY;
-    }
-#pragma unroll
-    for (int l = 0; l < LM; ++l)
-      if (l < L) mx = fmaxf(mx, sc[l]);
-    float sum = 0.f;
-#pragma unroll
-    for (int l = 0; l < LM; ++l) {
-      sc[l] = l < L ? expf(sc[l] - mx) : 0.f;
-      sum += sc[l];
-    }
-    const float inv = 1.f / sum;
-#pragma unroll
-    for (int l = 0; l < LM; ++l) {
-      sc[l] *= inv;
-      if (l < L && live[u]) attn[((long long)b * L + l) * Q + q[u]] = sc[l];
-    }
-#pragma unroll
-    for (int l = 0; l < LM / 2; ++l) s2[u][l] = make_float2(sc[2 * l], sc[2 * l + 1]);
-  }
-  for (int c4 = 0; c4 < cs; c4 += 4) {
-    float o[QPT][4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int c = c4 + k;
-      float2 a2[QPT], b2[QPT];
-#pragma unroll
-      for (int u = 0; u < QPT; ++u) a2[u] = b2[u] = make_float2(0.f, 0.f);
-      if (c < idf) {
-        const float4* sr = reinterpret_cast<const float4*>(ssrc + c * LM);
-#pragma unroll
-        for (int l4 = 0; l4 < LM / 4; ++l4) {
-          const float4 w = sr[l4];
-#pragma unroll
-          for (int u = 0; u < QPT; ++u) {
-            a2[u] = ffma2(make_float2(w.x, w.y), s2[u][2 * l4], a2[u]);
-            b2[u] = ffma2(make_float2(w.z, w.w), s2[u][2 * l4 + 1], b2[u]);
-          }
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < QPT; ++u) o[u][k] = (a2[u].x + b2[u].x) + (a2[u].y + b2[u].y);
-    }
-#pragma unroll
-    for (int u = 0; u < QPT; ++u)
-      if (live[u]) st4(wc + ((long long)b * Q + q[u]) * cs + c4, make_float4(o[u][0], o[u][1], o[u][2], o[u][3]));
-  }
-}
-
-template <int QPT>
-static int launch_att_reg(const float* h, const float* src, const unsigned char* mask, int B, int Q, int idf, int cs,
-                          int L, float* wc, float* attn, cudaStream_t stream) {
-  const size_t sm = sizeof(float) * idf * 20;
-  dim3 grid(og_cdiv(Q, ATT_Q * QPT), B);
-  att_general_fwd_reg_kernel<QPT><<<grid, ATT_Q, sm, stream>>>(h, src, mask, B, Q, idf, cs, L, wc, attn);
-  OG_RETURN_LAST_ERROR();
-}
-
 // attention_tc.cu: the tensor-core (wgmma) kernel for the large maps of the hot path; -1 = shape outside its envelope
 extern "C" int og_att_general_fwd_tc(const float* h, const float* src, const unsigned char* mask, int B, int Q, int idf,
                                      int cs, int L, float* wc, float* attn, cudaStream_t stream);
@@ -346,17 +213,9 @@ OG_API int og_att_general_fwd(const float* h, const float* src, const unsigned c
                               int cs, int L, float* wc, float* attn, cudaStream_t stream) {
   if (L > LMAX || cs % 4 || idf > cs) return (int)cudaErrorInvalidValue;
   if (B == 0 || Q == 0) return 0;
-  static const int use_tc = getenv("OG_ATT_TC") ? atoi(getenv("OG_ATT_TC")) : 1;
-  if (use_tc && Q >= 4096) {
+  if (Q >= 4096) {
     const int rc = og_att_general_fwd_tc(h, src, mask, B, Q, idf, cs, L, wc, attn, stream);
     if (rc >= 0) return rc;
-  }
-  // register-resident variant (row-strided 16-byte loads cost 32 L1 wavefronts each): kept selectable, not the default
-  static const int reg_qpt = getenv("OG_ATT_QPT") ? atoi(getenv("OG_ATT_QPT")) : 0;
-  if (reg_qpt > 0 && L <= 20 && Q >= 4096 && idf * 20 * sizeof(float) <= 48 * 1024) {
-    if (reg_qpt == 1) return launch_att_reg<1>(h, src, mask, B, Q, idf, cs, L, wc, attn, stream);
-    if (reg_qpt == 2) return launch_att_reg<2>(h, src, mask, B, Q, idf, cs, L, wc, attn, stream);
-    return launch_att_reg<4>(h, src, mask, B, Q, idf, cs, L, wc, attn, stream);
   }
   if (L <= 20 && Q >= 4096) {   // the large maps of the hot path: two queries per thread
     constexpr int QPT = 2;
@@ -643,13 +502,11 @@ OG_API int og_att_general_bwd(const float* h, const float* src, const float* att
   if (L > LMAX || cs % 4 || idf > cs) return (int)cudaErrorInvalidValue;
   OG_CHECK(cudaMemsetAsync(g_src, 0, sizeof(float) * (size_t)B * idf * L, stream));
   if (B == 0 || Q == 0) return 0;
-  static const int bwd_tc = getenv("OG_ATT_TC_BWD") ? atoi(getenv("OG_ATT_TC_BWD")) : 1;
-  if (bwd_tc && !g_attn && Q >= 4096) {
+  if (!g_attn && Q >= 4096) {
     const int rc = og_att_general_bwd_tc(h, src, attn, g_wc, B, Q, idf, cs, L, g_h, g_src, stream);
     if (rc >= 0) return rc;
   }
-  static const bool old_bwd = getenv("OG_ATT_OLD_BWD") != nullptr;
-  if (!old_bwd && L <= 20 && idf <= 64) {
+  if (L <= 20 && idf <= 64) {
     const size_t sm20 = sizeof(float) * ((size_t)idf * 20 + 2 * ATT_Q * 20 + 2 * (size_t)ATT_Q * (cs + 1));
     static size_t configured20 = 0;
     if (sm20 > configured20) {

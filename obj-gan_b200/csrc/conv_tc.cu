@@ -631,16 +631,13 @@ int tc_fit_width(int cols) {
 //   rows of the GEMM are the pixel grid N x OH x OW; output pixel (osy*h + opy, osx*w + opx)
 //   taps  : ntaps quadruples (dh, dw, dn, weight tap index): source pixel = image n + dn, (h + dh, w + dw), zero
 //           outside [0,SH)x[0,SW);  bias/act: optional epilogue (bias[K], OG_ACT_*)
-//   tap_layout : 1 when the taps come in groups of three with equal dw, dn and dh = d0, d0+1, d0+2 (3x3 kernels
-//           listed column by column); a layout hint the kernel does not need
 // ------------------------------------------------------------------------------------------------
 OG_API int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, int N, int SN, int SH, int SW, int C,
                         const void* wh, const void* wl, const unsigned* amax_w, int ntaps_w, int Kw, float* y, int OH,
                         int OW, int K, long long ysn,
                         long long ysh, long long ysw, int OHf, int OWf, int osy, int osx, int opy, int opx,
-                        const int* taps_host, int ntaps, int tap_layout, int nsplit, const float* bias, int act,
+                        const int* taps_host, int ntaps, int nsplit, const float* bias, int act,
                         float slope, cudaStream_t stream) {
-  (void)tap_layout;
   if (C % 8 || K % 4 || ntaps < 1 || ntaps > TC_MAX_TAPS || (nsplit != 1 && nsplit != 3)) return (int)cudaErrorInvalidValue;
   if ((long long)N * OH * OW == 0) return 0;
   TcParams p;
@@ -705,11 +702,9 @@ OG_API int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, 
   unsigned abox[4] = {(unsigned)TC_BK, (unsigned)TW, (unsigned)TH, (unsigned)TN};
   unsigned long long bdims[3] = {(unsigned long long)C, (unsigned long long)Kw, (unsigned long long)ntaps_w};
   unsigned long long bstr[2] = {(unsigned long long)C, (unsigned long long)Kw * C};
-  // <= 32 output channels in the parity mode: [w_hi | w_lo] stacked along N (see conv_tc_kernel); OG_STACKED=0 keeps
-  // the three-MMA form
-  static const int stacked_on = getenv("OG_STACKED") ? atoi(getenv("OG_STACKED")) : 1;
+  // <= 32 output channels in the parity mode: [w_hi | w_lo] stacked along N (see conv_tc_kernel)
   const int stk_rows = K <= 16 ? 16 : 32;
-  const bool stacked = stacked_on && nsplit == 3 && BNsel == 32 && K <= 32;
+  const bool stacked = nsplit == 3 && BNsel == 32 && K <= 32;
   unsigned bbox[3] = {(unsigned)TC_BK, (unsigned)(stacked ? stk_rows : BNsel), 1u};
   int rc;
   if ((rc = make_map(&mah, xh, 4, adims, astr, abox))) return rc;

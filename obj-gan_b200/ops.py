@@ -194,10 +194,6 @@ class PackPlan:
 # (faster, outside the 1e-3 parity budget), "simt" = exact fp32 FMA on the CUDA cores.
 import os as _os
 CONV_ENGINE = _os.environ.get("OBJGAN_CONV", "f16x3")
-TC_WGRAD = _os.environ.get("OBJGAN_TC_WGRAD", "1") == "1"
-FUSED_AMAX = _os.environ.get("OBJGAN_FUSED_AMAX", "1") == "1"   # producers leave max|x| for the consuming conv
-KEEP_SPLIT = _os.environ.get("OBJGAN_KEEP_SPLIT", "1") == "1"   # keep x's hi/lo copies from forward for the wgrad
-FUSED_SPLIT = _os.environ.get("OBJGAN_FUSED_SPLIT", "1") == "1"  # norm-apply emits the consumer conv's hi/lo operand copies
 TC_MIN_PIXELS = 256        # smaller problems go to the exact-fp32 SIMT kernels (the tc kernel splits K on small maps)
 
 
@@ -251,34 +247,25 @@ def _tag_amax(t):
 
 def _known_amax(t):
     tag = getattr(t, "og_amax", None)
-    if tag is not None and tag[1] == t._version and FUSED_AMAX:
+    if tag is not None and tag[1] == t._version:
         return tag[0]
     return None
 
 
-def _tc_launch(xs, n, ws, ntaps_w, kw_rows, y, oh, ow, k, osy, op, taps, bias=None, act=ACT_NONE, layout=0):
+def _tc_launch(xs, n, ws, ntaps_w, kw_rows, y, oh, ow, k, osy, op, taps, bias=None, act=ACT_NONE, yoff=0,
+               slope=LRELU_SLOPE):
     """xs / ws: (hi, lo, scale word) operand triples; taps: (dh, dw, dn, widx) quadruples; the source is
-    [SN, SH, SW, C] with SN = n or 4n (space-to-depth)."""
+    [SN, SH, SW, C] with SN = n or 4n (space-to-depth).  The k output channels start at channel yoff of y."""
     xh, xl, ax = xs
     wh, wl, aw = ws
     sn, sh, sw, c = xh.shape
     _, ohf, owf, kc = y.shape
     arr = _int_array(taps)
     import ctypes
-    _call("og_conv2d_tc", _p(xh), _p(xl), _p(ax), n, sn, sh, sw, c, _p(wh), _p(wl), _p(aw), ntaps_w, kw_rows, _p(y),
-          oh, ow, k,
-          ohf * owf * kc, owf * kc, kc, ohf, owf, osy, osy, op[0], op[1], ctypes.addressof(arr), len(taps), layout,
-          _nsplit(), _p(bias), act, LRELU_SLOPE)
-
-
-def _tile_n(oh, ow):
-    tw = 1
-    while tw * 2 <= ow and tw * 2 <= 16:
-        tw *= 2
-    th = 1
-    while th * 2 <= oh and tw * th * 2 <= 128:
-        th *= 2
-    return 128 // (tw * th)
+    _call("og_conv2d_tc", _p(xh), _p(xl), _p(ax), n, sn, sh, sw, c, _p(wh), _p(wl), _p(aw), ntaps_w, kw_rows,
+          _p(y) + 4 * yoff, oh, ow, k,
+          ohf * owf * kc, owf * kc, kc, ohf, owf, osy, osy, op[0], op[1], ctypes.addressof(arr), len(taps),
+          _nsplit(), _p(bias), act, slope)
 
 
 def _tc_kind(n, h, w, c, kh, kw, stride, pad, mode):
@@ -323,8 +310,8 @@ def _tc_fprop(kind, x, cache, weight, kp, split, splitp, mode, bias_p, act):
     if mode == PAD_REFLECT:
         xs = _split(x, 1)
         y = torch.empty((n, h, w, kp), device=dev, dtype=torch.float32)
-        taps = [(kh, kw, 0, kh * 3 + kw) for kw in range(3) for kh in range(3)]      # column by column (layout 1)
-        _tc_launch(xs, n, ws, 9, kp, y, h, w, kp, 1, (0, 0), taps, bias_p, act, layout=1)
+        taps = [(kh, kw, 0, kh * 3 + kw) for kw in range(3) for kh in range(3)]      # column by column
+        _tc_launch(xs, n, ws, 9, kp, y, h, w, kp, 1, (0, 0), taps, bias_p, act)
     elif mode == PAD_ZERO:
         k = weight.shape[2]
         xs = _split(x, 0)
@@ -334,7 +321,7 @@ def _tc_fprop(kind, x, cache, weight, kp, split, splitp, mode, bias_p, act):
             taps = [(kh - 1, kw - 1, 0, kh * 3 + kw) for kw in range(3) for kh in range(3)]
         else:
             taps = [(kh - 1, kw - 1, 0, kh * k + kw) for kh in range(k) for kw in range(k)]
-        _tc_launch(xs, n, ws, k * k, kp, y, oh, ow, kp, 1, (0, 0), taps, bias_p, act, layout=1 if k == 3 else 0)
+        _tc_launch(xs, n, ws, k * k, kp, y, oh, ow, kp, 1, (0, 0), taps, bias_p, act)
     else:  # UPSAMPLE2X: four output phases of 2x2 taps at low resolution, weights pre-summed per phase
         ws = cache.get_up_hilo(weight, c, kp, split, splitp, 1)
         xs = _split(x, 0)
@@ -376,7 +363,7 @@ def _tc_dgrad(kind, gs, n, cache, weight, c, kp, split, splitp, mode, h, w, oh, 
     if mode == PAD_REFLECT:
         gpad = torch.empty((n, h + 2, w + 2, c), device=dev, dtype=torch.float32)
         taps = [(-kh, -kw, 0, kh * 3 + kw) for kw in range(3) for kh in (2, 1, 0)]   # rows ascending: -2, -1, 0
-        _tc_launch(gs, n, ws, 9, c, gpad, h + 2, w + 2, c, 1, (0, 0), taps, layout=1)
+        _tc_launch(gs, n, ws, 9, c, gpad, h + 2, w + 2, c, 1, (0, 0), taps)
         gx = torch.empty((n, h, w, c), device=dev, dtype=torch.float32)
         _call("og_reflect_pad_bwd", _p(gpad), n, h, w, c, _p(gx))
         return gx
@@ -387,7 +374,7 @@ def _tc_dgrad(kind, gs, n, cache, weight, c, kp, split, splitp, mode, h, w, oh, 
             taps = [(1 - kh, 1 - kw, 0, kh * 3 + kw) for kw in range(3) for kh in (2, 1, 0)]
         else:       # gx[i, j] = sum g[i + 1 - kh, j + 1 - kw] W[kh, kw]^T over the (oh, ow) gradient grid
             taps = [(1 - kh, 1 - kw, 0, kh * k + kw) for kh in range(k) for kw in range(k)]
-        _tc_launch(gs, n, ws, k * k, c, gx, h, w, c, 1, (0, 0), taps, layout=1 if k == 3 else 0)
+        _tc_launch(gs, n, ws, k * k, c, gx, h, w, c, 1, (0, 0), taps)
         return gx
     # UPSAMPLE2X: adjoint of the four phase convolutions: gx[i,j] = sum_{p,q,a,b} G_pq[i - off(p,a), j - off(q,b)] Wp^T
     ws = cache.get_up_hilo(weight, c, kp, split, splitp, 0)
@@ -396,20 +383,6 @@ def _tc_dgrad(kind, gs, n, cache, weight, c, kp, split, splitp, mode, h, w, oh, 
             for p_ in range(2) for q_ in range(2) for a in range(2) for b in range(2)]
     _tc_launch(gs, n, ws, 16, c, gx, h, w, c, 1, (0, 0), taps)
     return gx
-
-
-def _tc_wgrad_ok(kind, mode, n, oh, ow):
-    """The wgrad kernel streams 64-pixel patches (cw x chh x cn, powers of two) of the gradient grid."""
-    if kind == "s1" and mode == UPSAMPLE2X:
-        oh, ow = oh // 2, ow // 2
-    cw = 1
-    while cw * 2 <= 64 and ow % (cw * 2) == 0:
-        cw *= 2
-    chh = 1
-    while cw * chh * 2 <= 64 and oh % (chh * 2) == 0:
-        chh *= 2
-    # a last image group that the batch does not fill adds nothing (the unstacked operand is zero filled there)
-    return True
 
 
 def _grad_sink(param):
@@ -463,8 +436,6 @@ def _tc_wgrad(kind, xs, gs, n, h, w, oh, ow, weight, c, kp, split, splitp, mode,
 def _out_hw(h, w, kh, kw, stride, pad, mode):
     if mode == UPSAMPLE2X:
         return 2 * h, 2 * w
-    if mode == PAD_REFLECT:
-        return (h + 2 * pad - kh) // stride + 1, (w + 2 * pad - kw) // stride + 1
     return (h + 2 * pad - kh) // stride + 1, (w + 2 * pad - kw) // stride + 1
 
 
@@ -509,8 +480,7 @@ class _Conv2d(torch.autograd.Function):
         xs = None
         if kind:
             y, xs = _tc_fprop(kind, x, cache, weight, kp, split, splitp, mode, bias_p, act)
-            if not (KEEP_SPLIT and ctx.needs_input_grad[1] and TC_WGRAD and _tc_wgrad_ok(kind, mode, n, oh, ow)) \
-                    and not f32_missing:
+            if not ctx.needs_input_grad[1] and not f32_missing:
                 xs = None
         elif narrow:
             wf, _ = cache.get(weight, c, kp, split, splitp, False)
@@ -567,7 +537,7 @@ class _Conv2d(torch.autograd.Function):
                     gw = torch.empty_like(weight)
                     _call("og_unpack_wgrad", _p(dwp), co, ci, kh, kw, c, kp, split, splitp, _p(gw), 0, 0)
             return gx, gw, gb, None, None, None, None, None, None
-        tc_w = bool(ctx.needs_input_grad[1] and kind and TC_WGRAD and _tc_wgrad_ok(kind, mode, n, oh, ow))
+        tc_w = bool(ctx.needs_input_grad[1] and kind)
         gs = _split_g(kind, g, mode) if kind and (ctx.needs_input_grad[0] or tc_w) else None
         if ctx.needs_input_grad[0] and kind:
             gx = _tc_dgrad(kind, gs, n, ctx.cache, weight, c, kp, split, splitp, mode, h, w, oh, ow)
@@ -630,7 +600,7 @@ class _NormAct(torch.autograd.Function):
         if res is not None:
             res = res.contiguous()
             assert res.shape == out.shape
-        fused = (split_pad is not None and FUSED_SPLIT and CONV_ENGINE in ("f16x3", "f16") and not _lib.DRY_RUN
+        fused = (split_pad is not None and CONV_ENGINE in ("f16x3", "f16") and not _lib.DRY_RUN
                  and (res is None or _known_amax(res) is not None) and (split_pad == 0 or (h > 1 and w > 1)))
         if fused:
             # the consuming convolution's operand copies straight from this pass, scaled by an a-priori bound of max|out|
@@ -1944,16 +1914,6 @@ class EncConv:
         return oh * ow * self.cout * self.cin * self.kh * self.kw
 
 
-def _enc_tc(xs, n, ws, ntaps_w, kw_rows, yptr, oh, ow, k, ystr, ohf, owf, osy, op, taps, bias, act):
-    import ctypes
-    xh = xs[0]
-    sn, sh, sw, c = xh.shape
-    arr = _int_array(taps)
-    _call("og_conv2d_tc", _p(xh), _p(xs[1]), _p(xs[2]), n, sn, sh, sw, c, _p(ws[0]), _p(ws[1]), _p(ws[2]), ntaps_w,
-          kw_rows, yptr, oh, ow, k, ystr[0], ystr[1], ystr[2], ohf, owf, osy, osy, op[0], op[1], ctypes.addressof(arr),
-          len(taps), 0, _nsplit(), _p(bias), act, 0.0)
-
-
 def _split_s2d_odd(x):
     n, h, w, c = x.shape
     shape = (4 * n, (h + 1) // 2, (w + 1) // 2, c)
@@ -1989,7 +1949,7 @@ def enc_conv_fwd(layer, x, y, yoff=0):
         else:
             xs = _split(x, 0)
             taps = [(i - layer.padh, j - layer.padw, 0, i * layer.kw + j) for i in range(layer.kh) for j in range(layer.kw)]
-        _enc_tc(xs, n, ws, kk, k, yptr, oh, ow, k, ystr, oh, ow, 1, (0, 0), taps, bias, layer.act)
+        _tc_launch(xs, n, ws, kk, k, y, oh, ow, k, 1, (0, 0), taps, bias, layer.act, yoff=yoff, slope=0.0)
     else:
         wp, _ = cache.get(wf, c, k, 0, 0, False)
         _call("og_conv2d_simt_pad2", _p(x), n, h, w, c, h * w * c, w * c, c, _p(wp), yptr, oh, ow, k, ystr[0], ystr[1],
@@ -2006,18 +1966,16 @@ def enc_conv_dgrad(layer, gp, h, w):
     if layer.on_tc(n, h, w):
         ws = cache.get_hilo(wf, c, k, 0, 0, 0)                    # [tap][ci][co]
         gs = _split(gp, 0)
-        ystr = (h * w * c, w * c, c)
         if layer.stride == 2:     # input pixel (2i + a, 2j + b) <- kernel taps with kh = a, kw = b (mod 2)
             for a in range(2):
                 for b in range(2):
                     taps = [(-((i - a) // 2), -((j - b) // 2), 0, i * layer.kw + j)
                             for i in range(layer.kh) if (i - a) % 2 == 0 for j in range(layer.kw) if (j - b) % 2 == 0]
-                    _enc_tc(gs, n, ws, layer.kh * layer.kw, c, gx.data_ptr(), (h + 1) // 2, (w + 1) // 2, c, ystr,
-                            h, w, 2, (a, b), taps, None, ACT_NONE)
+                    _tc_launch(gs, n, ws, layer.kh * layer.kw, c, gx, (h + 1) // 2, (w + 1) // 2, c, 2, (a, b), taps,
+                               slope=0.0)
         else:
             taps = [(layer.padh - i, layer.padw - j, 0, i * layer.kw + j) for i in range(layer.kh) for j in range(layer.kw)]
-            _enc_tc(gs, n, ws, layer.kh * layer.kw, c, gx.data_ptr(), h, w, c, ystr, h, w, 1, (0, 0), taps, None,
-                    ACT_NONE)
+            _tc_launch(gs, n, ws, layer.kh * layer.kw, c, gx, h, w, c, 1, (0, 0), taps, slope=0.0)
     else:
         _, wt = cache.get(wf, c, k, 0, 0, True)
         _call("og_conv2d_simt_pad2", _p(gp), n, oh, ow, k, oh * ow * k, ow * k, k, _p(wt), _p(gx), h, w, c, h * w * c,

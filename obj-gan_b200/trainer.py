@@ -24,8 +24,6 @@ from . import losses, model, ops
 from .config import cfg
 
 ALIGN = 64  # floats; keeps every parameter view 256-byte aligned inside its bucket
-BRANCH_ADAM = os.environ.get("OBJGAN_BRANCH_ADAM", "1") == "1"   # exchange + optimiser step of each D on its own stream
-PACK_PLAN = os.environ.get("OBJGAN_PACK_PLAN", "1") == "1"       # re-pack a network's operand copies right after Adam
 
 
 def prepare_data(dev: dict, num_classes: int | None = None, into: dict | None = None) -> dict:
@@ -153,8 +151,7 @@ class FlatBucket:
         ops.adam_ema_(self.flat, self.grad, self.m, self.v, self.avg, self.step, lr=lr, b1=0.5, b2=0.999, eps=1e-8,
                       gscale=gscale, decay=0.999, step_dev=self.step_dev, bump=False)
         self.epoch[0] += 1
-        if PACK_PLAN:
-            self.plan.run()                   # every tensor-core operand copy of this network, two launches
+        self.plan.run()                       # every tensor-core operand copy of this network, two launches
 
     def ema_state_dict(self):
         """EMA weights keyed like ``module.state_dict()`` (what the reference saves as netG_epoch_%d.pth,
@@ -209,7 +206,7 @@ class StepATrainer:
 
     def _branch_streams(self):
         """Side streams for the three independent discriminator branches (None: run them in sequence)."""
-        if os.environ.get("OBJGAN_D_STREAMS", "1") != "1" or not torch.cuda.is_available() or _lib.DRY_RUN:
+        if not torch.cuda.is_available() or _lib.DRY_RUN:
             return None
         if not hasattr(self, "_dstreams"):
             self._dstreams = [torch.cuda.Stream() for _ in self.netsPatD]
@@ -289,9 +286,8 @@ class StepATrainer:
             for t, s0 in zip(mod.buffers(), saved):
                 t.copy_(s0)
         ops.bump_param_epoch()
-        if PACK_PLAN:
-            for b in [self.bG, *self.bD]:
-                b.plan.run()                 # operand copies of the restored weights
+        for b in [self.bG, *self.bD]:
+            b.plan.run()                     # operand copies of the restored weights
         torch.cuda.synchronize()
         self._graph = torch.cuda.CUDAGraph()
         n0 = _l.get().launches
@@ -345,7 +341,6 @@ class StepATrainer:
             fake_imgs, _bt_c, _att, _bt_att, mu, logvar = self.generate(inp)
         out = {}
         # (3-1) update the patch discriminators
-        works = []
         streams = self._branch_streams()
         main = torch.cuda.current_stream() if streams else None
         for b in self.bD:
@@ -364,20 +359,13 @@ class StepATrainer:
                 # the gradient exchange and the optimiser step of this discriminator stay on ITS branch: the
                 # all-reduce of the small 64 / 128 discriminators runs under the backward pass of the 256 one
                 # (every rank issues the three collectives in the same program order)
-                if BRANCH_ADAM:
-                    w = self._allreduce(b)
-                    if w is not None:
-                        w.wait()
-                    b.adam(lr_d, gs)
-        for i, b in enumerate(self.bD):
-            if streams:
-                main.wait_stream(streams[i])
-        if not BRANCH_ADAM:
-            works = [self._allreduce(b) for b in self.bD]
-            for w, b in zip(works, self.bD):
+                w = self._allreduce(b)
                 if w is not None:
                     w.wait()
                 b.adam(lr_d, gs)
+        for i, b in enumerate(self.bD):
+            if streams:
+                main.wait_stream(streams[i])
         # (4) update G through the updated discriminators (their weight gradients are not needed)
         for b in self.bD:
             b.requires_grad_(False)

@@ -6,7 +6,7 @@ import time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
-from objgan_b200 import ops, synth, trainer
+from objgan_b200 import synth, trainer
 
 steps = int(sys.argv[1]) if len(sys.argv) > 1 else 4
 tr = trainer.StepATrainer(device="cuda", seed=1234)
@@ -24,5 +24,4 @@ for _ in range(steps):
     tr.step(dev)
 e1.record()
 torch.cuda.synchronize()
-print(f"step a B=16 fused_split={ops.FUSED_SPLIT} d_streams={os.environ.get('OBJGAN_D_STREAMS', '1')}: "
-      f"GPU {e0.elapsed_time(e1) / steps:.1f} ms/step", flush=True)
+print(f"step a B=16: GPU {e0.elapsed_time(e1) / steps:.1f} ms/step", flush=True)

@@ -27,5 +27,5 @@ for _ in range(steps):
 e1.record()
 t_enq = (time.perf_counter() - t0) / steps
 torch.cuda.synchronize()
-print(f"step b B=16 streams={os.environ.get('OBJGAN_D_STREAMS', '1')}: host enqueue {t_enq * 1e3:.1f} ms/step, "
+print(f"step b B=16: host enqueue {t_enq * 1e3:.1f} ms/step, "
       f"GPU {e0.elapsed_time(e1) / steps:.1f} ms/step, peak memory {torch.cuda.max_memory_allocated() / 2**30:.1f} GiB", flush=True)

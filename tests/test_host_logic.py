@@ -220,7 +220,7 @@ def test_checkpoint_files_round_trip(dry, tmp_path):
 
 
 def test_res_chain_tells_each_block_its_consumer(dry):
-    """Producer-side operand split (ops.FUSED_SPLIT): every residual block of the generator knows which operand layout
+    """Producer-side operand split (og_norm_apply_split): every residual block of the generator knows which operand layout
     the convolution after it wants -- the next block's reflection-padded conv (halo 1) or the upsample conv that ends
     the chain (plain copies, halo 0) -- and the C ABI declares the two launchers the fused pass needs."""
     from objgan_b200 import lib as L
