@@ -71,7 +71,7 @@ def _patch(oh, ow):
     return 128 // (tw * th), th, tw
 
 
-def issued_tc(n, oh, ow, c, k, ntaps, nsplit=3):
+def issued_tc(n, oh, ow, c, k, ntaps):
     """Issued MMA flops of one og_conv2d_tc launch: GEMM rows n x oh x ow, c input channels, k output channels."""
     tn, th, tw = _patch(oh, ow)
     m = math.ceil(n / tn) * math.ceil(oh / th) * math.ceil(ow / tw) * 128
@@ -80,12 +80,12 @@ def issued_tc(n, oh, ow, c, k, ntaps, nsplit=3):
     ntile = math.ceil(k / 128)
     bn8 = (math.ceil(k / ntile) + 7) // 8 * 8
     bn = next((b for b in BN_SET if b >= bn8), 128)
-    if nsplit == 3 and bn == 32 and k <= 32:       # stacked [w_hi | w_lo]: two MMAs of twice the width
+    if bn == 32 and k <= 32:                       # stacked [w_hi | w_lo]: two MMAs of twice the width
         return 2 * 2.0 * m * (32 if k <= 16 else 64) * kred
-    return nsplit * 2.0 * m * math.ceil(k / bn) * bn * kred
+    return 3 * 2.0 * m * math.ceil(k / bn) * bn * kred
 
 
-def issued_wgrad(n, oh, ow, kp, c, entries, nsplit=3):
+def issued_wgrad(n, oh, ow, kp, c, entries):
     """Issued MMA flops of one og_conv2d_wgrad_tc launch over an oh x ow gradient grid of n images."""
     cw = 1
     while cw * 2 <= 64 and ow % (cw * 2) == 0:
@@ -98,7 +98,7 @@ def issued_wgrad(n, oh, ow, kp, c, entries, nsplit=3):
     ntile = math.ceil(c / 128)                     # ci tiles fitted like the forward's N tile
     bnw = next((b for b in BN_SET if b >= (math.ceil(c / ntile) + 7) // 8 * 8), 128)
     rows = math.ceil(kp / 64) * 64                 # a 64-row co slab wholly past kp issues nothing
-    return nsplit * 2.0 * rows * ntile * bnw * pix * entries
+    return 3 * 2.0 * rows * ntile * bnw * pix * entries
 
 
 def layer_work(cin, cout, k, stride, mode, split, n, h, w):
@@ -160,7 +160,7 @@ def bench_layer(spec, window_ms, dirs=("fprop", "dgrad", "wgrad")):
         x = torch.randn(n, h, w, c, device="cuda")
         x[..., cin:] = 0
         xs = ops._split_x(kind, x, mode)
-        x.og_split = (*xs, pad, s2d, x._version, ops._nsplit())  # fprop reuses these copies: no split pass timed
+        x.og_split = (*xs, pad, s2d, x._version)  # fprop reuses these copies: no split pass timed
         g = torch.randn(n, oh, ow, kp, device="cuda")
         gs = ops._split_g(kind, g, mode)
         sets.append((x, xs, gs))

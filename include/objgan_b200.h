@@ -60,11 +60,12 @@ int og_roi_align_avg_nhwc_bwd(const float* grad_out, int height, int width, int 
  * x: source NHWC [N,H,W,C] with element strides (xsn,xsh,xsw); y likewise [N,OH,OW,K]; C % 8 == 0, K % 4 == 0.
  * mode selects how a (row pixel, tap) pair maps to a source pixel: zero padding, reflection padding
  * (nn.ReflectionPad2d), nearest-2x upsampling followed by zero padding (nn.Upsample + conv), or the
- * transposed map used for the input gradient.  wpacked is produced by og_pack_weights.
+ * transposed map used for the input gradient.  wpacked is produced by og_pack_weights.  padh / padw: row / column
+ * padding (they differ for the 1x7, 7x1, 1x3 and 3x1 kernels of the Inception-v3 image encoder).
  * ---------------------------------------------------------------------------------------------------- */
 int og_conv2d_simt(const float* x, int N, int H, int W, int C, long long xsn, long long xsh, long long xsw,
                    const float* wpacked, float* y, int OH, int OW, int K, long long ysn, long long ysh, long long ysw,
-                   int KH, int KW, int stride, int pad, int mode, const float* bias, int act, float slope,
+                   int KH, int KW, int stride, int padh, int padw, int mode, const float* bias, int act, float slope,
                    int allow_splitk, cudaStream_t stream);
 int og_conv2d_wgrad_simt(const float* x, int N, int H, int W, int C, long long xsn, long long xsh, long long xsw,
                          const float* g, int OH, int OW, int K, long long gsn, long long gsh, long long gsw,
@@ -106,15 +107,15 @@ int og_unpack_upsample_wgrad(const float* dwp, int Co, int Ci, int Cip, int Kp, 
  * the nn.ReflectionPad2d(1) halo, ref: model.py:67; s2d=1 writes the four space-to-depth phase blocks used by
  * the stride-2 convs of the discriminators and by the adjoint of the 2x upsampling); og_conv2d_tc computes
  *     y[n, osy*h+opy, osx*w+opx, :] = act(bias + sum_t x[n+dn_t, h+dh_t, w+dw_t, :] * W[widx_t])   (x OOB = 0)
- * with taps = ntaps host quadruples (dh, dw, dn, widx); nsplit = 3 is the error-compensated product (fp32-level
- * accuracy), nsplit = 1 a single fp16 product (xl / wl unused). */
+ * with taps = ntaps host quadruples (dh, dw, dn, widx), as the error-compensated product (fp32-level accuracy).
+ * Every entry point that takes a hi / lo pair returns cudaErrorInvalidValue if either pointer is null. */
 int og_amax(const float* x, long long n, unsigned* amax, cudaStream_t stream);
 int og_prep_split(const float* x, int N, int H, int W, int C, int pad, int s2d, unsigned* amax, int amax_ready,
                   void* xh, void* xl, cudaStream_t stream);
 int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, int N, int SN, int SH, int SW, int C,
                  const void* wh, const void* wl, const unsigned* amax_w, int ntaps_w, int Kw, float* y, int OH, int OW,
                  int K, long long ysn, long long ysh, long long ysw, int OHf, int OWf, int osy, int osx, int opy,
-                 int opx, const int* taps_host, int ntaps, int nsplit, const float* bias, int act, float slope,
+                 int opx, const int* taps_host, int ntaps, const float* bias, int act, float slope,
                  cudaStream_t stream);
 /* Weight gradient: dw[tap][co][ci] = sum_{n,h,w} G[n+gdn, h, w, co] * X[n+xdn, h+dh, w+dw, ci]  (X out of range = 0).
  * Both operands are the same NHWC fp16 hi/lo tensors og_prep_split writes for the forward / input-gradient kernels
@@ -123,7 +124,7 @@ int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, int N, 
  * entries_host: nentries quintuples (gdn, dh, dw, xdn, output tap); dw is [ntaps_out][Kp][C], zero-filled here. */
 int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* amax_g, int N, int GN, int OH, int OW, int Kp,
                        const void* xh, const void* xl, const unsigned* amax_x, int XN, int SH, int SW, int C, float* dw,
-                       int ntaps_out, const int* entries_host, int nentries, int nsplit, cudaStream_t stream);
+                       int ntaps_out, const int* entries_host, int nentries, cudaStream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------
  * InstanceNorm2d / BatchNorm (train and eval mode) + fused GLU / LeakyReLU / residual
@@ -384,7 +385,6 @@ int og_zero_bytes(float* p, long long bytes, cudaStream_t stream);
 
 /* ----------------------------------------------------------------------------------------------------
  * Inception-v3 image encoder (CNN_ENCODER, ref: model.py:182-287; csrc/inception.cu).  NHWC fp32, C % 8 == 0.
- * og_conv2d_simt_pad2 is og_conv2d_simt with separate row / column padding (1x7, 7x1, 1x3, 3x1 kernels).
  * Pooling: max_pool2d(3, 2) (output may be a channel slice: pixel stride ldy, offset yoff; the backward reads the
  * gradient slice the same way), avg_pool2d(3, 1, 1, count_include_pad=True), the global average over P pixels; every
  * backward is a deterministic gather.  og_bilinear_bwd_gather: adjoint of og_bilinear_fwd without atomics.
@@ -393,10 +393,6 @@ int og_zero_bytes(float* p, long long bytes, cudaStream_t stream);
  * ceil(H/2) x ceil(W/2), zero past an odd edge).  og_relu_grad_slice: out[p, ooff + c] = g[p, goff + c] masked by
  * y[p, yoff + c] > 0 (relu = 1) or copied (relu = 0), c < nch.
  * ---------------------------------------------------------------------------------------------------- */
-int og_conv2d_simt_pad2(const float* x, int N, int H, int W, int C, long long xsn, long long xsh, long long xsw,
-                        const float* wpacked, float* y, int OH, int OW, int K, long long ysn, long long ysh,
-                        long long ysw, int KH, int KW, int stride, int padh, int padw, int mode, const float* bias,
-                        int act, float slope, int allow_splitk, cudaStream_t stream);
 int og_maxpool3s2_fwd(const float* x, int N, int H, int W, int C, float* y, int ldy, int yoff, cudaStream_t stream);
 int og_maxpool3s2_bwd(const float* x, const float* g, int ldg, int goff, int N, int H, int W, int C, float* gx,
                       cudaStream_t stream);

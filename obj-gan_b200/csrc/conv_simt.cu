@@ -332,7 +332,7 @@ __device__ __forceinline__ void store_hilo_f16(float v, float scale, __half* hi,
   v *= scale;
   const __half h = __float2half_rn(v);
   hi[o] = h;
-  if (lo) lo[o] = __float2half_rn(v - __half2float(h));
+  lo[o] = __float2half_rn(v - __half2float(h));
 }
 
 template <bool F16>
@@ -600,12 +600,13 @@ static int pick_splits(long long tiles, int nk, int want_ctas) {
   return s < 1 ? 1 : s;
 }
 
-static int conv2d_simt(const float* x, int N, int H, int W, int C, long long xsn, long long xsh, long long xsw,
-                       const float* wpacked, float* y, int OH, int OW, int K, long long ysn, long long ysh,
-                       long long ysw, int KH, int KW, int stride, int pad, int padw, int mode, const float* bias,
-                       int act, float slope, int allow_splitk, cudaStream_t stream) {
+// padh / padw: row / column padding (they differ for the 1x7 / 7x1 / 1x3 / 3x1 convolutions of Inception-v3)
+OG_API int og_conv2d_simt(const float* x, int N, int H, int W, int C, long long xsn, long long xsh, long long xsw,
+                          const float* wpacked, float* y, int OH, int OW, int K, long long ysn, long long ysh,
+                          long long ysw, int KH, int KW, int stride, int padh, int padw, int mode, const float* bias,
+                          int act, float slope, int allow_splitk, cudaStream_t stream) {
   if (C % 8 || K % 4) return (int)cudaErrorInvalidValue;
-  ConvArgs a{x, N, H, W, C, xsn, xsh, xsw, wpacked, y, OH, OW, K, ysn, ysh, ysw, KH, KW, stride, pad, mode, bias, act, slope};
+  ConvArgs a{x, N, H, W, C, xsn, xsh, xsw, wpacked, y, OH, OW, K, ysn, ysh, ysw, KH, KW, stride, padh, mode, bias, act, slope};
   a.padw = padw;
   long long M = (long long)N * OH * OW;
   if (M == 0) return 0;
@@ -638,23 +639,6 @@ static int conv2d_simt(const float* x, int N, int H, int W, int C, long long xsn
     if (!rc) rc = (int)e;
   }
   return rc;
-}
-
-OG_API int og_conv2d_simt(const float* x, int N, int H, int W, int C, long long xsn, long long xsh, long long xsw,
-                          const float* wpacked, float* y, int OH, int OW, int K, long long ysn, long long ysh,
-                          long long ysw, int KH, int KW, int stride, int pad, int mode, const float* bias, int act,
-                          float slope, int allow_splitk, cudaStream_t stream) {
-  return conv2d_simt(x, N, H, W, C, xsn, xsh, xsw, wpacked, y, OH, OW, K, ysn, ysh, ysw, KH, KW, stride, pad, pad, mode,
-                     bias, act, slope, allow_splitk, stream);
-}
-
-// og_conv2d_simt with separate row / column padding (the 1x7 / 7x1 / 1x3 / 3x1 convolutions of Inception-v3)
-OG_API int og_conv2d_simt_pad2(const float* x, int N, int H, int W, int C, long long xsn, long long xsh, long long xsw,
-                               const float* wpacked, float* y, int OH, int OW, int K, long long ysn, long long ysh,
-                               long long ysw, int KH, int KW, int stride, int padh, int padw, int mode,
-                               const float* bias, int act, float slope, int allow_splitk, cudaStream_t stream) {
-  return conv2d_simt(x, N, H, W, C, xsn, xsh, xsw, wpacked, y, OH, OW, K, ysn, ysh, ysw, KH, KW, stride, padh, padw,
-                     mode, bias, act, slope, allow_splitk, stream);
 }
 
 OG_API int og_conv2d_wgrad_simt(const float* x, int N, int H, int W, int C, long long xsn, long long xsh,
@@ -707,6 +691,7 @@ OG_API int og_pack_weights(const float* w_oihw, int Co, int Ci, int KH, int KW, 
 OG_API int og_pack_weights_f16(const float* w_oihw, int Co, int Ci, int KH, int KW, int Cip, int Kp, int split,
                                int splitp, int transposed, const unsigned* amax, void* hi, void* lo,
                                cudaStream_t stream) {
+  if (!hi || !lo) return (int)cudaErrorInvalidValue;
   long long total = (long long)KH * KW * Cip * Kp;
   int blocks = (int)((total + 255) / 256);
   if (blocks > og_num_sms() * 16) blocks = og_num_sms() * 16;
@@ -838,9 +823,10 @@ __global__ void unpack_upsample_wgrad_kernel(const float* __restrict__ dwp, int 
 OG_API int og_pack_upsample_weights(const float* w_oihw, int Co, int Ci, int Cip, int Kp, int split, int splitp,
                                     int transposed, const unsigned* amax, unsigned* amax_up, void* hi, void* lo,
                                     cudaStream_t stream) {
+  if (!hi || !lo) return (int)cudaErrorInvalidValue;
   long long n = (long long)16 * Cip * Kp;
   OG_CHECK(cudaMemsetAsync(hi, 0, sizeof(__half) * n, stream));
-  if (lo) OG_CHECK(cudaMemsetAsync(lo, 0, sizeof(__half) * n, stream));
+  OG_CHECK(cudaMemsetAsync(lo, 0, sizeof(__half) * n, stream));
   long long total = (long long)16 * Co * Ci;
   int blocks = (int)((total + 255) / 256);
   if (blocks > og_num_sms() * 16) blocks = og_num_sms() * 16;

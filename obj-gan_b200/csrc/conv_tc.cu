@@ -15,7 +15,6 @@
 // range is handled by scaling every operand tensor by a power of two taken from its max|x| (og_prep_split /
 // og_pack_weights_f16 write x * 2^k; the epilogue multiplies the accumulator by 2^-(ka+kb)): elements within
 // 2^-18 of the tensor maximum keep all 22 bits, smaller ones an absolute error <= 2^-39 of the maximum.
-// nsplit = 1 runs a single fp16 product (reported separately, never the parity mode).
 //
 // GEMM tiling: one CTA = 128 output pixels (a TN x TH x TW patch) x BN output channels (BN % 8 == 0,
 // <= 128); K loop over taps x 64-channel chunks; STAGES-deep smem ring of {A_hi, A_lo, B_hi, B_lo}.
@@ -131,8 +130,8 @@ struct TcAccWide {
 // touches the accumulator registers; otherwise ptxas waits for every wgmma before issuing the next (C7520 / C7519 /
 // C7514 warnings).  The wait sits in here too, so that a caller choosing KS at run time (a switch) merges the
 // accumulators only after it (C7517 otherwise).
-// NSPLIT = 3: al*bh, ah*bl, ah*bh (small terms first); 1: ah*bh.  STACKED: al*[bh_hi | bh_lo], ah*[bh_hi | bh_lo].
-template <int KS, uint32_t KSTEP, int NSPLIT, bool STACKED, class Acc>
+// al*bh, ah*bl, ah*bh (small terms first); STACKED: al*[bh_hi | bh_lo], ah*[bh_hi | bh_lo].
+template <int KS, uint32_t KSTEP, bool STACKED, class Acc>
 __device__ __forceinline__ void tc_stage_mma(Acc& part, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl) {
   wg_fence();
 #pragma unroll
@@ -141,12 +140,10 @@ __device__ __forceinline__ void tc_stage_mma(Acc& part, uint64_t ah, uint64_t al
     if constexpr (STACKED) {
       part.mma(al + koff, bh + koff, k > 0);
       part.mma(ah + koff, bh + koff, 1);
-    } else if constexpr (NSPLIT == 3) {
+    } else {
       part.mma(al + koff, bh + koff, k > 0);
       part.mma(ah + koff, bl + koff, 1);
       part.mma(ah + koff, bh + koff, 1);
-    } else {
-      part.mma(ah + koff, bh + koff, k > 0);
     }
   }
   wg_commit();
@@ -159,18 +156,16 @@ __device__ __forceinline__ void tc_stage_mma(Acc& part, uint64_t ah, uint64_t al
 __device__ __forceinline__ int tc_warp_uniform() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
 
 // ------------------------------------------------------------------------------------------------
-// STACKED (3xFP16 only, <= 32 output channels): B is [w_hi | w_lo] of the same BN / 2 output channels stacked along
-// N, so a k-step is two MMAs, a_lo [w_hi | w_lo] and a_hi [w_hi | w_lo], and the epilogue adds the two column halves
-// (the extra a_lo w_lo term is below the rounding of the others).  Each A copy is read from shared memory once per
-// k-step instead of 1.5 times -- narrow layers are bound by those reads, not by the MMA rate.
-// NSPLIT: products per k-step (3 = 3xFP16, 1 = one fp16 product), a template parameter so that the issue window
-// holds no branch.
-template <int BN, int STAGES, bool STACKED, int NSPLIT>
+// STACKED (<= 32 output channels): B is [w_hi | w_lo] of the same BN / 2 output channels stacked along N, so a k-step
+// is two MMAs, a_lo [w_hi | w_lo] and a_hi [w_hi | w_lo], and the epilogue adds the two column halves (the extra
+// a_lo w_lo term is below the rounding of the others).  Each A copy is read from shared memory once per k-step
+// instead of 1.5 times -- narrow layers are bound by those reads, not by the MMA rate.
+template <int BN, int STAGES, bool STACKED>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant__ CUtensorMap map_al,
                const __grid_constant__ CUtensorMap map_bh, const __grid_constant__ CUtensorMap map_bl,
                const TcParams p) {
-  static_assert(BN % 8 == 0 && BN <= 128 && (NSPLIT == 1 || NSPLIT == 3) && (!STACKED || NSPLIT == 3), "");
+  static_assert(BN % 8 == 0 && BN <= 128, "");
   constexpr uint32_t A_BYTES = TC_BM * 128;         // 128 rows of 128 bytes = 16 KB
   constexpr uint32_t B_BYTES = BN * 128;            // BN % 8 == 0: a whole number of 1024-byte swizzle atoms
   constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + (STACKED ? 1 : 2) * B_BYTES;
@@ -191,16 +186,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
   const int per_split = (nk_total + p.ksplit - 1) / p.ksplit;
   const int it_beg = blockIdx.z * per_split;
   const int nk = min(nk_total, it_beg + per_split) - it_beg;
-  constexpr uint32_t tx_bytes = (NSPLIT == 3) ? STAGE_BYTES : (A_BYTES + B_BYTES);
   if (nk <= 0) return;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&map_ah);
     prefetch_tmap(&map_bh);
-    if (NSPLIT == 3) {
-      prefetch_tmap(&map_al);
-      prefetch_tmap(&map_bl);
-    }
+    prefetch_tmap(&map_al);
+    prefetch_tmap(&map_bl);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], TC_CONSUMER_WARPS);
@@ -218,16 +210,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
         const int tap = (it_beg + it) / p.cchunks, cc = (it_beg + it) - tap * p.cchunks;
         mbar_wait(&empty_bar[stage], phase ^ 1);
         uint8_t* sa = smem + (size_t)stage * STAGE_BYTES;
-        mbar_expect_tx(&full_bar[stage], tx_bytes);
+        mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
         const int c0 = cc * TC_BK, ws = w0 + p.taps.dw[tap], hs = h0 + p.taps.dh[tap], widx = p.taps.widx[tap];
         const int ns = n0 + p.taps.dn[tap];   // image offset: selects a space-to-depth phase block of the source
         tma_load_4d(sa, &map_ah, &full_bar[stage], c0, ws, hs, ns);
         tma_load_3d(sa + 2 * A_BYTES, &map_bh, &full_bar[stage], c0, col0, widx);
-        if (NSPLIT == 3) {
-          tma_load_4d(sa + A_BYTES, &map_al, &full_bar[stage], c0, ws, hs, ns);
-          // stacked: the lo rows follow the hi rows inside the same N extent (maps with a box of BN / 2 rows)
-          tma_load_3d(sa + 2 * A_BYTES + (STACKED ? B_BYTES / 2 : B_BYTES), &map_bl, &full_bar[stage], c0, col0, widx);
-        }
+        tma_load_4d(sa + A_BYTES, &map_al, &full_bar[stage], c0, ws, hs, ns);
+        // stacked: the lo rows follow the hi rows inside the same N extent (maps with a box of BN / 2 rows)
+        tma_load_3d(sa + 2 * A_BYTES + (STACKED ? B_BYTES / 2 : B_BYTES), &map_bl, &full_bar[stage], c0, col0, widx);
         if (++stage == STAGES) {
           stage = 0;
           phase ^= 1;
@@ -256,10 +246,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
       // A k-step advances 32 bytes (16 fp16) inside the swizzle row; stacked, bh addresses [w_hi | w_lo].
       const int ks = ((it_beg + it + 1) % p.cchunks == 0) ? p.klast : 4;
       switch (ks) {
-        case 1: tc_stage_mma<1, 32, NSPLIT, STACKED>(part, ah, al, bh, bl); break;
-        case 2: tc_stage_mma<2, 32, NSPLIT, STACKED>(part, ah, al, bh, bl); break;
-        case 3: tc_stage_mma<3, 32, NSPLIT, STACKED>(part, ah, al, bh, bl); break;
-        default: tc_stage_mma<4, 32, NSPLIT, STACKED>(part, ah, al, bh, bl); break;
+        case 1: tc_stage_mma<1, 32, STACKED>(part, ah, al, bh, bl); break;
+        case 2: tc_stage_mma<2, 32, STACKED>(part, ah, al, bh, bl); break;
+        case 3: tc_stage_mma<3, 32, STACKED>(part, ah, al, bh, bl); break;
+        default: tc_stage_mma<4, 32, STACKED>(part, ah, al, bh, bl); break;
       }
       if (lane == 0) mbar_arrive(&empty_bar[stage]);   // this stage's MMAs have completed: free its slot
       acc.add(part);
@@ -345,7 +335,7 @@ constexpr int tc_stages(size_t stage_bytes) {
   return TC_SMEM_BUDGET / stage_bytes >= 4 ? 4 : (int)(TC_SMEM_BUDGET / stage_bytes);
 }
 
-template <int BN, int NSPLIT, bool STACKED = false>
+template <int BN, bool STACKED = false>
 int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
               const TcParams& p, dim3 grid, cudaStream_t stream) {
   constexpr size_t stage = 2 * TC_BM * 128 + (STACKED ? 1 : 2) * BN * 128;
@@ -353,12 +343,12 @@ int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
   constexpr size_t smem = (size_t)STAGES * stage + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES, STACKED, NSPLIT>,
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES, STACKED>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     configured = true;
   }
-  conv_tc_kernel<BN, STAGES, STACKED, NSPLIT><<<grid, TC_THREADS, smem, stream>>>(ah, al, bh, bl, p);
+  conv_tc_kernel<BN, STAGES, STACKED><<<grid, TC_THREADS, smem, stream>>>(ah, al, bh, bl, p);
   return (int)cudaGetLastError();
 }
 
@@ -366,22 +356,19 @@ int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
 // 96, 48, ...) each run within 8 columns of their real width
 constexpr int TC_BN_SET[] = {32, 48, 64, 96, 104, 112, 128};
 
-template <int NSPLIT>
 int launch_tc_bn(int bn, bool stacked, int stk_rows, const CUtensorMap& ah, const CUtensorMap& al,
                  const CUtensorMap& bh, const CUtensorMap& bl, const TcParams& p, dim3 grid, cudaStream_t stream) {
-  if constexpr (NSPLIT == 3) {
-    if (stacked)
-      return stk_rows == 16 ? launch_tc<32, 3, true>(ah, al, bh, bl, p, grid, stream)
-                            : launch_tc<64, 3, true>(ah, al, bh, bl, p, grid, stream);
-  }
+  if (stacked)
+    return stk_rows == 16 ? launch_tc<32, true>(ah, al, bh, bl, p, grid, stream)
+                          : launch_tc<64, true>(ah, al, bh, bl, p, grid, stream);
   switch (bn) {
-    case 32:  return launch_tc<32, NSPLIT>(ah, al, bh, bl, p, grid, stream);
-    case 48:  return launch_tc<48, NSPLIT>(ah, al, bh, bl, p, grid, stream);
-    case 64:  return launch_tc<64, NSPLIT>(ah, al, bh, bl, p, grid, stream);
-    case 96:  return launch_tc<96, NSPLIT>(ah, al, bh, bl, p, grid, stream);
-    case 104: return launch_tc<104, NSPLIT>(ah, al, bh, bl, p, grid, stream);
-    case 112: return launch_tc<112, NSPLIT>(ah, al, bh, bl, p, grid, stream);
-    case 128: return launch_tc<128, NSPLIT>(ah, al, bh, bl, p, grid, stream);
+    case 32:  return launch_tc<32>(ah, al, bh, bl, p, grid, stream);
+    case 48:  return launch_tc<48>(ah, al, bh, bl, p, grid, stream);
+    case 64:  return launch_tc<64>(ah, al, bh, bl, p, grid, stream);
+    case 96:  return launch_tc<96>(ah, al, bh, bl, p, grid, stream);
+    case 104: return launch_tc<104>(ah, al, bh, bl, p, grid, stream);
+    case 112: return launch_tc<112>(ah, al, bh, bl, p, grid, stream);
+    case 128: return launch_tc<128>(ah, al, bh, bl, p, grid, stream);
     default:  return (int)cudaErrorInvalidValue;
   }
 }
@@ -426,7 +413,7 @@ constexpr uint32_t WG_SLAB = WG_PIX * 128;     // bytes of one slab: 64 pixels x
 
 __device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr) { return wg_desc(saddr, WG_SLAB, 1024); }
 
-template <int BNW, int STAGES, int NSPLIT, int TAPS>
+template <int BNW, int STAGES, int TAPS>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_wgrad_wide_kernel(const __grid_constant__ CUtensorMap map_gh, const __grid_constant__ CUtensorMap map_gl,
                           const __grid_constant__ CUtensorMap map_xh, const __grid_constant__ CUtensorMap map_xl,
@@ -446,7 +433,7 @@ conv_tc_wgrad_wide_kernel(const __grid_constant__ CUtensorMap map_gh, const __gr
   const int ch_beg = blockIdx.z * p.chunks_per_cta;
   const int ch_end = min(p.total_chunks, ch_beg + p.chunks_per_cta);
   const int nk = ch_end - ch_beg;
-  const uint32_t tx_bytes = (NSPLIT == 3) ? 2 * A_BYTES + ne * 2 * B_BYTES : A_BYTES + ne * B_BYTES;
+  const uint32_t tx_bytes = 2 * A_BYTES + ne * 2 * B_BYTES;
   if (nk <= 0) return;
 
   if (threadIdx.x == 0) {
@@ -476,13 +463,13 @@ conv_tc_wgrad_wide_kernel(const __grid_constant__ CUtensorMap map_gh, const __gr
         uint8_t* sa = smem + (size_t)stage * STAGE_BYTES;
         mbar_expect_tx(&full_bar[stage], tx_bytes);
         tma_load_5d(sa, &map_gh, &full_bar[stage], 0, w0, h, n + gdn, aslab);
-        if (NSPLIT == 3) tma_load_5d(sa + A_BYTES, &map_gl, &full_bar[stage], 0, w0, h, n + gdn, aslab);
+        tma_load_5d(sa + A_BYTES, &map_gl, &full_bar[stage], 0, w0, h, n + gdn, aslab);
         for (int t = 0; t < ne; ++t) {
           const int e = e0 + t;
           const int xw = w0 + p.xdw[e], xh = h + p.xdh[e], xn = n + p.xdn[e];
           uint8_t* sb = sa + 2 * A_BYTES + t * 2 * B_BYTES;
           tma_load_5d(sb, &map_xh, &full_bar[stage], ci0, xw, xh, xn, 0);
-          if (NSPLIT == 3) tma_load_5d(sb + B_BYTES, &map_xl, &full_bar[stage], ci0, xw, xh, xn, 0);
+          tma_load_5d(sb + B_BYTES, &map_xl, &full_bar[stage], ci0, xw, xh, xn, 0);
         }
         if (++stage == STAGES) {
           stage = 0;
@@ -520,13 +507,12 @@ conv_tc_wgrad_wide_kernel(const __grid_constant__ CUtensorMap map_gh, const __gr
       const uint32_t sa = smem_u32(smem + (size_t)stage * STAGE_BYTES);
       const uint64_t ah = make_desc_mn(sa + cg * WG_SLAB), al = make_desc_mn(sa + A_BYTES + cg * WG_SLAB);
       const uint32_t sb = sa + 2 * A_BYTES;
-      tc_stage_mma<WG_PIX / 16, 16 * 128, NSPLIT, false>(part, ah, al, make_desc_mn(sb), make_desc_mn(sb + B_BYTES));
+      tc_stage_mma<WG_PIX / 16, 16 * 128, false>(part, ah, al, make_desc_mn(sb), make_desc_mn(sb + B_BYTES));
       acc[0].add(part);
       if constexpr (TAPS == 2) {
         if (ne == 2) {
           const uint32_t sb1 = sb + 2 * B_BYTES;
-          tc_stage_mma<WG_PIX / 16, 16 * 128, NSPLIT, false>(part, ah, al, make_desc_mn(sb1),
-                                                             make_desc_mn(sb1 + B_BYTES));
+          tc_stage_mma<WG_PIX / 16, 16 * 128, false>(part, ah, al, make_desc_mn(sb1), make_desc_mn(sb1 + B_BYTES));
           acc[1].add(part);
         }
       }
@@ -574,7 +560,7 @@ __global__ void __launch_bounds__(256) wgrad_sum_kernel(const float* __restrict_
   }
 }
 
-template <int BNW, int NSPLIT, int TAPS>
+template <int BNW, int TAPS>
 int launch_wgrad(const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap& xh, const CUtensorMap& xl,
                  const TcWgradParams& p, dim3 grid, cudaStream_t stream) {
   constexpr size_t stage = 2 * 2 * WG_SLAB + TAPS * 2 * ((BNW + WG_CH - 1) / WG_CH) * WG_SLAB;
@@ -582,29 +568,28 @@ int launch_wgrad(const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap
   constexpr size_t smem = (size_t)STAGES * stage + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_wgrad_wide_kernel<BNW, STAGES, NSPLIT, TAPS>,
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_wgrad_wide_kernel<BNW, STAGES, TAPS>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     configured = true;
   }
-  conv_tc_wgrad_wide_kernel<BNW, STAGES, NSPLIT, TAPS><<<grid, TC_THREADS, smem, stream>>>(gh, gl, xh, xl, p);
+  conv_tc_wgrad_wide_kernel<BNW, STAGES, TAPS><<<grid, TC_THREADS, smem, stream>>>(gh, gl, xh, xl, p);
   return (int)cudaGetLastError();
 }
 
 // widths up to 104 take two entries per CTA (three accumulator sets of BNW / 2 registers fit the 168 of a thread)
 constexpr int WG_PAIR_MAX_BN = 104;
 
-template <int NSPLIT>
 int launch_wgrad_bn(int bn, bool pair, const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap& xh,
                     const CUtensorMap& xl, const TcWgradParams& p, dim3 grid, cudaStream_t stream) {
   switch (bn) {
-    case 32:  return pair ? launch_wgrad<32, NSPLIT, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<32, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
-    case 48:  return pair ? launch_wgrad<48, NSPLIT, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<48, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
-    case 64:  return pair ? launch_wgrad<64, NSPLIT, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<64, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
-    case 96:  return pair ? launch_wgrad<96, NSPLIT, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<96, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
-    case 104: return pair ? launch_wgrad<104, NSPLIT, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<104, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
-    case 112: return launch_wgrad<112, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
-    case 128: return launch_wgrad<128, NSPLIT, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 32:  return pair ? launch_wgrad<32, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<32, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 48:  return pair ? launch_wgrad<48, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<48, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 64:  return pair ? launch_wgrad<64, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<64, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 96:  return pair ? launch_wgrad<96, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<96, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 104: return pair ? launch_wgrad<104, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<104, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 112: return launch_wgrad<112, 1>(gh, gl, xh, xl, p, grid, stream);
+    case 128: return launch_wgrad<128, 1>(gh, gl, xh, xl, p, grid, stream);
     default:  return (int)cudaErrorInvalidValue;
   }
 }
@@ -636,9 +621,9 @@ OG_API int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, 
                         const void* wh, const void* wl, const unsigned* amax_w, int ntaps_w, int Kw, float* y, int OH,
                         int OW, int K, long long ysn,
                         long long ysh, long long ysw, int OHf, int OWf, int osy, int osx, int opy, int opx,
-                        const int* taps_host, int ntaps, int nsplit, const float* bias, int act,
+                        const int* taps_host, int ntaps, const float* bias, int act,
                         float slope, cudaStream_t stream) {
-  if (C % 8 || K % 4 || ntaps < 1 || ntaps > TC_MAX_TAPS || (nsplit != 1 && nsplit != 3)) return (int)cudaErrorInvalidValue;
+  if (!xh || !xl || !wh || !wl || C % 8 || K % 4 || ntaps < 1 || ntaps > TC_MAX_TAPS) return (int)cudaErrorInvalidValue;
   if ((long long)N * OH * OW == 0) return 0;
   TcParams p;
   p.N = N; p.OH = OH; p.OW = OW;
@@ -702,23 +687,17 @@ OG_API int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, 
   unsigned abox[4] = {(unsigned)TC_BK, (unsigned)TW, (unsigned)TH, (unsigned)TN};
   unsigned long long bdims[3] = {(unsigned long long)C, (unsigned long long)Kw, (unsigned long long)ntaps_w};
   unsigned long long bstr[2] = {(unsigned long long)C, (unsigned long long)Kw * C};
-  // <= 32 output channels in the parity mode: [w_hi | w_lo] stacked along N (see conv_tc_kernel)
+  // <= 32 output channels: [w_hi | w_lo] stacked along N (see conv_tc_kernel)
   const int stk_rows = K <= 16 ? 16 : 32;
-  const bool stacked = nsplit == 3 && BNsel == 32 && K <= 32;
+  const bool stacked = BNsel == 32 && K <= 32;
   unsigned bbox[3] = {(unsigned)TC_BK, (unsigned)(stacked ? stk_rows : BNsel), 1u};
   int rc;
   if ((rc = make_map(&mah, xh, 4, adims, astr, abox))) return rc;
   if ((rc = make_map(&mbh, wh, 3, bdims, bstr, bbox))) return rc;
-  if (nsplit == 3) {
-    if ((rc = make_map(&mal, xl, 4, adims, astr, abox))) return rc;
-    if ((rc = make_map(&mbl, wl, 3, bdims, bstr, bbox))) return rc;
-  } else {
-    mal = mah;
-    mbl = mbh;
-  }
+  if ((rc = make_map(&mal, xl, 4, adims, astr, abox))) return rc;
+  if ((rc = make_map(&mbl, wl, 3, bdims, bstr, bbox))) return rc;
   if (p.ksplit > 1) OG_CHECK(og_work_alloc(&p.work, (size_t)p.ksplit * p.work_plane, stream));
-  rc = nsplit == 3 ? launch_tc_bn<3>(BNsel, stacked, stk_rows, mah, mal, mbh, mbl, p, grid, stream)
-                   : launch_tc_bn<1>(BNsel, stacked, stk_rows, mah, mal, mbh, mbl, p, grid, stream);
+  rc = launch_tc_bn(BNsel, stacked, stk_rows, mah, mal, mbh, mbl, p, grid, stream);
   if (p.ksplit > 1) {
     if (!rc) rc = og_split_sum(p.work, p.work_plane, p.ksplit, y, stream);
     const cudaError_t e = cudaFreeAsync(p.work, stream);
@@ -740,8 +719,8 @@ OG_API int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, 
 OG_API int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* amax_g, int N, int GN, int OH, int OW,
                               int Kp, const void* xh, const void* xl, const unsigned* amax_x, int XN, int SH, int SW,
                               int C, float* dw,
-                              int ntaps_out, const int* entries_host, int nentries, int nsplit, cudaStream_t stream) {
-  if (nentries < 1 || nentries > TC_MAX_TAPS || (nsplit != 1 && nsplit != 3) || Kp % 8 || C % 8)
+                              int ntaps_out, const int* entries_host, int nentries, cudaStream_t stream) {
+  if (!gh || !gl || !xh || !xl || nentries < 1 || nentries > TC_MAX_TAPS || Kp % 8 || C % 8)
     return (int)cudaErrorInvalidValue;
   OG_CHECK(cudaMemsetAsync(dw, 0, sizeof(float) * (size_t)ntaps_out * Kp * C, stream));
   if ((long long)N * OH * OW == 0) return 0;
@@ -819,13 +798,8 @@ OG_API int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* am
   int rc;
   if ((rc = make_map(&mgh, gh, 5, gd, gs, gb))) return rc;
   if ((rc = make_map(&mxh, xh, 5, xd, xs, xb))) return rc;
-  if (nsplit == 3) {
-    if ((rc = make_map(&mgl, gl, 5, gd, gs, gb))) return rc;
-    if ((rc = make_map(&mxl, xl, 5, xd, xs, xb))) return rc;
-  } else {
-    mgl = mgh;
-    mxl = mxh;
-  }
+  if ((rc = make_map(&mgl, gl, 5, gd, gs, gb))) return rc;
+  if ((rc = make_map(&mxl, xl, 5, xd, xs, xb))) return rc;
   // every element of an output tap has one writer unless pixel splits or several entries meet there: then each
   // (split, entry) writes its own plane of a workspace, summed in a fixed order by wgrad_sum_kernel
   bool shared_out = splits > 1;
@@ -834,8 +808,7 @@ OG_API int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* am
   p.work = nullptr;
   const long long plane = (long long)Kp * C;
   if (shared_out) OG_CHECK(og_work_alloc(&p.work, (size_t)splits * nentries * plane, stream));
-  rc = nsplit == 3 ? launch_wgrad_bn<3>(BNsel, pair, mgh, mgl, mxh, mxl, p, grid, stream)
-                   : launch_wgrad_bn<1>(BNsel, pair, mgh, mgl, mxh, mxl, p, grid, stream);
+  rc = launch_wgrad_bn(BNsel, pair, mgh, mgl, mxh, mxl, p, grid, stream);
   if (shared_out) {
     if (!rc) {
       WgradSum ws;
@@ -917,17 +890,17 @@ __global__ void __launch_bounds__(256) prep_split_kernel(const float* __restrict
 #pragma unroll
     for (int j = 0; j < 8; ++j) split_f16(v[j], scale, hi[j], lo[j]);
     *reinterpret_cast<uint4*>(xh + i * 8) = *reinterpret_cast<const uint4*>(hi);
-    if (xl) *reinterpret_cast<uint4*>(xl + i * 8) = *reinterpret_cast<const uint4*>(lo);
+    *reinterpret_cast<uint4*>(xl + i * 8) = *reinterpret_cast<const uint4*>(lo);
   }
 }
 
 // fp16 hi/lo operand copies of an NHWC fp32 tensor, scaled by the power of two that og_scale_exp derives from
 // max|x| (*amax as float bits: computed here, or, with amax_ready, left there by the kernel that produced x --
 // any upper bound of max|x| is valid, it only positions the 22-bit window).  pad = 0: plain; pad = 1: nn.ReflectionPad2d(1) halo (model.py:67)
-// materialised while splitting; s2d = 1: four space-to-depth phase blocks.  xl may be null (single-product mode).
+// materialised while splitting; s2d = 1: four space-to-depth phase blocks.
 OG_API int og_prep_split(const float* x, int N, int H, int W, int C, int pad, int s2d, unsigned* amax, int amax_ready,
                          void* xh, void* xl, cudaStream_t stream) {
-  if (C % 8 || pad < 0 || pad > 1 || (s2d && (pad || (H & 1) || (W & 1)))) return (int)cudaErrorInvalidValue;
+  if (!xh || !xl || C % 8 || pad < 0 || pad > 1 || (s2d && (pad || (H & 1) || (W & 1)))) return (int)cudaErrorInvalidValue;
   const long long n4 = (long long)N * H * W * C / 4;
   if (!amax_ready) OG_CHECK(cudaMemsetAsync(amax, 0, sizeof(unsigned), stream));
   if (n4 == 0) return 0;

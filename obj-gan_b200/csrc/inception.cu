@@ -262,7 +262,7 @@ __global__ void __launch_bounds__(256) split_s2d_kernel(const float* __restrict_
       lo[j] = __float2half_rn(s - __half2float(hi[j]));
     }
     *reinterpret_cast<uint4*>(xh + i * 8) = *reinterpret_cast<const uint4*>(hi);
-    if (xl) *reinterpret_cast<uint4*>(xl + i * 8) = *reinterpret_cast<const uint4*>(lo);
+    *reinterpret_cast<uint4*>(xl + i * 8) = *reinterpret_cast<const uint4*>(lo);
   }
 }
 
@@ -500,10 +500,10 @@ OG_API int og_bn_fold(const float* w, int Co, long long R, const float* gamma, c
   OG_RETURN_LAST_ERROR();
 }
 
-// xh / xl: [4N][ceil(H/2)][ceil(W/2)][C] (xl may be null); *amax as in og_prep_split
+// xh / xl: [4N][ceil(H/2)][ceil(W/2)][C]; *amax as in og_prep_split
 OG_API int og_prep_split_s2d(const float* x, int N, int H, int W, int C, unsigned* amax, int amax_ready, void* xh,
                              void* xl, cudaStream_t stream) {
-  if (C % 8) return (int)cudaErrorInvalidValue;
+  if (!xh || !xl || C % 8) return (int)cudaErrorInvalidValue;
   if (!amax_ready) {
     const int rc = og_amax(x, (long long)N * H * W * C, amax, stream);
     if (rc) return rc;

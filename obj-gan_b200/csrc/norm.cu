@@ -545,7 +545,7 @@ __global__ void __launch_bounds__(256) norm_apply_split_kernel(
       lo[j] = __float2half_rn(v - __half2float(hi[j]));
     }
     *reinterpret_cast<uint4*>(xh + i * 8) = *reinterpret_cast<const uint4*>(hi);
-    if (xl) *reinterpret_cast<uint4*>(xl + i * 8) = *reinterpret_cast<const uint4*>(lo);
+    *reinterpret_cast<uint4*>(xl + i * 8) = *reinterpret_cast<const uint4*>(lo);
   }
 }
 
@@ -798,13 +798,13 @@ OG_API int og_norm_bound(const float* gamma, const float* beta, int C, long long
 
 // og_norm_apply fused with og_prep_split of its output: y [N][H][W][Cy] -> fp16 hi / lo [N][H + 2 pad][W + 2 pad][Co]
 // scaled by the power of two of *bound_word (og_norm_bound), pad = 1 adds the reflection halo; out (fp32, [N][H][W][Co])
-// may be null when nothing else reads the activation; xl may be null (single-product mode).
+// may be null when nothing else reads the activation.
 OG_API int og_norm_apply_split(const float* y, int N, int H, int W, int Cy, int instance, const float* mean,
                                const float* rstd, const float* gamma, const float* beta, const float* res, int act,
                                float slope, float* out, const unsigned* bound_word, int pad, void* xh, void* xl,
                                cudaStream_t stream) {
   const int Co = act == OG_NA_GLU ? Cy / 2 : Cy;
-  if (Co % 8 || pad < 0 || pad > 1 || (pad && (H < 2 || W < 2))) return (int)cudaErrorInvalidValue;
+  if (!xh || !xl || Co % 8 || pad < 0 || pad > 1 || (pad && (H < 2 || W < 2))) return (int)cudaErrorInvalidValue;
   const long long total = (long long)N * (H + 2 * pad) * (W + 2 * pad) * (Co / 8);
   if (total == 0) return 0;
   long long b = (total + 255) / 256;

@@ -106,7 +106,7 @@ class PackedWeights:
         if key not in self.hl:
             co, ci, _, _ = w.shape
             hi = torch.empty(16 * cip * kp, device=w.device, dtype=torch.float16)
-            lo = torch.empty_like(hi) if _nsplit() == 3 else None
+            lo = torch.empty_like(hi)
             amax_up = torch.empty(1, device=w.device, dtype=torch.int32)
             _call("og_pack_upsample_weights", _p(w), co, ci, cip, kp, split, splitp, transposed, _p(self._amax(w)),
                   _p(amax_up), _p(hi), _p(lo))
@@ -120,9 +120,9 @@ class PackedWeights:
             co, ci, kh, kw = w.shape
             # hi and lo live back to back in one buffer
             nel = kh * kw * cip * kp
-            buf = torch.empty(nel * (2 if _nsplit() == 3 else 1), device=w.device, dtype=torch.float16)
+            buf = torch.empty(2 * nel, device=w.device, dtype=torch.float16)
             hi = buf[:nel]
-            lo = buf[nel:] if _nsplit() == 3 else None
+            lo = buf[nel:]
             _call("og_pack_weights_f16", _p(w), co, ci, kh, kw, cip, kp, split, splitp, transposed,
                   _p(self._amax(w)), _p(hi), _p(lo))
             self.hl[transposed] = (hi, lo, self._amax(w))
@@ -162,7 +162,7 @@ class PackPlan:
                 ab += (w.numel() + CH - 1) // CH
             co, ci, kh, kw = w.shape
             total = kh * kw * cip * kp
-            prows.append([w.data_ptr(), hi.data_ptr(), 0 if lo is None else lo.data_ptr(), amax.data_ptr(), co, ci,
+            prows.append([w.data_ptr(), hi.data_ptr(), lo.data_ptr(), amax.data_ptr(), co, ci,
                           kh * kw, cip, kp, split, splitp, tr, total, pb])
             pb += (total + CH - 1) // CH
         mk = lambda rows: h2d(rows, device, torch.int64)
@@ -190,10 +190,12 @@ class PackPlan:
 
 
 # Contraction engine for the convolutions: "f16x3" = wgmma tensor cores with the error-compensated
-# three-product fp16 hi/lo split (22-bit operands, fp32-level accuracy: the default and the parity mode), "f16" = one fp16 product
-# (faster, outside the 1e-3 parity budget), "simt" = exact fp32 FMA on the CUDA cores.
+# three-product fp16 hi/lo split (22-bit operands, fp32-level accuracy: the default), "simt" = exact fp32 FMA on the
+# CUDA cores.
 import os as _os
 CONV_ENGINE = _os.environ.get("OBJGAN_CONV", "f16x3")
+if CONV_ENGINE not in ("f16x3", "simt"):
+    raise ValueError("OBJGAN_CONV=%r: the convolution engine is 'f16x3' or 'simt'" % CONV_ENGINE)
 TC_MIN_PIXELS = 256        # smaller problems go to the exact-fp32 SIMT kernels (the tc kernel splits K on small maps)
 
 
@@ -212,23 +214,19 @@ def _empty_slack(shape, device):
     return flat[:n].view(shape)
 
 
-def _nsplit():
-    return 3 if CONV_ENGINE == "f16x3" else 1
-
-
 def _split(x, pad=0, s2d=False):
     """(fp16 hi, fp16 lo, scale word) of an NHWC tensor scaled by a power of two from its max|x|; pad=1 adds the
     reflection halo; s2d gives [4N, H/2, W/2, C]."""
     n, h, w, c = x.shape
     ready_made = getattr(x, "og_split", None)          # the producer already wrote them (og_norm_apply_split)
-    if ready_made is not None and ready_made[3:] == (pad, bool(s2d), x._version, _nsplit()):
+    if ready_made is not None and ready_made[3:] == (pad, bool(s2d), x._version):
         return ready_made[:3]
     if getattr(x, "og_f32_invalid", False):
         raise RuntimeError("this activation exists only as tensor-core operand copies (pad=%s); a consumer asked for "
                            "another layout" % (ready_made[3] if ready_made else None))
     shape = (4 * n, h // 2, w // 2, c) if s2d else (n, h + 2 * pad, w + 2 * pad, c)
     xh = _empty_slack(shape, x.device)
-    xl = _empty_slack(shape, x.device) if CONV_ENGINE == "f16x3" else None
+    xl = _empty_slack(shape, x.device)
     amax = _known_amax(x)
     ready = amax is not None
     if not ready:
@@ -265,13 +263,13 @@ def _tc_launch(xs, n, ws, ntaps_w, kw_rows, y, oh, ow, k, osy, op, taps, bias=No
     _call("og_conv2d_tc", _p(xh), _p(xl), _p(ax), n, sn, sh, sw, c, _p(wh), _p(wl), _p(aw), ntaps_w, kw_rows,
           _p(y) + 4 * yoff, oh, ow, k,
           ohf * owf * kc, owf * kc, kc, ohf, owf, osy, osy, op[0], op[1], ctypes.addressof(arr), len(taps),
-          _nsplit(), _p(bias), act, slope)
+          _p(bias), act, slope)
 
 
 def _tc_kind(n, h, w, c, kh, kw, stride, pad, mode):
     """Which tensor-core formulation (if any) applies to this convolution.  The batch need not fill the last pixel
     tile: GEMM rows are independent and rows past the batch are never stored."""
-    if CONV_ENGINE not in ("f16x3", "f16") or _lib.DRY_RUN:
+    if CONV_ENGINE != "f16x3" or _lib.DRY_RUN:
         return None
     if kh == kw and stride == 1 and pad == 1 and (kh == 3 or (kh == 4 and mode == PAD_ZERO)):
         # 3x3 (any padding mode), and the 4x4 stride-1 zero-padded roi_code layer of the object discriminators
@@ -420,7 +418,7 @@ def _tc_wgrad(kind, xs, gs, n, h, w, oh, ow, weight, c, kp, split, splitp, mode,
     arr = _int_array(ent)
     dwp = torch.empty(nt * kp * c, device=xh.device, dtype=torch.float32)
     _call("og_conv2d_wgrad_tc", _p(gh), _p(gl), _p(ag), n, gh.shape[0], oh, ow, kp, _p(xh), _p(xl), _p(ax),
-          xh.shape[0], xh.shape[1], xh.shape[2], c, _p(dwp), nt, ctypes.addressof(arr), len(ent), _nsplit())
+          xh.shape[0], xh.shape[1], xh.shape[2], c, _p(dwp), nt, ctypes.addressof(arr), len(ent))
     if mode == UPSAMPLE2X and kind == "s1":
         gw = torch.empty_like(weight)
         _call("og_unpack_upsample_wgrad", _p(dwp), co, ci, c, kp, split, splitp, _p(gw))
@@ -442,7 +440,7 @@ def _out_hw(h, w, kh, kw, stride, pad, mode):
 def _conv_raw(x, wp, n, h, w, c, oh, ow, k, kh, kw, stride, pad, mode, bias, act, splitk=True):
     y = torch.empty((n, oh, ow, k), device=x.device, dtype=torch.float32)
     _call("og_conv2d_simt", _p(x), n, h, w, c, h * w * c, w * c, c, _p(wp), _p(y), oh, ow, k, oh * ow * k, ow * k, k,
-          kh, kw, stride, pad, mode, _p(bias), act, LRELU_SLOPE, 1 if splitk else 0)
+          kh, kw, stride, pad, pad, mode, _p(bias), act, LRELU_SLOPE, 1 if splitk else 0)
     return y
 
 
@@ -600,7 +598,7 @@ class _NormAct(torch.autograd.Function):
         if res is not None:
             res = res.contiguous()
             assert res.shape == out.shape
-        fused = (split_pad is not None and CONV_ENGINE in ("f16x3", "f16") and not _lib.DRY_RUN
+        fused = (split_pad is not None and CONV_ENGINE == "f16x3" and not _lib.DRY_RUN
                  and (res is None or _known_amax(res) is not None) and (split_pad == 0 or (h > 1 and w > 1)))
         if fused:
             # the consuming convolution's operand copies straight from this pass, scaled by an a-priori bound of max|out|
@@ -608,11 +606,11 @@ class _NormAct(torch.autograd.Function):
             _call("og_norm_bound", _p(gamma), _p(beta), cy if gamma is not None else 0, P,
                   _p(_known_amax(res)) if res is not None else 0, _p(word))
             xh = _empty_slack((n, h + 2 * split_pad, w + 2 * split_pad, co), dev)
-            xl = _empty_slack((n, h + 2 * split_pad, w + 2 * split_pad, co), dev) if CONV_ENGINE == "f16x3" else None
+            xl = _empty_slack((n, h + 2 * split_pad, w + 2 * split_pad, co), dev)
             _call("og_norm_apply_split", _p(y), n, h, w, cy, 1 if instance else 0, _p(mean), _p(rstd), _p(gamma),
                   _p(beta), _p(res), act, LRELU_SLOPE, _p(out) if keep_f32 else 0, _p(word), split_pad, _p(xh), _p(xl))
             out.og_amax = (word, out._version)          # an upper bound is a valid operand scale for other consumers
-            out.og_split = (xh, xl, word, split_pad, False, out._version, _nsplit())
+            out.og_split = (xh, xl, word, split_pad, False, out._version)
             if not keep_f32:
                 out.og_f32_invalid = True               # nothing may read the fp32 tensor: it was never written
         else:
@@ -1907,7 +1905,7 @@ class EncConv:
 
     def on_tc(self, n, h, w):
         oh, ow = self.out_hw(h, w)
-        return CONV_ENGINE in ("f16x3", "f16") and n * oh * ow >= TC_MIN_PIXELS
+        return CONV_ENGINE == "f16x3" and n * oh * ow >= TC_MIN_PIXELS
 
     def macs(self, h, w):
         oh, ow = self.out_hw(h, w)
@@ -1918,7 +1916,7 @@ def _split_s2d_odd(x):
     n, h, w, c = x.shape
     shape = (4 * n, (h + 1) // 2, (w + 1) // 2, c)
     xh = _empty_slack(shape, x.device)
-    xl = _empty_slack(shape, x.device) if CONV_ENGINE == "f16x3" else None
+    xl = _empty_slack(shape, x.device)
     amax = torch.empty(1, device=x.device, dtype=torch.int32)
     _call("og_prep_split_s2d", _p(x), n, h, w, c, _p(amax), 0, _p(xh), _p(xl))
     return xh, xl, amax
@@ -1952,7 +1950,7 @@ def enc_conv_fwd(layer, x, y, yoff=0):
         _tc_launch(xs, n, ws, kk, k, y, oh, ow, k, 1, (0, 0), taps, bias, layer.act, yoff=yoff, slope=0.0)
     else:
         wp, _ = cache.get(wf, c, k, 0, 0, False)
-        _call("og_conv2d_simt_pad2", _p(x), n, h, w, c, h * w * c, w * c, c, _p(wp), yptr, oh, ow, k, ystr[0], ystr[1],
+        _call("og_conv2d_simt", _p(x), n, h, w, c, h * w * c, w * c, c, _p(wp), yptr, oh, ow, k, ystr[0], ystr[1],
               ystr[2], layer.kh, layer.kw, layer.stride, layer.padh, layer.padw, PAD_ZERO, _p(bias), layer.act, 0.0,
               1 if (bias is None and layer.act == ACT_NONE and yoff == 0 and cy == k) else 0)
 
@@ -1978,7 +1976,7 @@ def enc_conv_dgrad(layer, gp, h, w):
             _tc_launch(gs, n, ws, layer.kh * layer.kw, c, gx, h, w, c, 1, (0, 0), taps, slope=0.0)
     else:
         _, wt = cache.get(wf, c, k, 0, 0, True)
-        _call("og_conv2d_simt_pad2", _p(gp), n, oh, ow, k, oh * ow * k, ow * k, k, _p(wt), _p(gx), h, w, c, h * w * c,
+        _call("og_conv2d_simt", _p(gp), n, oh, ow, k, oh * ow * k, ow * k, k, _p(wt), _p(gx), h, w, c, h * w * c,
               w * c, c, layer.kh, layer.kw, layer.stride, layer.padh, layer.padw, TRANSPOSED, 0, ACT_NONE, 0.0, 1)
     return gx
 

@@ -66,9 +66,9 @@ def _stage_groups(sass_lines):
     return groups
 
 
-def test_stage_mmas_issue_as_one_group(compiled):
-    """The widest HGMMA group of each kernel is a whole stage: 4 k-steps x products x column blocks (one wide MMA per
-    product in the fprop / dgrad kernel; 64-wide blocks plus a tail in the weight-gradient kernel)."""
+def test_stage_of_three_products_issues_as_one_group(compiled):
+    """The widest HGMMA group of each kernel is a whole stage: 4 k-steps x 3 products, or x 2 in the stacked form
+    (one wide MMA per product and k-step in the fprop / dgrad and in the weight-gradient kernel)."""
     obj, _ = compiled
     cuobjdump = os.path.join(os.path.dirname(NVCC), "cuobjdump")
     if not os.path.exists(cuobjdump):
@@ -88,14 +88,12 @@ def test_stage_mmas_issue_as_one_group(compiled):
     checked = 0
     for f, lines in funcs.items():
         name = names[f]
-        m = re.search(r"conv_tc_kernel<(\d+), (\d+), (true|false), (\d+)>", name)
-        w = re.search(r"conv_tc_wgrad_kernel<(\d+), (\d+), (\d+)>", name)
+        m = re.search(r"conv_tc_kernel<(\d+), (\d+), (true|false)>", name)
+        w = re.search(r"conv_tc_wgrad_wide_kernel<(\d+), (\d+), (\d+)>", name)
         if m:
-            products = 2 if m.group(3) == "true" else int(m.group(4))
-            want = 4 * products
+            want = 4 * (2 if m.group(3) == "true" else 3)
         elif w:
-            bnw, nsplit = int(w.group(1)), int(w.group(3))
-            want = 4 * nsplit * (bnw // 64 + (1 if bnw % 64 else 0))
+            want = 4 * 3
         else:
             continue
         groups = _stage_groups(lines)

@@ -1,5 +1,5 @@
 """The weight-gradient kernel of conv_tc.cu in SASS, checked without a GPU: every instantiated ci width issues one
-wgmma over its whole (MN-major, several-slab) B extent per product and k-step, so a stage is 4 x products HGMMAs in
+wgmma over its whole (MN-major, several-slab) B extent per product and k-step, so a stage is 4 x 3 HGMMAs in
 one run that ends in its own wait (twice per stage when two entries share the G tile), with no C75xx serialization
 note and no spills."""
 import os
@@ -33,16 +33,16 @@ def _demangle(names):
 
 
 def _wgrad(name):
-    """(ci width, products, entries per CTA) of a weight-gradient kernel instantiation."""
-    m = re.search(r"conv_tc_wgrad\w*<(\d+), (\d+), (\d+), (\d+)>", name)
-    return (int(m.group(1)), int(m.group(3)), int(m.group(4))) if m else None
+    """(ci width, entries per CTA) of a weight-gradient kernel instantiation."""
+    m = re.search(r"conv_tc_wgrad\w*<(\d+), (\d+), (\d+)>", name)
+    return (int(m.group(1)), int(m.group(3))) if m else None
 
 
 # every width with one entry per CTA; widths up to 104 also with two entries sharing the G tile
-KERNELS = {(w, s, t) for w in WIDTHS for s in (1, 3) for t in (1, 2) if t == 1 or w <= 104}
+KERNELS = {(w, t) for w in WIDTHS for t in (1, 2) if t == 1 or w <= 104}
 
 
-def test_wgrad_no_serialization_or_spills(compiled):
+def test_wgrad_kernels_no_serialization_or_spills(compiled):
     _, log = compiled
     notes = [ln for ln in log.splitlines() if re.search(r"\(C75\d\d\)", ln)]
     assert not notes, "\n".join(notes[:10])
@@ -58,7 +58,7 @@ def test_wgrad_no_serialization_or_spills(compiled):
     assert all(v == (0, 0) for v in spills.values()), spills
 
 
-def test_wgrad_stage_is_one_wide_mma_per_product(compiled):
+def test_wgrad_stage_is_one_wide_mma_per_product_and_k_step(compiled):
     obj, _ = compiled
     cuobjdump = os.path.join(os.path.dirname(NVCC), "cuobjdump")
     if not os.path.exists(cuobjdump):
@@ -79,7 +79,7 @@ def test_wgrad_stage_is_one_wide_mma_per_product(compiled):
         key = _wgrad(name)
         if not key:
             continue
-        bnw, nsplit, _ = key
+        bnw, _ = key
         groups, n, shapes = [], 0, set()
         for ln in funcs[f]:
             if "HGMMA" in ln:
@@ -88,7 +88,7 @@ def test_wgrad_stage_is_one_wide_mma_per_product(compiled):
             elif "WARPGROUP.DEPBAR" in ln:
                 groups.append(n)
                 n = 0
-        assert groups and max(groups) == 4 * nsplit, (name, groups)
+        assert groups and max(groups) == 4 * 3, (name, groups)
         assert shapes == {str(bnw)}, (name, shapes)
         seen.add(key)
     assert seen == KERNELS, sorted(seen)

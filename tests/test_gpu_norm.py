@@ -287,7 +287,7 @@ def _scale_exp(bound):
     return 13 - math.floor(math.log2(bound))
 
 
-def _split_run(instance, N, H, W, Cy, act, residual, pad, two, y=None, gamma=None, beta=None, res=None):
+def _split_run(instance, N, H, W, Cy, act, residual, pad, y=None, gamma=None, beta=None, res=None):
     Co = Cy // 2 if act == NA_GLU else Cy
     G, P = (N, H * W) if instance else (1, N * H * W)
     if y is None:
@@ -307,7 +307,7 @@ def _split_run(instance, N, H, W, Cy, act, residual, pad, two, y=None, gamma=Non
     bound = word.view(torch.float32).item()
     Hp, Wp = H + 2 * pad, W + 2 * pad
     xh = torch.empty(N, Hp, Wp, Co, device=DEV, dtype=torch.float16)
-    xl = torch.empty_like(xh) if two else None
+    xl = torch.empty_like(xh)
     out = torch.empty_like(out_apply)
     _call("og_norm_apply_split", y, N, H, W, Cy, instance, mean, rstd, gamma, beta, res, act, SLOPE, out, word, pad,
           xh, xl)
@@ -316,7 +316,7 @@ def _split_run(instance, N, H, W, Cy, act, residual, pad, two, y=None, gamma=Non
 
 @pytest.mark.parametrize("case", SPLIT_CASES, ids=lambda c: "-".join(map(str, c)))
 def test_norm_apply_split(case):
-    instance, N, H, W, Cy, act, residual, pad, two = case
+    instance, N, H, W, Cy, act, residual, pad = case
     out_apply, out, xh, xl, bound = _split_run(*case)
     assert _ulps(out, out_apply) <= 1                        # same arithmetic as og_norm_apply
     assert bound >= out_apply.abs().max().item()
@@ -328,9 +328,8 @@ def test_norm_apply_split(case):
         hi = xh.permute(0, 3, 1, 2).float()
         assert torch.equal(F.pad(hi[:, :, 1:-1, 1:-1], (1, 1, 1, 1), mode="reflect"), hi)   # halo = reflection
     want = want.permute(0, 2, 3, 1)
-    rec = xh.double() + (xl.double() if two else 0)
-    rec = rec * 2.0 ** -k
-    rel = 2.0 ** -22 if two else 2.0 ** -11
+    rec = (xh.double() + xl.double()) * 2.0 ** -k
+    rel = 2.0 ** -22
     err = ((rec - want).abs() / torch.clamp(want.abs() * rel, min=bound * 2.0 ** -38)).max().item()
     _note("og_norm_apply_split reconstruction (x bound)", err)
     assert err <= 1.0, err
@@ -358,8 +357,8 @@ def test_norm_bound_adversarial(instance, act):
     res = torch.zeros(G, P, Co, device=DEV)
     res[:, 0, :] = 2.0
     res[:, 1, :] = -1.0
-    out_apply, out, xh, xl, bound = _split_run(instance, N, H, W, Cy, act, True, 1, True, y=y, gamma=gamma,
-                                               beta=beta, res=res)
+    out_apply, out, xh, xl, bound = _split_run(instance, N, H, W, Cy, act, True, 1, y=y, gamma=gamma, beta=beta,
+                                               res=res)
     mx = out_apply.abs().max().item()
     assert bound >= mx, (bound, mx)
     if act != NA_GLU or instance:   # (BatchNorm + GLU: the bound counts the gate half's max|beta| too)

@@ -194,7 +194,7 @@ def _record_calls(fn):
     return log
 
 
-def test_dry_run_call_sequences():
+def test_dry_run_library_calls():
     """The forwards issue library calls only; the FID program stops at its last block; CNN_ENCODER's forward and
     input-gradient calls are the ones recorded before the trunk builder was shared."""
     lib.DRY_RUN = True
