@@ -702,6 +702,8 @@ OG_API int og_paint_max_fwd(const float* f, const float* m, int B, int num, int 
     return 0;
   }
   size_t sm = sizeof(float) * (num * R + R * PAINT_PIX);
+  if (sm > 48 * 1024)
+    OG_CHECK(cudaFuncSetAttribute(paint_max_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
   dim3 grid(og_cdiv(P, PAINT_PIX), B);
   paint_max_fwd_kernel<<<grid, 256, sm, stream>>>(f, m, num, R, Rtot, P, out, dstride, doff);
   OG_RETURN_LAST_ERROR();
