@@ -417,6 +417,10 @@ int og_softmax_rows(const float* x, int rows, int C, float* y, cudaStream_t stre
 int og_moments_f64(const float* x, int n, int d, int init, double* k, double* s1, double* s2, cudaStream_t stream);
 int og_relu_grad_slice(const float* y, int ldy, int yoff, const float* g, int ldg, int goff, float* out, int ldo,
                        int ooff, int nch, long long P, int relu, cudaStream_t stream);
+/* og_images_to_u8: NCHW (N, 3, H, W) fp32 images -> NHWC (N, H, W, 3) bytes with the arithmetic of the evaluator's
+ * save_singleimages (ref: evaluator.py:235-237): round(round(x + 1) * 0.5 * 255), clamped to [0, 255], truncated
+ * toward zero; NaN gives 0 (csrc/elementwise.cu). */
+int og_images_to_u8(const float* x, int N, int H, int W, unsigned char* out, cudaStream_t stream);
 
 #ifdef __cplusplus
 }

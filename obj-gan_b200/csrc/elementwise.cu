@@ -680,3 +680,29 @@ OG_API int og_permute_channels(const float* x, const long long* perm, int B, int
   permute_channels_kernel<<<dim3(bx, C, B), 256, 0, stream>>>(x, perm, C, P, out);
   OG_RETURN_LAST_ERROR();
 }
+
+// NCHW (N, 3, H, W) fp32 images in [-1, 1] -> NHWC (N, H, W, 3) uint8, the arithmetic of the reference's
+// save_singleimages (ref: evaluator.py:235-237): x.add(1).div(2).mul(255).clamp(0, 255).byte(), then permute(1, 2, 0).
+// Each step is rounded on its own (__fadd_rn / __fmul_rn: no contraction into an FMA may move a value across a byte
+// boundary); the halving is exact.  The clamp then the truncation toward zero of .byte(); fmaxf maps NaN to 0.
+__global__ void __launch_bounds__(256) images_to_u8_kernel(const float* __restrict__ x, long long HW, long long total,
+                                                           unsigned char* __restrict__ out) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const long long n = i / HW, p = i - n * HW;
+    const float* xp = x + n * 3 * HW + p;
+    unsigned char* op = out + i * 3;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      float v = __fmul_rn(__fmul_rn(__fadd_rn(__ldg(xp + c * HW), 1.f), 0.5f), 255.f);
+      v = fminf(fmaxf(v, 0.f), 255.f);
+      op[c] = (unsigned char)__float2uint_rz(v);
+    }
+  }
+}
+OG_API int og_images_to_u8(const float* x, int N, int H, int W, unsigned char* out, cudaStream_t stream) {
+  const long long total = (long long)N * H * W;
+  if (total == 0) return 0;
+  images_to_u8_kernel<<<eblocks(total), 256, 0, stream>>>(x, (long long)H * W, total, out);
+  OG_RETURN_LAST_ERROR();
+}

@@ -483,6 +483,40 @@ class _Moments:
         ops.moments_f64(x, self.k, self.s1, self.s2, self.n == 0)
         self.n += x.shape[0]
 
+    def symmetric_s2(self):
+        """s2 with both triangles filled (og_moments_f64 writes the 32-wide tiles on or above the diagonal)."""
+        t = torch.arange(self.dims, device=self.s2.device) // 32
+        return torch.where(t[:, None] <= t[None, :], self.s2, self.s2.T)
+
+    @classmethod
+    def from_sums(cls, n, k, s1, s2):
+        """Moments of ``n`` rows from their float64 shifted sums (s2 symmetric or upper-tiled)."""
+        m = cls(k.shape[0])
+        m.n = int(n)
+        if m.n > 0:
+            m.k, m.s1, m.s2 = k, s1, s2
+        return m
+
+    def merge(self, others):
+        """These moments combined with ``others`` (_Moments of other row sets, e.g. the other data-parallel ranks'),
+        in float64 torch ops: every s2 is symmetrised, every set of sums is re-centred on this one's shift k with
+        delta = k_j - k (S1 += n_j delta, S2 += S1_j delta^T + delta S1_j^T + n_j delta delta^T), and the re-centred
+        sums are added.  Sets without rows are skipped.  Returns a new _Moments."""
+        parts = [m for m in (self, *others) if m.n > 0]
+        if not parts:
+            return _Moments(self.dims)
+        k = parts[0].k
+        s1 = torch.zeros_like(parts[0].s1)
+        s2 = torch.zeros_like(parts[0].s2)
+        n = 0
+        for m in parts:
+            d = m.k.to(k.device) - k
+            m1, m2 = m.s1.to(k.device), m.symmetric_s2().to(k.device)
+            s1 += m1 + m.n * d
+            s2 += m2 + torch.outer(m1, d) + torch.outer(d, m1) + m.n * torch.outer(d, d)
+            n += m.n
+        return _Moments.from_sums(n, k, s1, s2)
+
     def statistics(self):
         """(mu (d,), sigma (d, d)) float64; sigma as np.cov(rowvar=False), with n - 1."""
         import numpy as np

@@ -2162,3 +2162,17 @@ def moments_f64(x, k, s1, s2, init):
     _chk(x, k, s1, s2)
     x = x.detach().float().contiguous()
     _call("og_moments_f64", _p(x), x.shape[0], x.shape[1], 1 if init else 0, _p(k), _p(s1), _p(s2))
+
+
+def images_to_u8(x):
+    """(N, 3, H, W) fp32 images in [-1, 1] -> (N, H, W, 3) uint8 on the device (og_images_to_u8): bitwise the
+    reference's x.add(1).div(2).mul(255).clamp(0, 255).byte().permute(1, 2, 0) per image (ref: evaluator.py:235-237),
+    with NaN -> 0.  A quarter of the float images' bytes crosses to the host for the JPEG encoder."""
+    _chk(x)
+    x = x.detach().contiguous()
+    n, c, h, w = x.shape
+    if c != 3 or x.dtype != torch.float32:
+        raise ValueError(f"images_to_u8 takes (N, 3, H, W) float32 images, got {tuple(x.shape)} {x.dtype}")
+    out = torch.empty((n, h, w, 3), device=x.device, dtype=torch.uint8)
+    _call("og_images_to_u8", _p(x), n, h, w, _p(out))
+    return out

@@ -402,9 +402,12 @@ class GSampler:
         hmaps, bt_masks, fm_bt_masks = ops.form_gen_hmaps(raw_masks, dev["roi_cls"], dev["num_rois"], IMG_SIZES, nbf)
         return dict(raw_masks=raw_masks, bbox_fmaps=fmaps, hmaps=hmaps, bt_masks=bt_masks, fm_bt_masks=fm_bt_masks)
 
-    def _forward(self, dev: dict):
+    def _forward(self, dev: dict, text_out: dict | None = None):
         if "captions" in dev:
-            dev = dict(dev, **self._text(dev))
+            text = self._text(dev)
+            if text_out is not None:
+                text_out.update(text)
+            dev = dict(dev, **text)
         if "noise_shp" in dev:
             d = dict(dev, **self._shapes(dev))
             d["slabels_feat"] = ops.form_clabels_feat(dev["clabels_emb"], dev["roi_cls"], dev["num_rois"],
@@ -418,10 +421,11 @@ class GSampler:
             g.ca_net.eps_override = None
 
     # ------------------------------------------------------------------ sampling
-    def sample_eager(self, inp: dict):
-        """The same forward pass without graphs."""
+    def sample_eager(self, inp: dict, text_out: dict | None = None):
+        """The same forward pass without graphs.  ``text_out``: a dict that receives the text stage's outputs
+        (``words_embs``, ``sent_emb``, ``mask``, ``glove_words_embs``) of a caption batch, for R-precision."""
         with torch.no_grad():
-            return self._forward(self._prepare(inp, eager=True))
+            return self._forward(self._prepare(inp, eager=True), text_out)
 
     def sample_shapes(self, inp: dict) -> dict:
         """The generated shapes of a batch without masks (eager): ``raw_masks`` (B, R, 64, 64), the SHP_G_NET output the

@@ -215,3 +215,77 @@ def reference_encoders(directory: str, n_words: int = 200, seed: int = 0) -> str
                os.path.join(directory, "text_encoder100.pth"))
     torch.save(model.CNN_ENCODER(cfg.TEXT.EMBEDDING_DIM).state_dict(), os.path.join(directory, "image_encoder100.pth"))
     return os.path.join(directory, "text_encoder100.pth")
+
+
+def loader_box_maps(rois0, fm_rois, num_rois, num_classes: int = 80):
+    """The box maps of the reference's test loader, float64 (ref: miscc/load.py:621-645 rasterises, 178-212 places
+    them per slot): bbox_maps_fwd (B, BOXES_NUM, num_classes, 64, 64) with box r of its class in slot r,
+    bbox_maps_bwd the slots reversed, and bbox_fmaps (B, BOXES_NUM, 16, 16) from fm_rois / 2.  A box covers
+    [round(y), round(y + h)) x [round(x), round(x + w)), each edge min(round-half-even(v), size - 1)."""
+    boxes, s, fs = cfg.ROI.BOXES_NUM, IMG_SIZES[0], cfg.ROI.FM_SIZE
+    edge = lambda v, size: min(int(round(float(v))), size - 1)
+    r0, fm = np.asarray(rois0, dtype=np.float64), np.asarray(fm_rois, dtype=np.float64)
+    b = r0.shape[0]
+    fwd = np.zeros((b, boxes, num_classes, s, s))
+    fmaps = np.zeros((b, boxes, fs, fs))
+    for i in range(b):
+        for r in range(int(num_rois[i])):
+            x, y, w, h = r0[i, r, :4]
+            fwd[i, r, int(r0[i, r, 4]), edge(y, s):edge(y + h, s), edge(x, s):edge(x + w, s)] = 1
+            x, y, w, h = fm[i, r, :4] / 2.0
+            fmaps[i, r, edge(y, fs):edge(y + h, fs), edge(x, fs):edge(x + w, fs)] = 1
+    fwd = torch.from_numpy(fwd)
+    return fwd, fwd.flip(1).contiguous(), torch.from_numpy(fmaps)
+
+
+def reference_test_batch(batch: int, seed: int = 1234, mode: int = 2, *, lens=None, full_maps: bool = True,
+                         max_rois: int | None = None, n_words: int = 200, n_glove: int = 200, num_classes: int = 80,
+                         fid_dims: int = 2048):
+    """One batch in the format the reference's DataLoader collates from ``TestDataset.__getitem__`` (ref:
+    testDataset.py:67-103): for ``mode`` (cfg.TEST.USE_GT_BOX_SEG) 0 / 1 the 17 fields (imgs, acts, captions
+    (B, 18, 1), glove_captions, cap_lens UNSORTED, hmaps, bbox_maps_fwd, bbox_maps_bwd, bbox_fmaps, rois, fm_rois,
+    num_rois, bt_masks, fm_bt_masks, class_ids, keys, sent_ids), for mode 2 the 14 without hmaps and masks.  Captions,
+    layout, masks and images are ``reference_batch``'s; ``acts`` are float64 (B, fid_dims) activations (float32
+    values, non-negative like pooled ReLU features); ``sent_ids`` index * 5 + a seeded caption index.
+
+    The box maps are float64 (B, BOXES_NUM, num_classes, 64, 64) / (B, BOXES_NUM, 16, 16), rasterised from the box
+    tables like the reference's loader (``loader_box_maps``).  ``full_maps`` False: the box maps and heat maps are
+    zero-stride float64 views of their shapes instead (no memory; an intake that never reads them cannot tell)."""
+    data = reference_batch(batch, seed, lens=lens, max_rois=max_rois, n_words=n_words, n_glove=n_glove,
+                           num_classes=num_classes)
+    imgs, caps, gcaps, lens, hmaps, rois, fm_rois, num_rois, bt_masks, fm_bt_masks, class_ids, keys = data
+    g = torch.Generator().manual_seed(seed + 2)
+    acts = torch.randn(batch, fid_dims, generator=g).abs().double()
+    sent_ids = torch.arange(batch) * cfg.TEXT.CAPTIONS_PER_IMAGE + torch.randint(0, cfg.TEXT.CAPTIONS_PER_IMAGE,
+                                                                                  (batch,), generator=g)
+    boxes, s, fs = cfg.ROI.BOXES_NUM, IMG_SIZES[0], cfg.ROI.FM_SIZE
+    if full_maps:
+        fwd, bwd, fmaps = loader_box_maps(rois[0], fm_rois, num_rois, num_classes)
+    else:
+        zero = torch.zeros((), dtype=torch.float64)
+        fwd = bwd = zero.expand(batch, boxes, num_classes, s, s)
+        fmaps = zero.expand(batch, boxes, fs, fs)
+        hmaps = [zero.expand(h.shape) for h in hmaps]
+    keys = [k.replace("train", "val") for k in keys]
+    if mode == 2:
+        return (imgs, acts, caps, gcaps, lens, fwd, bwd, fmaps, rois, fm_rois, num_rois, class_ids, keys, sent_ids)
+    return (imgs, acts, caps, gcaps, lens, hmaps, fwd, bwd, fmaps, rois, fm_rois, num_rois, bt_masks, fm_bt_masks,
+            class_ids, keys, sent_ids)
+
+
+def reference_test_dataset(n_words: int = 200, n_glove: int = 200, num_classes: int = 80, seed: int = 0):
+    """An object with the attributes the reference's condGANEvaluator reads from its ``TestDataset``: those of
+    ``reference_dataset``, and ``acts_dict`` None (no activation file read yet)."""
+    ds = reference_dataset(n_words, n_glove, num_classes, seed)
+    ds.acts_dict = None
+    return ds
+
+
+def reference_acts_batches(batch: int, n: int, seed: int = 1234):
+    """``n`` batches as the reference's DataLoader collates them from ``TestDataset.__getitem__`` before the
+    activation file exists (ref: testDataset.py:76-77): (imgs, keys), the images of ``make_inputs``."""
+    out = []
+    for i in range(n):
+        inp = make_inputs(batch, seed + i, parity=True)
+        out.append((inp["imgs"], [f"COCO_val2014_{seed + i:06d}{j:06d}" for j in range(batch)]))
+    return out

@@ -60,6 +60,26 @@ def text_stage(text_encoder, glove, captions, cap_lens, glove_captions, max_len:
     return dict(words_embs=words, sent_emb=sent, mask=mask, glove_words_embs=glove_words)
 
 
+def _length_sort(cap_lens):
+    """(order, order as a list, take) for a batch sorted by caption length, longest first, with a stable sort:
+    ``take(t, dtype=None)`` gathers the per-sample tensor ``t`` into that order, converting it to ``dtype`` in the
+    same pass, into pinned memory when CUDA is available."""
+    order = torch.sort(cap_lens, dim=0, descending=True, stable=True).indices
+    pin = torch.cuda.is_available()          # a copy from pageable memory blocks the host until the GPU drains
+    idx = order.tolist()
+
+    def take(t, dtype=None):
+        t = torch.as_tensor(t)
+        out = torch.empty(t.shape, dtype=dtype or t.dtype, pin_memory=pin)
+        if out.dtype == t.dtype:
+            return torch.index_select(t, 0, order, out=out)
+        for j, i in enumerate(idx):          # gather and convert in one pass (the float64 masks: ~110 MB at batch 16)
+            out[j].copy_(t[i])
+        return out
+
+    return order, idx, take
+
+
 def prepare_reference_batch(data):
     """The reference's ``prepare_data`` (ref: trainDataset.py:79-128) on the host, producing the compact batch that
     ``StepATrainer.to_device`` takes.  ``data`` is what the reference's DataLoader collates from
@@ -80,21 +100,10 @@ def prepare_reference_batch(data):
         keys = data
     cap_lens = torch.as_tensor(cap_lens).to(torch.int64).view(-1)
     b = cap_lens.shape[0]
-    order = torch.sort(cap_lens, dim=0, descending=True, stable=True).indices
-    pin = torch.cuda.is_available()          # a copy from pageable memory blocks the host until the GPU drains
-    idx = order.tolist()
-
-    def take(t, dtype=None):
-        t = torch.as_tensor(t)
-        out = torch.empty(t.shape, dtype=dtype or t.dtype, pin_memory=pin)
-        if out.dtype == t.dtype:
-            return torch.index_select(t, 0, order, out=out)
-        for j, i in enumerate(idx):          # gather and convert in one pass (the float64 masks: ~110 MB at batch 16)
-            out[j].copy_(t[i])
-        return out
-
+    order, idx, take = _length_sort(cap_lens)
     rois = [take(r) for r in rois]
-    roi_cls = torch.empty(rois[0].shape[:2], dtype=torch.int64, pin_memory=pin).copy_(rois[0][..., 4])
+    roi_cls = torch.empty(rois[0].shape[:2], dtype=torch.int64, pin_memory=torch.cuda.is_available())
+    roi_cls.copy_(rois[0][..., 4])
     batch = dict(imgs=[take(x) for x in imgs], captions=take(torch.as_tensor(captions).reshape(b, -1)),
                  glove_captions=take(torch.as_tensor(glove_captions).reshape(b, -1)), cap_lens=take(cap_lens),
                  rois=rois, fm_rois=take(fm_rois), num_rois=take(torch.as_tensor(num_rois).to(torch.int64).view(-1)),
@@ -104,6 +113,81 @@ def prepare_reference_batch(data):
     batch["max_len"] = int(cap_lens.max())
     batch["host_boxes"] = {"rois": rois, "fm_rois": batch["fm_rois"], "num_rois": batch["num_rois"]}
     return batch, torch.as_tensor(class_ids)[order].numpy(), [keys[i] for i in idx]
+
+
+TEST_TUPLE_LEN = {0: 17, 1: 17, 2: 14}     # TestDataset.__getitem__ per cfg.TEST.USE_GT_BOX_SEG (testDataset.py:89-103)
+
+
+def prepare_reference_test_batch(data, mode=None):
+    """The reference's test-time ``prepare_data`` / ``prepare_gen_data`` (ref: testDataset.py:109-244) on the host,
+    producing the compact batch that ``GSampler.sample_eager`` takes.  ``data`` is what the reference's DataLoader
+    collates from ``TestDataset.__getitem__``: for ``mode`` (cfg.TEST.USE_GT_BOX_SEG when None) 0 or 1 the 17 fields
+    (imgs, acts, captions, glove_captions, cap_lens, hmaps, bbox_maps_fwd, bbox_maps_bwd, bbox_fmaps, rois, fm_rois,
+    num_rois, bt_masks, fm_bt_masks, class_ids, keys, sent_ids), for mode 2 the 14 without hmaps and masks.  A tuple
+    of the other length raises ValueError.
+
+    The sort is ``prepare_reference_batch``'s (stable, longest caption first).  Never read: the images (the evaluator
+    scores generated images only), the float64 box maps (~420 MB each at batch 16; ``GSampler`` rasterises them on
+    the device from ``rois[0]``, ``fm_rois``, the roi classes and ``num_rois`` with the loader's own rules,
+    ops.form_bbox_maps) and the float64 heat maps (rebuilt on the device from the masks, unclamped, ``hmap_clamp``
+    0).  Mode 0 keeps the ground-truth masks as float32; modes 1 and 2 send no masks, so the sampler generates them.
+    The box tables keep their float64.
+
+    Returns (batch, acts, class_ids, keys, sent_ids), all in the sorted order: the batch dict (with ``max_len`` =
+    max(cap_lens)), the real images' FID activations as a float64 tensor, the class ids as a numpy array, and the
+    keys and sentence ids as lists."""
+    mode = cfg.TEST.USE_GT_BOX_SEG if mode is None else mode
+    if mode not in TEST_TUPLE_LEN:
+        raise ValueError(f"cfg.TEST.USE_GT_BOX_SEG must be 0, 1 or 2, got {mode}")
+    if len(data) != TEST_TUPLE_LEN[mode]:
+        raise ValueError(f"USE_GT_BOX_SEG = {mode} takes the {TEST_TUPLE_LEN[mode]}-field test tuple, got "
+                         f"{len(data)} fields")
+    if mode == 2:
+        _imgs, acts, captions, glove_captions, cap_lens, _fwd, _bwd, _fmaps, rois, fm_rois, num_rois, class_ids, keys, \
+            sent_ids = data
+    else:
+        _imgs, acts, captions, glove_captions, cap_lens, _hmaps, _fwd, _bwd, _fmaps, rois, fm_rois, num_rois, bt_masks, \
+            fm_bt_masks, class_ids, keys, sent_ids = data
+    cap_lens = torch.as_tensor(cap_lens).to(torch.int64).view(-1)
+    b = cap_lens.shape[0]
+    order, idx, take = _length_sort(cap_lens)
+    rois = [take(r) for r in rois]
+    roi_cls = torch.empty(rois[0].shape[:2], dtype=torch.int64, pin_memory=torch.cuda.is_available())
+    roi_cls.copy_(rois[0][..., 4])
+    batch = dict(captions=take(torch.as_tensor(captions).reshape(b, -1)),
+                 glove_captions=take(torch.as_tensor(glove_captions).reshape(b, -1)), cap_lens=take(cap_lens),
+                 rois=rois, fm_rois=take(fm_rois), num_rois=take(torch.as_tensor(num_rois).to(torch.int64).view(-1)),
+                 roi_cls=roi_cls)
+    if mode == 0:
+        batch.update(bt_masks=[take(m, torch.float32) for m in bt_masks], fm_bt_masks=take(fm_bt_masks, torch.float32),
+                     hmap_clamp=0.0)
+    batch["glb_max_num_roi"] = int(batch["num_rois"].max())
+    batch["max_len"] = int(cap_lens.max())
+    sent_ids = torch.as_tensor(sent_ids).view(-1).tolist()
+    return (batch, take(acts), torch.as_tensor(class_ids)[order].numpy(), [keys[i] for i in idx],
+            [sent_ids[i] for i in idx])
+
+
+def gather_inception_score(score, world, rank, process_group=None):
+    """An InceptionScore over every data-parallel rank's predictions: one gather to rank 0 (None on the other ranks).
+    Rank r's predictions follow rank r-1's."""
+    if world == 1:
+        return score
+    local = torch.cat(score.predictions, 0)
+    n = torch.tensor([local.shape[0]], device=local.device, dtype=torch.int64)
+    counts = [torch.zeros_like(n) for _ in range(world)]
+    dist.all_gather(counts, n, group=process_group)
+    counts = [int(c) for c in counts]
+    pad = local.new_zeros((max(counts), local.shape[1]))
+    pad[:local.shape[0]] = local
+    parts = [torch.empty_like(pad) for _ in range(world)]
+    dist.all_gather(parts, pad, group=process_group)
+    if rank != 0:
+        return None
+    out = losses.InceptionScore(score.num_splits)
+    for p, c in zip(parts, counts):
+        out.add(p[:c])
+    return out
 
 
 class FlatBucket:
@@ -727,23 +811,7 @@ class condGANTrainer:
     def epoch_score(self, score):
         """The epoch's InceptionScore over every rank's predictions: one gather to rank 0 (None on the other
         ranks).  Rank r's predictions follow rank r-1's."""
-        if self.world == 1:
-            return score
-        local = torch.cat(score.predictions, 0)
-        n = torch.tensor([local.shape[0]], device=local.device, dtype=torch.int64)
-        counts = [torch.zeros_like(n) for _ in range(self.world)]
-        dist.all_gather(counts, n, group=self.pg)
-        counts = [int(c) for c in counts]
-        pad = local.new_zeros((max(counts), local.shape[1]))
-        pad[:local.shape[0]] = local
-        parts = [torch.empty_like(pad) for _ in range(self.world)]
-        dist.all_gather(parts, pad, group=self.pg)
-        if self.rank != 0:
-            return None
-        out = losses.InceptionScore(score.num_splits)
-        for p, c in zip(parts, counts):
-            out.add(p[:c])
-        return out
+        return gather_inception_score(score, self.world, self.rank, self.pg)
 
     def write_score(self, epoch, score):
         """Score/scores_%d.txt in the reference's format (ref: trainer.py:495-506)."""
