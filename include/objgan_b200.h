@@ -422,6 +422,21 @@ int og_relu_grad_slice(const float* y, int ldy, int yoff, const float* g, int ld
  * toward zero; NaN gives 0 (csrc/elementwise.cu). */
 int og_images_to_u8(const float* x, int N, int H, int W, unsigned char* out, cudaStream_t stream);
 
+/* og_snapshot_canvas: the pixels of one attention-map snapshot PNG (ref: miscc/utils.py:59-306, build_super_images /
+ * build_super_shape_images) for images i < nvis, without the caption glyphs: uint8 HWC `out` of
+ * (nvis * (strip + 2 vis)) x ((words + 2) (vis + 2)) pixels.  img (>= nvis, 3, img_side, img_side) and lr (the same
+ * with lr_side; NULL: img) are fp32 in [-1, 1]; maps (>= nvis, L, att, att) fp32; lens (>= nvis) int64 map counts
+ * per image (NULL: L each).  vis must be a multiple of att; upscale vis / att > 1 expands every map with skimage
+ * 0.14's pyramid_expand(sigma=20) in float64 (then vis must be a multiple of 4 and above 80).  per_map selects the
+ * shape snapshots' per-map min / max (guarded by max != min) instead of one pair per image starting at (1, 0).
+ * Workspaces: maxmap nvis att^2 floats; mm0 and stats nvis (L + 1) 2 doubles; with upscale > 1 also work
+ * nvis (L + 1) vis^2 and part nvis (L + 1) (vis / 4) 2 doubles (else NULL).  words <= 20 (the caption colours).
+ * Five launches with upscale > 1, three without (csrc/snapshot.cu). */
+int og_snapshot_canvas(const float* img, int img_side, const float* lr, int lr_side, const float* maps, int L,
+                       int att, const long long* lens, int nvis, int vis, int words, int strip, int per_map,
+                       float* maxmap, double* mm0, double* work, double* part, double* stats, unsigned char* out,
+                       cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -21,6 +21,7 @@ class AttrDict(dict):
 def default_cfg():
     c = AttrDict()
     c.GPU_IDS = "0"
+    c.DATA_DIR = ""        # the dataset root; the snapshot PNGs' caption font is read below it (snapshots.py)
     c.CUDA = True
     c.RNN_TYPE = "LSTM"    # the text encoder's recurrent cell; RNN_ENCODER implements the LSTM only
     c.TREE = AttrDict(BRANCH_NUM=3, BASE_SIZE=64)

@@ -16,8 +16,12 @@ batches; at the end the predictions are gathered to rank 0 once, the FID moments
 R-precision pools, so the pools hold different images than a single-process run's: the mean over pools estimates the
 same quantity, but is not the same number.  Only rank 0 prints and writes files.
 
-Not produced: the attention-map PNGs of SAVE_OPTIONS = 'SNAPSHOT' (``save_img_results`` / ``build_super_images``
-need skimage's ``pyramid_expand`` and the dataset's FreeMono font) and the ``save_shape_results`` PNGs.  The
+On display batches rank 0 writes the reference's snapshot PNGs to ``Snapshot/`` when a caption font is available
+(``font=``, or the reference's cfg.DATA_DIR + '/share/Pillow/Tests/fonts/FreeMono.ttf'): with SAVE_OPTIONS =
+'SNAPSHOT' the attention maps of each stage (``G_<it>_<i>.png``, ``bt_G_<it>_<i>.png``), and in modes 1 and 2 the
+generated shapes (``ShapeG_<it>.png``) and, in mode 1, the ground-truth heat maps (``ShapeD_<it>.png``), composed on
+the device (snapshots.py).  The reference's SNAPSHOT call cannot run (it passes parameters build_super_images does
+not have); this is what it evidently means: build_super_images per stage with the batch's images and font 50.  The
 TensorFlow Inception path (cfg.TEST.USE_TF = 1) is refused."""
 from __future__ import annotations
 
@@ -29,7 +33,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import losses, model, ops
+from . import losses, model, ops, snapshots
 from .config import cfg
 from .sampler import GSampler
 from .trainer import gather_inception_score, prepare_reference_test_batch
@@ -71,7 +75,8 @@ class condGANEvaluator:
     encoder's path with ``text_encoder`` -> ``image_encoder``), the shape generator cfg.TEST.NET_SHP_G when
     cfg.TEST.USE_GT_BOX_SEG > 0."""
 
-    def __init__(self, output_dir, data_loader, dataset, *, inception_weights, device=None, process_group=None):
+    def __init__(self, output_dir, data_loader, dataset, *, inception_weights, device=None, process_group=None,
+                 font=None):
         _refuse_unsupported()
         self.pg = process_group
         self.world = dist.get_world_size(process_group) if (dist.is_available() and dist.is_initialized()) else 1
@@ -98,6 +103,9 @@ class condGANEvaluator:
         self.mode = cfg.TEST.USE_GT_BOX_SEG
         self.sampler = None
         self._warned_snapshot = False
+        self.ixtoword = getattr(dataset, "ixtoword", None)
+        self.font = snapshots.load_font(font) if self.rank == 0 else None
+        self._writer = None
 
     def build_models(self) -> GSampler:
         """The sampler with every network of the evaluation (ref: evaluator.py:74-86, 88-146): G_NET from
@@ -174,24 +182,73 @@ class condGANEvaluator:
             if v is not None:
                 inp[k] = v
         text = {}
+        display = gen_iterations is not None and gen_iterations % self.display_interval == 0
+        snap = display and self.font is not None
+        shapes = {} if snap and self.mode > 0 else None
         with torch.no_grad():
-            fake_imgs = s.sample_eager(inp, text_out=text)[0]
+            kw = {} if shapes is None else {"shapes_out": shapes}
+            sampled = s.sample_eager(inp, text_out=text, **kw)
+            fake_imgs = sampled[0]
             region_features, cnn_code = s.encode_image(fake_imgs)
             rp.add(region_features, cnn_code, text["words_embs"], text["sent_emb"],
                    batch["cap_lens"].to(self.device, non_blocking=True), class_ids)
             pred, fake_acts = s.score_images(fake_imgs)
             is_.add(pred)
             fid.add(fake_acts, acts.to(self.device, non_blocking=True))
-        if gen_iterations is not None and gen_iterations % self.display_interval == 0:
+        if display:
             if cfg.TEST.SAVE_OPTIONS == "IMAGE":
                 self.save_singleimages(fake_imgs[-1], keys, sent_ids)
+            elif snap:
+                self.save_img_results(fake_imgs, sampled[2], sampled[3], batch["captions"], gen_iterations)
             elif not self._warned_snapshot:
                 warnings.warn("cfg.TEST.SAVE_OPTIONS = 'SNAPSHOT': the attention-map PNGs (save_img_results) are not "
                               "produced by this library")
                 self._warned_snapshot = True
+            if shapes:
+                self.save_shape_results(data, batch, shapes["raw_masks"], gen_iterations)
             if self.rank == 0:
                 print("%d / %d" % (gen_iterations, self.num_batches))
         return dict(fake_imgs=fake_imgs, class_ids=class_ids, keys=keys, sent_ids=sent_ids)
+
+    def _submit(self, jobs):
+        if self._writer is None:
+            self._writer = snapshots.PngWriter()
+        self._writer.submit(jobs)
+
+    def save_img_results(self, fake_imgs, att_maps, bt_att_maps, captions, gen_iterations):
+        """ref: evaluator.py:170-205, as it evidently means: per stage i, build_super_images of fake_imgs[i + 1]
+        (lr fake_imgs[i]) with the stage's word and box-word attention maps: ``Snapshot/G_<it>_<i>.png`` and
+        ``Snapshot/bt_G_<it>_<i>.png``."""
+        if self.rank != 0:
+            return
+        jobs = []
+        for i in range(len(att_maps)):
+            for prefix, maps in (("G", att_maps[i]), ("bt_G", bt_att_maps[i])):
+                c = snapshots.super_images(fake_imgs[i + 1], captions, self.ixtoword, maps, lr_images=fake_imgs[i],
+                                           font=self.font)
+                jobs.append((os.path.join(self.snapshot_dir, "%s_%d_%d.png" % (prefix, gen_iterations, i)), c))
+        self._submit(jobs)
+
+    def save_shape_results(self, data, batch, raw_masks, gen_iterations):
+        """ref: evaluator.py:207-229 and 316-324: ``Snapshot/ShapeG_<it>.png`` from the real 64-pixel images and the
+        shape generator's masks and, in mode 1, ``Snapshot/ShapeD_<it>.png`` from the ground-truth heat maps of the
+        64 scale, rebuilt on the device from the loader's masks.  The loader's images and masks are read on display
+        batches only, in the batch's caption-length order."""
+        if self.rank != 0:
+            return
+        order = torch.sort(torch.as_tensor(data[4]).to(torch.int64).view(-1), dim=0, descending=True,
+                           stable=True).indices
+        to_dev = lambda t: torch.as_tensor(t)[order].to(self.device, torch.float32)
+        imgs0 = to_dev(data[0][0])
+        jobs = [(os.path.join(self.snapshot_dir, "ShapeG_%d.png" % gen_iterations),
+                 snapshots.super_shape_images(imgs0, raw_masks))]
+        if self.mode == 1:
+            cls = batch["roi_cls"].to(self.device)
+            nr = batch["num_rois"].to(self.device)
+            hmaps = ops.form_hmaps(to_dev(data[12][0]).contiguous(), cls, nr, len(self.cats_index_dict), 0.0)
+            jobs.append((os.path.join(self.snapshot_dir, "ShapeD_%d.png" % gen_iterations),
+                         snapshots.super_shape_images(imgs0, hmaps)))
+        self._submit(jobs)
 
     def save_singleimages(self, images, keys, sent_ids):
         """ref: evaluator.py:231-239: one JPEG per image, the bytes made on the device (ops.images_to_u8)."""
@@ -245,15 +302,27 @@ class condGANEvaluator:
         is_ = losses.InceptionScore(num_splits)
         fid = losses.FrechetDistance(cfg.TEST.FID_DIMS)
         gen_iterations = 0
-        for data in self.data_loader:
-            self.evaluate_batch(data, rp, is_, fid, gen_iterations=gen_iterations)
-            gen_iterations += 1
-            if gen_iterations >= cfg.TEST.TEST_IMG_NUM:
-                break
+        try:
+            for data in self.data_loader:
+                self.evaluate_batch(data, rp, is_, fid, gen_iterations=gen_iterations)
+                gen_iterations += 1
+                if gen_iterations >= cfg.TEST.TEST_IMG_NUM:
+                    break
+        except BaseException:
+            self.close_writer(raise_error=False)
+            raise
         return self.finish(rp, is_, fid)
 
+    def close_writer(self, raise_error=True):
+        """Waits until every snapshot PNG of the batches so far is written (``finish`` calls it)."""
+        if self._writer is not None:
+            writer, self._writer = self._writer, None
+            writer.close(raise_error)
+
     def finish(self, rp, is_, fid):
-        """The scores over every rank (ref: evaluator.py:443-467), written and printed by rank 0."""
+        """The scores over every rank (ref: evaluator.py:443-467), written and printed by rank 0, after the snapshot
+        PNGs of ``evaluate_batch`` are written."""
+        self.close_writer()
         score = gather_inception_score(is_, self.world, self.rank, self.pg)
         moments = self._merged_fid(fid)
         accs = self._merged_rp(rp)

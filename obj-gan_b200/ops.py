@@ -2176,3 +2176,49 @@ def images_to_u8(x):
     out = torch.empty((n, h, w, 3), device=x.device, dtype=torch.uint8)
     _call("og_images_to_u8", _p(x), n, h, w, _p(out))
     return out
+
+
+def snapshot_canvas(images, maps, *, lr_images=None, lens=None, nvis, vis, words, strip, per_map):
+    """The pixels of one attention-map snapshot PNG on the device (og_snapshot_canvas; ref: miscc/utils.py:59-306):
+    (nvis (strip + 2 vis), (words + 2) (vis + 2), 3) uint8 with the caption strips' backgrounds but no glyphs.
+    ``images`` / ``lr_images`` (B, 3, s, s) fp32 in [-1, 1] (None: ``images``), resized to ``vis`` like nn.Upsample
+    bilinear; ``maps`` (B, L, att, att) fp32, expanded with pyramid_expand(sigma=20) when vis // att > 1; ``lens``
+    int64 (B,) map counts per image (None: L each).  ``per_map``: the shape snapshots' per-map normalisation instead
+    of one min / max per image."""
+    _chk(images, maps, lr_images, lens)
+    for name, t in (("lr_images", lr_images), ("lens", lens)):
+        if t is not None and t.device != maps.device:
+            raise ValueError(f"snapshot_canvas: {name} is on {t.device}, the maps on {maps.device}")
+    if lens is not None and (lens.dim() != 1 or lens.shape[0] < nvis):
+        raise ValueError(f"snapshot_canvas: lens must hold >= {nvis} counts, got {tuple(lens.shape)}")
+    images = images.detach().contiguous()
+    maps = maps.detach().contiguous()
+    lr = None if lr_images is None else lr_images.detach().contiguous()
+    for name, t in (("images", images), ("lr_images", lr)):
+        if t is not None and (t.dim() != 4 or t.shape[1] != 3 or t.shape[2] != t.shape[3] or t.dtype != torch.float32
+                              or t.shape[0] < nvis):
+            raise ValueError(f"snapshot_canvas: {name} must be (>= {nvis}, 3, s, s) float32, got {tuple(t.shape)} "
+                             f"{t.dtype}")
+    if maps.dim() != 4 or maps.shape[2] != maps.shape[3] or maps.dtype != torch.float32 or maps.shape[0] < nvis \
+            or maps.shape[1] < 1:
+        raise ValueError(f"snapshot_canvas: maps must be (>= {nvis}, L >= 1, att, att) float32, got "
+                         f"{tuple(maps.shape)} {maps.dtype}")
+    L, att = maps.shape[1], maps.shape[2]
+    up = vis // att
+    if vis % att or not 0 <= words <= 20 or (up > 1 and (vis % 4 or vis <= 80)):
+        raise ValueError(f"snapshot_canvas: vis {vis} with {att}-pixel maps and {words} words is not supported")
+    if lens is not None:
+        _chk(lens)
+        lens = lens.to(torch.int64).contiguous()
+    dev, m = maps.device, L + 1
+    f64 = dict(device=dev, dtype=torch.float64)
+    maxmap = torch.empty((nvis, att, att), device=dev, dtype=torch.float32)
+    mm0 = torch.empty((nvis, m, 2), **f64)
+    stats = torch.empty((nvis, m, 2), **f64)
+    work = torch.empty((nvis, m, vis, vis), **f64) if up > 1 else None
+    part = torch.empty((nvis, m, vis // 4, 2), **f64) if up > 1 else None
+    out = torch.empty((nvis * (strip + 2 * vis), (words + 2) * (vis + 2), 3), device=dev, dtype=torch.uint8)
+    _call("og_snapshot_canvas", _p(images), images.shape[2], _p(lr), 0 if lr is None else lr.shape[2], _p(maps), L,
+          att, _p(lens), nvis, vis, words, strip, 1 if per_map else 0, _p(maxmap), _p(mm0), _p(work), _p(part),
+          _p(stats), _p(out))
+    return out

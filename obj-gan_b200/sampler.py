@@ -402,14 +402,17 @@ class GSampler:
         hmaps, bt_masks, fm_bt_masks = ops.form_gen_hmaps(raw_masks, dev["roi_cls"], dev["num_rois"], IMG_SIZES, nbf)
         return dict(raw_masks=raw_masks, bbox_fmaps=fmaps, hmaps=hmaps, bt_masks=bt_masks, fm_bt_masks=fm_bt_masks)
 
-    def _forward(self, dev: dict, text_out: dict | None = None):
+    def _forward(self, dev: dict, text_out: dict | None = None, shapes_out: dict | None = None):
         if "captions" in dev:
             text = self._text(dev)
             if text_out is not None:
                 text_out.update(text)
             dev = dict(dev, **text)
         if "noise_shp" in dev:
-            d = dict(dev, **self._shapes(dev))
+            shapes = self._shapes(dev)
+            if shapes_out is not None:
+                shapes_out.update(shapes)
+            d = dict(dev, **shapes)
             d["slabels_feat"] = ops.form_clabels_feat(dev["clabels_emb"], dev["roi_cls"], dev["num_rois"],
                                                       int(dev["glb_max_num_roi"]))
             dev = d
@@ -421,11 +424,12 @@ class GSampler:
             g.ca_net.eps_override = None
 
     # ------------------------------------------------------------------ sampling
-    def sample_eager(self, inp: dict, text_out: dict | None = None):
+    def sample_eager(self, inp: dict, text_out: dict | None = None, shapes_out: dict | None = None):
         """The same forward pass without graphs.  ``text_out``: a dict that receives the text stage's outputs
-        (``words_embs``, ``sent_emb``, ``mask``, ``glove_words_embs``) of a caption batch, for R-precision."""
+        (``words_embs``, ``sent_emb``, ``mask``, ``glove_words_embs``) of a caption batch, for R-precision.
+        ``shapes_out``: a dict that receives ``sample_shapes``' outputs of a batch without masks."""
         with torch.no_grad():
-            return self._forward(self._prepare(inp, eager=True), text_out)
+            return self._forward(self._prepare(inp, eager=True), text_out, shapes_out)
 
     def sample_shapes(self, inp: dict) -> dict:
         """The generated shapes of a batch without masks (eager): ``raw_masks`` (B, R, 64, 64), the SHP_G_NET output the

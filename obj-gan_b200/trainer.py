@@ -15,12 +15,13 @@ from __future__ import annotations
 import contextlib
 import os
 import time
+import warnings
 
 import torch
 import torch.distributed as dist
 
 from . import lib as _lib
-from . import losses, model, ops
+from . import losses, model, ops, snapshots
 from .config import cfg
 
 ALIGN = 64  # floats; keeps every parameter view 256-byte aligned inside its bucket
@@ -700,10 +701,15 @@ class condGANTrainer:
     and the ranks exchange gradients through ``process_group``; the epoch's Inception score covers every rank's
     predictions, gathered to rank 0 once per epoch, and only rank 0 prints and writes files.
 
-    Not produced: the attention-map PNGs the reference saves every DISPLAY_INTERVAL steps (``save_img_results``);
-    ``Image/`` is created for the reference's directory layout and stays empty."""
+    Every DISPLAY_INTERVAL steps rank 0 writes the reference's attention-map PNGs to ``Image/`` (``save_img_results``)
+    from the EMA weights and the noise drawn once in ``setup()``: ``G_average_<epoch>_<i>.png`` and
+    ``bt_G_average_<epoch>_<i>.png`` per stage, ``D_average_<epoch>.png`` with the DAMSM word maps.  ``font``: the
+    caption font, a TrueType path or a PIL font (default: the reference's cfg.DATA_DIR +
+    '/share/Pillow/Tests/fonts/FreeMono.ttf' at size 50); without one no PNG is written and the first display step
+    warns.  ``dataset.ixtoword`` names the caption tokens."""
 
-    def __init__(self, output_dir, data_loader, dataset, *, inception_weights, device=None, process_group=None):
+    def __init__(self, output_dir, data_loader, dataset, *, inception_weights, device=None, process_group=None,
+                 font=None):
         self.pg = process_group
         self.world = dist.get_world_size(process_group) if (dist.is_available() and dist.is_initialized()) else 1
         self.rank = dist.get_rank(process_group) if self.world > 1 else 0
@@ -728,6 +734,11 @@ class condGANTrainer:
         self.num_batches = len(data_loader)
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         self.inception_weights = inception_weights
+        self.ixtoword = getattr(dataset, "ixtoword", None)
+        self.font = snapshots.load_font(font)
+        self.fixed_noise = None
+        self._display = None
+        self._warned_font = False
 
     def build_models(self):
         """(text_encoder, image_encoder, StepBTrainer, INCEPTION_V3, start_epoch), like the reference's build_models
@@ -761,6 +772,11 @@ class condGANTrainer:
         glove = getattr(self.glove_emb, "weight", self.glove_emb)
         self.glove = glove.detach().to(self.device).float().contiguous()
         self.clabels_emb = self.prepare_cat_emb()
+        # ref: trainer.py:336-337: drawn from the host generator, as there, but only when the PNGs can be written, so
+        # that without a font the host random stream (the loader's shuffles) is the one it always was.  Every rank
+        # loads the font and draws, so the ranks' streams stay alike; only rank 0 renders.
+        if self.font is not None:
+            self.fixed_noise = torch.randn(self.batch_size, cfg.GAN.Z_DIM).to(self.device)
         return start
 
     def train_step(self, data, score=None, z=None, eps=None) -> dict:
@@ -779,6 +795,8 @@ class condGANTrainer:
         if eps is not None:
             dev["eps"] = eps
         out = self.net.step(dev, class_ids)
+        if self.fixed_noise is not None and self.rank == 0:
+            self._display = (dev, batch["captions"])      # the inputs of a display right after this step
         pred = self.inception(out["fake_imgs"][-1])
         if score is not None:
             score.add(pred)
@@ -822,9 +840,59 @@ class condGANTrainer:
         print("inception_score: mean, std, mean_conf, std_conf")
         print("inception_score: %f, %f, %f, %f" % (mean, std, mean_conf, std_conf))
 
+    def save_img_results(self, epoch, writer):
+        """ref: trainer.py:275-329 and 478-484: the generator forward with the EMA weights and ``fixed_noise`` on the
+        last step's inputs, in train mode (BatchNorm uses the batch statistics and updates its running buffers, which
+        keep that update), the image encoder and the DAMSM word maps of the last stage; the weights are restored
+        afterwards.  The PNGs go to ``writer``."""
+        if self.font is None:
+            if not self._warned_font:
+                warnings.warn("no caption font (cfg.DATA_DIR + '%s' or font=): the attention-map PNGs are not "
+                              "written" % snapshots.FONT_PATH)
+                self._warned_font = True
+            return
+        dev, captions = self._display
+        b = dev["num_rois"].shape[0]
+        bucket = self.net.bG
+        live = bucket.flat.clone()
+        self._load_g(bucket.avg)
+        try:
+            with torch.no_grad():
+                inp = {k: v for k, v in dev.items() if k != "eps"}
+                inp["z"] = self.fixed_noise[:b]
+                fake_imgs, _, att_maps, bt_att_maps, _, _ = self.net.generate(inp)
+                region, _ = self.image_encoder(fake_imgs[-1])
+                _, attn = ops.words_pairs(region, dev["words_embs"], dev["cap_lens"], cfg.TRAIN.SMOOTH.GAMMA1,
+                                          cfg.TRAIN.SMOOTH.GAMMA2)
+                idx = torch.arange(b, device=attn.device)
+                word_maps = attn[idx, idx]                                # (B, T, 17, 17): caption i's own maps
+        finally:
+            self._load_g(live)
+        jobs = []
+        for i in range(len(att_maps)):
+            for prefix, maps in (("G", att_maps[i]), ("bt_G", bt_att_maps[i])):
+                c = snapshots.super_images(fake_imgs[i + 1], captions, self.ixtoword, maps, lr_images=fake_imgs[i],
+                                           font=self.font)
+                jobs.append((os.path.join(self.image_dir, "%s_average_%d_%d.png" % (prefix, epoch, i)), c))
+        c = snapshots.super_images(fake_imgs[-1], captions, self.ixtoword, word_maps, lens=dev["cap_lens"],
+                                   font=self.font)
+        jobs.append((os.path.join(self.image_dir, "D_average_%d.png" % epoch), c))
+        writer.submit(jobs)
+
+    def _load_g(self, weights):
+        """Copies ``weights`` into the generator's flat parameters and re-packs their tensor-core operand copies."""
+        bucket = self.net.bG
+        bucket.flat.copy_(weights)
+        bucket.epoch[0] += 1
+        bucket.plan.run()
+
     def train(self):
         """ref: trainer.py:331-511."""
         start_epoch = self.setup()
+        with snapshots.writing(snapshots.PngWriter() if self.rank == 0 else None) as writer:
+            self._train(start_epoch, writer)
+
+    def _train(self, start_epoch, writer):
         gen_iterations = 0
         lead = self.rank == 0
         for epoch in range(start_epoch, self.max_epoch):
@@ -837,6 +905,8 @@ class condGANTrainer:
                 gen_iterations += 1
                 if gen_iterations % self.print_interval == 0 and lead:
                     self._log(epoch, gen_iterations, self.host_losses(out))
+                if gen_iterations % self.display_interval == 0 and lead:
+                    self.save_img_results(epoch, writer)
             if out is None:
                 continue
             h = self.host_losses(out)
