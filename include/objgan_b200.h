@@ -92,12 +92,13 @@ int og_unpack_wgrad(const float* dw_packed, int Co, int Ci, int KH, int KW, int 
 
 /* upBlock (nearest 2x upsample + conv3x3, ref: model.py:43-49) as four 2x2 phase convolutions with pre-summed
  * weights: Wp[16][..] (tap t = ((p*2+q)*2+a)*2+b) from the OIHW parameter as fp16 hi/lo operands (scale word
- * *amax_up = 4 * *amax, the bound of the pre-sums), and the adjoint map for the gradient. */
+ * *amax_up = 4 * *amax, the bound of the pre-sums), and the adjoint map for the gradient (accumulate = 1 adds it to
+ * grad_oihw, a persistent gradient buffer, like og_unpack_wgrad). */
 int og_pack_upsample_weights(const float* w_oihw, int Co, int Ci, int Cip, int Kp, int split, int splitp,
                              int transposed, const unsigned* amax, unsigned* amax_up, void* hi, void* lo,
                              cudaStream_t stream);
 int og_unpack_upsample_wgrad(const float* dwp, int Co, int Ci, int Cip, int Kp, int split, int splitp,
-                             float* grad_oihw, cudaStream_t stream);
+                             float* grad_oihw, int accumulate, cudaStream_t stream);
 
 /* Tensor-core path (wgmma f16 with fp32 register accumulators, TMA operand staging) for the
  * contractions that dominate the step (HmapResBlock / upBlock / jointConv / discriminator convs: forward, input

@@ -800,7 +800,7 @@ __global__ void pack_upsample_weights_kernel(const float* __restrict__ w, int Co
 }
 // dW[kh][kw] = sum_{p,q} dWp[p][q][up_row(p,kh)][up_row(q,kw)]   (dWp packed [16][Kp][Cip], i.e. "transposed" layout)
 __global__ void unpack_upsample_wgrad_kernel(const float* __restrict__ dwp, int Co, int Ci, int Cip, int Kp, int split,
-                                             int splitp, float* __restrict__ grad) {
+                                             int splitp, float* __restrict__ grad, int accumulate) {
   long long total = (long long)Co * Ci * 9;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
@@ -817,7 +817,7 @@ __global__ void unpack_upsample_wgrad_kernel(const float* __restrict__ dwp, int 
         int t = ((p * 2 + q) * 2 + up_row(p, kh)) * 2 + up_row(q, kw);
         v += dwp[((long long)t * Kp + cm) * Cip + ci];
       }
-    grad[i] = v;
+    grad[i] = accumulate ? grad[i] + v : v;
   }
 }
 OG_API int og_pack_upsample_weights(const float* w_oihw, int Co, int Ci, int Cip, int Kp, int split, int splitp,
@@ -835,11 +835,11 @@ OG_API int og_pack_upsample_weights(const float* w_oihw, int Co, int Ci, int Cip
   OG_RETURN_LAST_ERROR();
 }
 OG_API int og_unpack_upsample_wgrad(const float* dwp, int Co, int Ci, int Cip, int Kp, int split, int splitp,
-                                    float* grad_oihw, cudaStream_t stream) {
+                                    float* grad_oihw, int accumulate, cudaStream_t stream) {
   long long total = (long long)Co * Ci * 9;
   int blocks = (int)((total + 255) / 256);
   if (blocks > og_num_sms() * 16) blocks = og_num_sms() * 16;
-  unpack_upsample_wgrad_kernel<<<blocks, 256, 0, stream>>>(dwp, Co, Ci, Cip, Kp, split, splitp, grad_oihw);
+  unpack_upsample_wgrad_kernel<<<blocks, 256, 0, stream>>>(dwp, Co, Ci, Cip, Kp, split, splitp, grad_oihw, accumulate);
   OG_RETURN_LAST_ERROR();
 }
 

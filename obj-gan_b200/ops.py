@@ -420,8 +420,11 @@ def _tc_wgrad(kind, xs, gs, n, h, w, oh, ow, weight, c, kp, split, splitp, mode,
     _call("og_conv2d_wgrad_tc", _p(gh), _p(gl), _p(ag), n, gh.shape[0], oh, ow, kp, _p(xh), _p(xl), _p(ax),
           xh.shape[0], xh.shape[1], xh.shape[2], c, _p(dwp), nt, ctypes.addressof(arr), len(ent))
     if mode == UPSAMPLE2X and kind == "s1":
+        if sink is not None:
+            _call("og_unpack_upsample_wgrad", _p(dwp), co, ci, c, kp, split, splitp, _p(sink), 1)
+            return None
         gw = torch.empty_like(weight)
-        _call("og_unpack_upsample_wgrad", _p(dwp), co, ci, c, kp, split, splitp, _p(gw))
+        _call("og_unpack_upsample_wgrad", _p(dwp), co, ci, c, kp, split, splitp, _p(gw), 0)
         return gw
     if sink is not None:
         _call("og_unpack_wgrad", _p(dwp), co, ci, kh_, kw_, c, kp, split, splitp, _p(sink), 1, 1)
