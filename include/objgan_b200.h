@@ -236,23 +236,14 @@ int og_adam_ema(float* p, const float* g, float* m, float* v, float* avg, long l
 int og_inc_i64(long long* counter, cudaStream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------
- * DAMSM matching losses around func_attention (ref: miscc/losses.py:13-159: cosine_similarity, sent_loss,
- * words_loss).  Dense row-major fp32; B <= 128 captions (og_ce_pair: the R-precision pool of 100).
- *  og_cosine_cl_*     : out[b][l] = cos(word[:, l], wei[b, :, l]) over the D features (word [D][L] shared by all
- *                       images, wei [B][D][L]); backward w.r.t. wei (losses.py:101-108)
- *  og_expsumlog_*     : out[b] = log(sum_l exp(gamma * s[b][l]))            (Eq. 10, losses.py:112-115)
+ * DAMSM matching losses (ref: miscc/losses.py:22-71, 131-147: sent_loss and the cross-entropies of words_loss; the
+ * word-level similarities are og_words_pairs_*).  Dense row-major fp32; B <= 128 captions (og_ce_pair: the R-precision pool of 100).
  *  og_cosine_matrix_* : out[i][j] = <a_i, b_j> / max(|a_i||b_j|, eps); backward w.r.t. a   (losses.py:43-50)
  *  og_ce_pair         : scores = gamma3 * sim with masked entries at -inf; loss0 = CrossEntropy(scores, labels),
  *                       loss1 = CrossEntropy(scores^T, labels) (means), their gradients G0 / G1 w.r.t. sim, and the
  *                       number of top-1 hits of both directions (losses.py:50-68, 131-147)
  *  og_ce_pair_bwd     : gsim = *g0 * G0 + *g1 * G1 (device scalars; NULL = 0)
  * ---------------------------------------------------------------------------------------------------- */
-int og_cosine_cl_fwd(const float* word, const float* wei, int B, int D, int L, float eps, float* out,
-                     cudaStream_t stream);
-int og_cosine_cl_bwd(const float* word, const float* wei, const float* g, int B, int D, int L, float eps, float* gwei,
-                     cudaStream_t stream);
-int og_expsumlog_fwd(const float* s, int B, int L, float gamma, float* out, cudaStream_t stream);
-int og_expsumlog_bwd(const float* s, const float* g, int B, int L, float gamma, float* gs, cudaStream_t stream);
 int og_cosine_matrix_fwd(const float* a, const float* b, int Ba, int Bb, int D, float eps, float* out,
                          cudaStream_t stream);
 int og_cosine_matrix_bwd(const float* a, const float* b, const float* g, int Ba, int Bb, int D, float eps, float* ga,

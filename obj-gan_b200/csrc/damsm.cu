@@ -1,75 +1,12 @@
-// DAMSM matching losses around func_attention (ref: miscc/losses.py:13-159): the small reductions that sit between
-// the attention kernel (attention.cu) and the two cross-entropy terms.  Problem sizes are tiny (B <= 64 captions,
-// nef = 256, <= 32 words), so these are one-thread-per-output kernels; what matters is that no arithmetic is left to
-// host loops or library calls and that the backward formulas match autograd on the reference's expressions.
+// DAMSM matching losses (ref: miscc/losses.py:22-71, 131-147): the sentence cosine matrix and the two cross-entropy
+// terms over a B x B similarity matrix (the word-level similarities come from words_pairs.cu).  Problem sizes are
+// tiny (B <= 128 captions, nef = 256), so these are one-thread-per-output kernels; what matters is that no arithmetic
+// is left to host loops or library calls and that the backward formulas match autograd on the reference's expressions.
 #include "common.cuh"
 
 namespace {
 // largest B of og_ce_pair (one thread per row / column): the evaluator's R-precision pool is 100 (RP_POOL_SIZE)
 constexpr int DM_MAXB = 128;
-
-// ---- cosine_similarity(word, weiContext) over the feature axis (losses.py:13-19, 101-108) ----------------------
-// word [D][L] (one caption, shared by all images), wei [B][D][L]  ->  out[b][l]
-__global__ void cosine_cl_fwd_kernel(const float* __restrict__ word, const float* __restrict__ wei, int B, int D, int L,
-                                     float eps, float* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= B * L) return;
-  const int b = i / L, l = i - b * L;
-  float w12 = 0.f, w1 = 0.f, w2 = 0.f;
-  for (int c = 0; c < D; ++c) {
-    const float x = word[c * L + l], y = wei[((long long)b * D + c) * L + l];
-    w12 = fmaf(x, y, w12);
-    w1 = fmaf(x, x, w1);
-    w2 = fmaf(y, y, w2);
-  }
-  out[i] = w12 / fmaxf(sqrtf(w1) * sqrtf(w2), eps);
-}
-// gradient w.r.t. wei only (the caption embedding is a constant of the generator update)
-__global__ void cosine_cl_bwd_kernel(const float* __restrict__ word, const float* __restrict__ wei,
-                                     const float* __restrict__ g, int B, int D, int L, float eps,
-                                     float* __restrict__ gwei) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= B * L) return;
-  const int b = i / L, l = i - b * L;
-  float w12 = 0.f, w1 = 0.f, w2 = 0.f;
-  for (int c = 0; c < D; ++c) {
-    const float x = word[c * L + l], y = wei[((long long)b * D + c) * L + l];
-    w12 = fmaf(x, y, w12);
-    w1 = fmaf(x, x, w1);
-    w2 = fmaf(y, y, w2);
-  }
-  const float n1 = sqrtf(w1), n2 = sqrtf(w2), prod = n1 * n2;
-  const float go = g[i];
-  if (prod >= eps) {
-    // cos = w12 / (n1 n2):  d/dy_c = x_c / (n1 n2) - cos * y_c / n2^2
-    const float inv = 1.f / prod, k = w12 * inv / w2;
-    for (int c = 0; c < D; ++c) {
-      const long long o = ((long long)b * D + c) * L + l;
-      gwei[o] = go * (word[c * L + l] * inv - k * wei[o]);
-    }
-  } else {
-    const float inv = 1.f / eps;     // clamped denominator: cos = w12 / eps
-    for (int c = 0; c < D; ++c) gwei[((long long)b * D + c) * L + l] = go * word[c * L + l] * inv;
-  }
-}
-
-// ---- Eq. (10): out[b] = log(sum_l exp(gamma * s[b][l]))  (losses.py:112-115; no max shift, like the reference) ----
-__global__ void expsumlog_fwd_kernel(const float* __restrict__ s, int B, int L, float gamma, float* __restrict__ out) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
-  float acc = 0.f;
-  for (int l = 0; l < L; ++l) acc += expf(gamma * s[b * L + l]);
-  out[b] = logf(acc);
-}
-__global__ void expsumlog_bwd_kernel(const float* __restrict__ s, const float* __restrict__ g, int B, int L, float gamma,
-                                     float* __restrict__ gs) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
-  float acc = 0.f;
-  for (int l = 0; l < L; ++l) acc += expf(gamma * s[b * L + l]);
-  const float k = g[b] * gamma / acc;
-  for (int l = 0; l < L; ++l) gs[b * L + l] = k * expf(gamma * s[b * L + l]);
-}
 
 // ---- sent_loss scores (losses.py:43-50): out[i][j] = <a_i, b_j> / max(|a_i| |b_j|, eps) -----------------------------
 __global__ void cosine_matrix_fwd_kernel(const float* __restrict__ a, const float* __restrict__ b, int Ba, int Bb, int D,
@@ -182,28 +119,6 @@ __global__ void ce_pair_bwd_kernel(const float* __restrict__ G0, const float* __
 }
 }  // namespace
 
-OG_API int og_cosine_cl_fwd(const float* word, const float* wei, int B, int D, int L, float eps, float* out,
-                            cudaStream_t stream) {
-  if (B * L == 0) return 0;
-  cosine_cl_fwd_kernel<<<og_cdiv(B * L, 128), 128, 0, stream>>>(word, wei, B, D, L, eps, out);
-  OG_RETURN_LAST_ERROR();
-}
-OG_API int og_cosine_cl_bwd(const float* word, const float* wei, const float* g, int B, int D, int L, float eps,
-                            float* gwei, cudaStream_t stream) {
-  if (B * L == 0) return 0;
-  cosine_cl_bwd_kernel<<<og_cdiv(B * L, 128), 128, 0, stream>>>(word, wei, g, B, D, L, eps, gwei);
-  OG_RETURN_LAST_ERROR();
-}
-OG_API int og_expsumlog_fwd(const float* s, int B, int L, float gamma, float* out, cudaStream_t stream) {
-  if (B == 0) return 0;
-  expsumlog_fwd_kernel<<<og_cdiv(B, 64), 64, 0, stream>>>(s, B, L, gamma, out);
-  OG_RETURN_LAST_ERROR();
-}
-OG_API int og_expsumlog_bwd(const float* s, const float* g, int B, int L, float gamma, float* gs, cudaStream_t stream) {
-  if (B == 0) return 0;
-  expsumlog_bwd_kernel<<<og_cdiv(B, 64), 64, 0, stream>>>(s, g, B, L, gamma, gs);
-  OG_RETURN_LAST_ERROR();
-}
 OG_API int og_cosine_matrix_fwd(const float* a, const float* b, int Ba, int Bb, int D, float eps, float* out,
                                 cudaStream_t stream) {
   if (Ba * Bb == 0) return 0;

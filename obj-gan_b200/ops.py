@@ -1207,62 +1207,6 @@ def func_attention(query, context, gamma1):
     return _FuncAttention.apply(query, context, gamma1)
 
 
-class _CosineCL(torch.autograd.Function):
-    """out[b, l] = cosine_similarity(word[:, l], wei[b, :, l]) (ref: miscc/losses.py:13-19 as used at 101-108).
-    ``word`` (D, L) is one caption's embedding shared by all images and is treated as a constant."""
-
-    @staticmethod
-    def forward(ctx, word, wei, eps):
-        _chk(word, wei)
-        word, wei = word.detach().contiguous(), wei.contiguous()
-        b, d, l = wei.shape
-        assert word.shape == (d, l)
-        out = torch.empty((b, l), device=wei.device, dtype=torch.float32)
-        _call("og_cosine_cl_fwd", _p(word), _p(wei), b, d, l, float(eps), _p(out))
-        ctx.eps = float(eps)
-        ctx.save_for_backward(word, wei)
-        return out
-
-    @staticmethod
-    def backward(ctx, g):
-        word, wei = ctx.saved_tensors
-        b, d, l = wei.shape
-        gwei = torch.empty_like(wei)
-        _call("og_cosine_cl_bwd", _p(word), _p(wei), _p(g.contiguous()), b, d, l, ctx.eps, _p(gwei))
-        return None, gwei, None
-
-
-def cosine_cl(word, wei, eps=1e-8):
-    return _CosineCL.apply(word, wei, eps)
-
-
-class _ExpSumLog(torch.autograd.Function):
-    """out[b] = log(sum_l exp(gamma * s[b, l]))  (ref: miscc/losses.py:112-115)."""
-
-    @staticmethod
-    def forward(ctx, s, gamma):
-        _chk(s)
-        s = s.contiguous()
-        b, l = s.shape
-        out = torch.empty((b,), device=s.device, dtype=torch.float32)
-        _call("og_expsumlog_fwd", _p(s), b, l, float(gamma), _p(out))
-        ctx.gamma = float(gamma)
-        ctx.save_for_backward(s)
-        return out
-
-    @staticmethod
-    def backward(ctx, g):
-        (s,) = ctx.saved_tensors
-        b, l = s.shape
-        gs = torch.empty_like(s)
-        _call("og_expsumlog_bwd", _p(s), _p(g.contiguous()), b, l, ctx.gamma, _p(gs))
-        return gs, None
-
-
-def expsumlog(s, gamma):
-    return _ExpSumLog.apply(s, gamma)
-
-
 def h2d(data, device, dtype=None):
     """Small host table (list / numpy array / CPU tensor) -> device WITHOUT stalling the host: staged in pinned memory
     and copied asynchronously on the current stream (a pageable ``.to(device)`` blocks the calling thread until the GPU
