@@ -149,28 +149,27 @@ def bench_layer(spec, window_ms, dirs=("fprop", "dgrad", "wgrad")):
     c = ops.cpad(cin)
     splitp = ops.cpad(split) if split else 0
     kp = 2 * splitp if split else ops.cpad(cout)
-    kind = ops._tc_kind(n, h, w, c, k, k, stride, 1, mode)
-    assert kind, f"{name}: not a tensor-core shape"
+    path = ops.conv_path(n, h, w, k, k, stride, 1, 1, mode, kp, "f16x3")
+    assert path in ("s1", "s2"), f"{name}: not a tensor-core shape"
     oh, ow = ops._out_hw(h, w, k, k, stride, 1, mode)
-    pad, s2d = (1 if mode == PAD_REFLECT else 0), kind == "s2"
+    geo = ops._conv2d_geo(n, h, w, k, k, stride, 1, mode)
+    plan = ops._tc_plan(ops.FPROP, *geo)
     per_set = 2 * 2 * (n * h * w * c + n * oh * ow * kp)          # hi + lo copies of x and of g
     nsets = max(1, math.ceil(2 * L2_BYTES / per_set))
     sets = []
     for _ in range(nsets):
         x = torch.randn(n, h, w, c, device="cuda")
         x[..., cin:] = 0
-        xs = ops._split_x(kind, x, mode)
-        x.og_split = (*xs, pad, s2d, x._version)  # fprop reuses these copies: no split pass timed
+        xs = ops._split(x, *plan.xsplit)
+        x.og_split = (*xs, *plan.xsplit, x._version)  # fprop reuses these copies: no split pass timed
         g = torch.randn(n, oh, ow, kp, device="cuda")
-        gs = ops._split_g(kind, g, mode)
+        gs = ops._split(g, *plan.gsplit)
         sets.append((x, xs, gs))
     wt, cache = m.weight, m._cache
     calls = {
-        "fprop": lambda i: ops._tc_fprop(kind, sets[i % nsets][0], cache, wt, kp, split, splitp, mode, None, ACT_NONE),
-        "dgrad": lambda i: ops._tc_dgrad(kind, sets[i % nsets][2], n, cache, wt, c, kp, split, splitp, mode, h, w, oh,
-                                         ow),
-        "wgrad": lambda i: ops._tc_wgrad(kind, sets[i % nsets][1], sets[i % nsets][2], n, h, w, oh, ow, wt, c, kp,
-                                         split, splitp, mode),
+        "fprop": lambda i: ops._tc_fprop(sets[i % nsets][0], cache, wt, kp, split, splitp, geo, None, ACT_NONE),
+        "dgrad": lambda i: ops._tc_dgrad(sets[i % nsets][2], cache, wt, c, kp, split, splitp, geo),
+        "wgrad": lambda i: ops._tc_wgrad(sets[i % nsets][1], sets[i % nsets][2], wt, c, kp, split, splitp, geo),
     }
     alg, iss = layer_work(cin, cout, k, stride, mode_s, split, n, h, w)
     out = {}

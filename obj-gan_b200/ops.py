@@ -192,7 +192,10 @@ class PackPlan:
 # Contraction engine for the convolutions: "f16x3" = wgmma tensor cores with the error-compensated
 # three-product fp16 hi/lo split (22-bit operands, fp32-level accuracy: the default), "simt" = exact fp32 FMA on the
 # CUDA cores.
+import ctypes
+import functools
 import os as _os
+from collections import namedtuple
 CONV_ENGINE = _os.environ.get("OBJGAN_CONV", "f16x3")
 if CONV_ENGINE not in ("f16x3", "simt"):
     raise ValueError("OBJGAN_CONV=%r: the convolution engine is 'f16x3' or 'simt'" % CONV_ENGINE)
@@ -200,7 +203,6 @@ TC_MIN_PIXELS = 256        # smaller problems go to the exact-fp32 SIMT kernels 
 
 
 def _int_array(rows):
-    import ctypes
     flat = [int(v) for r in rows for v in r]
     return (ctypes.c_int * len(flat))(*flat)
 
@@ -216,7 +218,8 @@ def _empty_slack(shape, device):
 
 def _split(x, pad=0, s2d=False):
     """(fp16 hi, fp16 lo, scale word) of an NHWC tensor scaled by a power of two from its max|x|; pad=1 adds the
-    reflection halo; s2d gives [4N, H/2, W/2, C]."""
+    reflection halo; s2d gives the four space-to-depth phase blocks [4N, ceil(H/2), ceil(W/2), C] (_split_s2d_odd at
+    an odd size)."""
     n, h, w, c = x.shape
     ready_made = getattr(x, "og_split", None)          # the producer already wrote them (og_norm_apply_split)
     if ready_made is not None and ready_made[3:] == (pad, bool(s2d), x._version):
@@ -224,6 +227,8 @@ def _split(x, pad=0, s2d=False):
     if getattr(x, "og_f32_invalid", False):
         raise RuntimeError("this activation exists only as tensor-core operand copies (pad=%s); a consumer asked for "
                            "another layout" % (ready_made[3] if ready_made else None))
+    if s2d and (h % 2 or w % 2):
+        return _split_s2d_odd(x)
     shape = (4 * n, h // 2, w // 2, c) if s2d else (n, h + 2 * pad, w + 2 * pad, c)
     xh = _empty_slack(shape, x.device)
     xl = _empty_slack(shape, x.device)
@@ -232,6 +237,18 @@ def _split(x, pad=0, s2d=False):
     if not ready:
         amax = torch.empty(1, device=x.device, dtype=torch.int32)
     _call("og_prep_split", _p(x), n, h, w, c, pad, 1 if s2d else 0, _p(amax), 1 if ready else 0, _p(xh), _p(xl))
+    return xh, xl, amax
+
+
+def _split_s2d_odd(x):
+    """_split(x, s2d=True) at an odd H or W: og_prep_split_s2d zero-fills the phase blocks past the odd edge (at even
+    sizes it writes what og_prep_split(s2d=1) does)."""
+    n, h, w, c = x.shape
+    shape = (4 * n, (h + 1) // 2, (w + 1) // 2, c)
+    xh = _empty_slack(shape, x.device)
+    xl = _empty_slack(shape, x.device)
+    amax = torch.empty(1, device=x.device, dtype=torch.int32)
+    _call("og_prep_split_s2d", _p(x), n, h, w, c, _p(amax), 0, _p(xh), _p(xl))
     return xh, xl, amax
 
 
@@ -250,137 +267,126 @@ def _known_amax(t):
     return None
 
 
-def _tc_launch(xs, n, ws, ntaps_w, kw_rows, y, oh, ow, k, osy, op, taps, bias=None, act=ACT_NONE, yoff=0,
-               slope=LRELU_SLOPE):
-    """xs / ws: (hi, lo, scale word) operand triples; taps: (dh, dw, dn, widx) quadruples; the source is
-    [SN, SH, SW, C] with SN = n or 4n (space-to-depth).  The k output channels start at channel yoff of y."""
+def _out_hw(h, w, kh, kw, stride, pad, mode, padw=None):
+    if mode == UPSAMPLE2X:
+        return 2 * h, 2 * w
+    padw = pad if padw is None else padw
+    return (h + 2 * pad - kh) // stride + 1, (w + 2 * padw - kw) // stride + 1
+
+
+def conv_path(n, h, w, kh, kw, stride, padh, padw, mode, kp, engine, general=False):
+    """The path a convolution of an (n, h, w) source with kp (padded) output channels takes under ``engine``: "s1" /
+    "s2" (tensor cores; "s2" on the space-to-depth phases of a stride-2 layer), "narrow" (og_conv2d_narrow_*: 8 padded
+    output channels, zero padding, small maps) or "simt" (og_conv2d_simt / og_conv2d_wgrad_simt).
+
+    general: the layer has the tensor-core form at every zero-padded shape of stride 1 or 2 and no narrow form (the
+    Inception trunks).  Otherwise the tensor cores take the 3x3 pad-1 layers of any mode, the 4x4 stride-1 zero-padded
+    roi_code layer, and the 3x3 / 4x4 stride-2 pad-1 zero-padded layers on even maps.  Either way they need
+    TC_MIN_PIXELS output pixels; the batch need not fill the last pixel tile (rows past it are never stored)."""
+    oh, ow = _out_hw(h, w, kh, kw, stride, padh, mode, padw)
+    if engine == "f16x3" and n * oh * ow >= TC_MIN_PIXELS:
+        if general:
+            return "s%d" % stride
+        if kh == kw and padh == padw == 1:
+            if stride == 1 and (kh == 3 or (kh == 4 and mode == PAD_ZERO)):
+                return "s1"
+            if stride == 2 and kh in (3, 4) and mode == PAD_ZERO and h % 2 == 0 and w % 2 == 0:
+                return "s2"
+    if not general and kp == 8 and mode == PAD_ZERO and n * oh * ow <= 65536:
+        return "narrow"
+    return "simt"
+
+
+def _tc_kind(n, h, w, c, kh, kw, stride, pad, mode):
+    """The tensor-core form ("s1" / "s2") conv2d takes for this layer under CONV_ENGINE (conv_path), or None.  c, the
+    input channels, decides nothing: only the narrow form looks at channels, and it is not a tensor-core form."""
+    path = conv_path(n, h, w, kh, kw, stride, pad, pad, mode, 0, CONV_ENGINE)
+    return path if path in ("s1", "s2") else None
+
+
+FPROP, DGRAD, WGRAD = "fprop", "dgrad", "wgrad"
+_UP_OFF = ((-1, 0), (0, 1))   # low-res row/col offsets read by output phase 0 / 1 of upsample + conv3x3
+_Plan = namedtuple("_Plan", "xsplit gsplit up ntaps out launches")
+
+
+@functools.lru_cache(maxsize=None)
+def _tc_plan(d, n, h, w, kh, kw, stride, padh, padw, mode, cols=False):
+    """The tensor-core launches of one direction (FPROP, DGRAD or WGRAD) of a convolution over an (n, h, w) source.
+    Tap order is summation order: these lists fix the bits of the results.
+
+      xsplit, gsplit  the (pad, s2d) layouts _split makes of x and of the output gradient g
+      up              the weights are an upsample layer's pre-summed phase weights (get_up_hilo)
+      ntaps           taps of the packed weights and of the packed weight gradient
+      out             (rows, cols) of the buffer FPROP / DGRAD writes: y, or the input gradient (with the halo of a
+                      reflection-padded layer); for WGRAD the grid of g's copies
+      launches        FPROP / DGRAD: per og_conv2d_tc launch (taps, oh, ow, osy, opy, opx), taps (dh, dw, dn, widx);
+                      WGRAD: one (entries, oh, ow, 1, 0, 0), entries (gdn, dh, dw, xdn, output tap)
+
+    cols: the forward taps of a stride-1 layer without upsampling run column by column, and the input gradient's
+    column by column with the kernel rows descending (conv2d's 3x3 layers); otherwise every list runs row by row."""
+    oh, ow = _out_hw(h, w, kh, kw, stride, padh, mode, padw)
+    halo = padh if mode == PAD_REFLECT else 0             # reflect: x's copies carry the halo; zero pad: TMA fills
+    if mode == UPSAMPLE2X:      # 3x3 pad 1 on the 2x map: output phases p = (py, px) of 2x2 taps at low resolution
+        xsplit, gsplit, up, ntaps = (0, False), (0, True), True, 16
+        phases = [[(_UP_OFF[p // 2][a], _UP_OFF[p % 2][b], 0, (p * 2 + a) * 2 + b) for a in range(2) for b in range(2)]
+                  for p in range(4)]
+    else:
+        xsplit, gsplit, up, ntaps = (halo, stride == 2), (0, False), False, kh * kw
+        rows = [(i, j) for i in range(kh) for j in range(kw)]
+        if stride == 2:         # x as its four space-to-depth phases: tap (i, j) reads phase (a, b) at offset (dh, dw)
+            phases = [[(dh, dw, (a * 2 + b) * n, i * kw + j) for i, j in rows
+                       for (dh, a), (dw, b) in [(divmod(i - padh, 2), divmod(j - padw, 2))]]]
+        else:
+            phases = [[(i - padh + halo, j - padw + halo, 0, i * kw + j) for i, j in rows]]
+    cols = cols and stride == 1 and not up
+    if d == FPROP:
+        out = (oh, ow)
+        if up:
+            launches = [(taps, h, w, 2, p // 2, p % 2) for p, taps in enumerate(phases)]
+        else:
+            taps = phases[0]
+            if cols:
+                taps = [taps[i * kw + j] for j in range(kw) for i in range(kh)]
+            launches = [(taps, oh, ow, 1, 0, 0)]
+    elif d == DGRAD and stride == 2:    # input pixel (2y + a, 2x + b) <- the taps i = a + padh, j = b + padw (mod 2)
+        out = (h, w)
+        launches = [([((a + padh - i) // 2, (b + padw - j) // 2, 0, i * kw + j)
+                      for i in range(kh) if (a + padh - i) % 2 == 0 for j in range(kw) if (b + padw - j) % 2 == 0],
+                     (h + 1) // 2, (w + 1) // 2, 2, a, b) for a in range(2) for b in range(2)]
+    elif d == DGRAD:            # the adjoint of every phase in one launch, phase p of g at block dn = p n
+        out = (h + 2 * halo, w + 2 * halo)
+        taps = [(-dh, -dw, p * n, t) for p, ts in enumerate(phases) for dh, dw, _, t in ts]
+        if cols:
+            taps = [taps[i * kw + j] for j in range(kw) for i in reversed(range(kh))]
+        launches = [(taps, *out, 1, 0, 0)]
+    else:                       # dW[t] = sum g[gdn + m, y, x] x[xdn + m, y + dh, x + dw] over the grid of g's copies
+        out = (h, w) if up else (oh, ow)
+        launches = [([(p * n,) + tap for p, ts in enumerate(phases) for tap in ts], *out, 1, 0, 0)]
+    return _Plan(xsplit, gsplit, up, ntaps, out, tuple((tuple(taps), *rest) for taps, *rest in launches))
+
+
+def _tc_launch(xs, n, ws, plan, y, k, bias=None, act=ACT_NONE, yoff=0, slope=LRELU_SLOPE):
+    """The og_conv2d_tc launches of a FPROP / DGRAD plan.  xs / ws: (hi, lo, scale word) operand triples; the source
+    is [SN, SH, SW, C] with SN = n or 4n (space-to-depth).  The k output channels start at channel yoff of y."""
     xh, xl, ax = xs
     wh, wl, aw = ws
     sn, sh, sw, c = xh.shape
     _, ohf, owf, kc = y.shape
-    arr = _int_array(taps)
-    import ctypes
-    _call("og_conv2d_tc", _p(xh), _p(xl), _p(ax), n, sn, sh, sw, c, _p(wh), _p(wl), _p(aw), ntaps_w, kw_rows,
-          _p(y) + 4 * yoff, oh, ow, k,
-          ohf * owf * kc, owf * kc, kc, ohf, owf, osy, osy, op[0], op[1], ctypes.addressof(arr), len(taps),
-          _p(bias), act, slope)
+    for taps, oh, ow, osy, opy, opx in plan.launches:
+        arr = _int_array(taps)
+        _call("og_conv2d_tc", _p(xh), _p(xl), _p(ax), n, sn, sh, sw, c, _p(wh), _p(wl), _p(aw), plan.ntaps, k,
+              _p(y) + 4 * yoff, oh, ow, k, ohf * owf * kc, owf * kc, kc, ohf, owf, osy, osy, opy, opx,
+              ctypes.addressof(arr), len(taps), _p(bias), act, slope)
 
 
-def _tc_kind(n, h, w, c, kh, kw, stride, pad, mode):
-    """Which tensor-core formulation (if any) applies to this convolution.  The batch need not fill the last pixel
-    tile: GEMM rows are independent and rows past the batch are never stored."""
-    if CONV_ENGINE != "f16x3" or _lib.DRY_RUN:
-        return None
-    if kh == kw and stride == 1 and pad == 1 and (kh == 3 or (kh == 4 and mode == PAD_ZERO)):
-        # 3x3 (any padding mode), and the 4x4 stride-1 zero-padded roi_code layer of the object discriminators
-        oh, ow = _out_hw(h, w, kh, kw, stride, pad, mode)
-        if n * oh * ow < TC_MIN_PIXELS:
-            return None
-        return "s1"
-    if kh == kw and kh in (3, 4) and stride == 2 and pad == 1 and mode == PAD_ZERO and h % 2 == 0 and w % 2 == 0:
-        if n * (h // 2) * (w // 2) < TC_MIN_PIXELS:
-            return None
-        return "s2"
-    return None
-
-
-_UP_OFF = ((-1, 0), (0, 1))   # low-res row/col offsets read by output phase 0 / 1 of upsample + conv3x3
-
-
-def _tc_fprop(kind, x, cache, weight, kp, split, splitp, mode, bias_p, act):
-    """Returns (y, xs): the output and the fp16 operand triple of x (reused by the weight gradient)."""
+def _simt_conv(x, wp, y, k, kh, kw, stride, padh, padw, mode, bias=None, act=ACT_NONE, slope=LRELU_SLOPE,
+               splitk=True, yoff=0):
+    """og_conv2d_simt from the contiguous NHWC x into k channels of y (N, OH, OW, Cy) from channel yoff; returns y."""
     n, h, w, c = x.shape
-    dev = x.device
-    if mode != UPSAMPLE2X:
-        ws = cache.get_hilo(weight, c, kp, split, splitp, 1)      # [tap][co][ci]
-    if kind == "s2":                                 # 4x4 / 3x3 stride 2 pad 1 on space-to-depth phases
-        k = weight.shape[2]
-        xs = _split(x, s2d=True)
-        y = torch.empty((n, h // 2, w // 2, kp), device=dev, dtype=torch.float32)
-        taps = []
-        for kh in range(k):
-            dh, a = divmod(kh - 1, 2)
-            for kw in range(k):
-                dw, b = divmod(kw - 1, 2)
-                taps.append((dh, dw, (a * 2 + b) * n, kh * k + kw))
-        _tc_launch(xs, n, ws, k * k, kp, y, h // 2, w // 2, kp, 1, (0, 0), taps, bias_p, act)
-        return y, xs
-    if mode == PAD_REFLECT:
-        xs = _split(x, 1)
-        y = torch.empty((n, h, w, kp), device=dev, dtype=torch.float32)
-        taps = [(kh, kw, 0, kh * 3 + kw) for kw in range(3) for kh in range(3)]      # column by column
-        _tc_launch(xs, n, ws, 9, kp, y, h, w, kp, 1, (0, 0), taps, bias_p, act)
-    elif mode == PAD_ZERO:
-        k = weight.shape[2]
-        xs = _split(x, 0)
-        oh, ow = h + 3 - k, w + 3 - k
-        y = torch.empty((n, oh, ow, kp), device=dev, dtype=torch.float32)
-        if k == 3:
-            taps = [(kh - 1, kw - 1, 0, kh * 3 + kw) for kw in range(3) for kh in range(3)]
-        else:
-            taps = [(kh - 1, kw - 1, 0, kh * k + kw) for kh in range(k) for kw in range(k)]
-        _tc_launch(xs, n, ws, k * k, kp, y, oh, ow, kp, 1, (0, 0), taps, bias_p, act)
-    else:  # UPSAMPLE2X: four output phases of 2x2 taps at low resolution, weights pre-summed per phase
-        ws = cache.get_up_hilo(weight, c, kp, split, splitp, 1)
-        xs = _split(x, 0)
-        y = torch.empty((n, 2 * h, 2 * w, kp), device=dev, dtype=torch.float32)
-        for py in range(2):
-            for px in range(2):
-                taps = [(_UP_OFF[py][a], _UP_OFF[px][b], 0, ((py * 2 + px) * 2 + a) * 2 + b)
-                        for a in range(2) for b in range(2)]
-                _tc_launch(xs, n, ws, 16, kp, y, h, w, kp, 2, (py, px), taps, bias_p, act)
-    return y, xs
-
-
-def _split_x(kind, x, mode):
-    """The operand copies _tc_fprop makes of x."""
-    if kind == "s2":
-        return _split(x, s2d=True)
-    return _split(x, 1 if mode == PAD_REFLECT else 0)
-
-
-def _split_g(kind, g, mode):
-    """Hi/lo copies of the output gradient shared by the input- and weight-gradient kernels."""
-    return _split(g, s2d=(kind == "s1" and mode == UPSAMPLE2X))
-
-
-def _tc_dgrad(kind, gs, n, cache, weight, c, kp, split, splitp, mode, h, w, oh, ow):
-    """Input gradient on the tensor cores.  gs: hi/lo of g (N, oh, ow, kp) from _split_g; returns (N, h, w, c)."""
-    dev = gs[0].device
-    if mode != UPSAMPLE2X:
-        ws = cache.get_hilo(weight, c, kp, split, splitp, 0)      # [tap][ci][co]
-    if kind == "s2":
-        k = weight.shape[2]
-        gx = torch.empty((n, h, w, c), device=dev, dtype=torch.float32)
-        for a in range(2):                       # input pixel (2i + a, 2j + b) <- kernel rows with kh = a + 1 (mod 2)
-            for b in range(2):
-                taps = [((a + 1 - kh) // 2, (b + 1 - kw) // 2, 0, kh * k + kw)
-                        for kh in range(k) if (a + 1 - kh) % 2 == 0 for kw in range(k) if (b + 1 - kw) % 2 == 0]
-                _tc_launch(gs, n, ws, k * k, c, gx, oh, ow, c, 2, (a, b), taps)
-        return gx
-    if mode == PAD_REFLECT:
-        gpad = torch.empty((n, h + 2, w + 2, c), device=dev, dtype=torch.float32)
-        taps = [(-kh, -kw, 0, kh * 3 + kw) for kw in range(3) for kh in (2, 1, 0)]   # rows ascending: -2, -1, 0
-        _tc_launch(gs, n, ws, 9, c, gpad, h + 2, w + 2, c, 1, (0, 0), taps)
-        gx = torch.empty((n, h, w, c), device=dev, dtype=torch.float32)
-        _call("og_reflect_pad_bwd", _p(gpad), n, h, w, c, _p(gx))
-        return gx
-    if mode == PAD_ZERO:
-        k = weight.shape[2]
-        gx = torch.empty((n, h, w, c), device=dev, dtype=torch.float32)
-        if k == 3:
-            taps = [(1 - kh, 1 - kw, 0, kh * 3 + kw) for kw in range(3) for kh in (2, 1, 0)]
-        else:       # gx[i, j] = sum g[i + 1 - kh, j + 1 - kw] W[kh, kw]^T over the (oh, ow) gradient grid
-            taps = [(1 - kh, 1 - kw, 0, kh * k + kw) for kh in range(k) for kw in range(k)]
-        _tc_launch(gs, n, ws, k * k, c, gx, h, w, c, 1, (0, 0), taps)
-        return gx
-    # UPSAMPLE2X: adjoint of the four phase convolutions: gx[i,j] = sum_{p,q,a,b} G_pq[i - off(p,a), j - off(q,b)] Wp^T
-    ws = cache.get_up_hilo(weight, c, kp, split, splitp, 0)
-    gx = torch.empty((n, h, w, c), device=dev, dtype=torch.float32)
-    taps = [(-_UP_OFF[p_][a], -_UP_OFF[q_][b], (p_ * 2 + q_) * n, ((p_ * 2 + q_) * 2 + a) * 2 + b)
-            for p_ in range(2) for q_ in range(2) for a in range(2) for b in range(2)]
-    _tc_launch(gs, n, ws, 16, c, gx, h, w, c, 1, (0, 0), taps)
-    return gx
+    _, oh, ow, cy = y.shape
+    _call("og_conv2d_simt", _p(x), n, h, w, c, h * w * c, w * c, c, _p(wp), _p(y) + 4 * yoff, oh, ow, k, oh * ow * cy,
+          ow * cy, cy, kh, kw, stride, padh, padw, mode, _p(bias), act, slope, 1 if splitk else 0)
+    return y
 
 
 def _grad_sink(param):
@@ -392,59 +398,59 @@ def _grad_sink(param):
     return None
 
 
-def _tc_wgrad(kind, xs, gs, n, h, w, oh, ow, weight, c, kp, split, splitp, mode, sink=None):
-    """Weight gradient on the tensor cores from the hi/lo copies of x (_split_x) and g (_split_g), both NHWC;
-    (h, w) is the extent of x, (oh, ow) of g.  Returns the OIHW gradient."""
-    import ctypes
+def _unpack_wgrad(dwp, weight, c, kp, split, splitp, sink, transposed=0, up=False):
+    """The OIHW gradient of a packed weight gradient ([tap][kp][c] when transposed, else [tap][c][kp]; up: the 16
+    phase taps of an upsample layer), added to the sink if there is one (then None is returned)."""
+    co, ci, kh, kw = weight.shape
+    gw = torch.empty_like(weight) if sink is None else sink
+    acc = 0 if sink is None else 1
+    if up:
+        _call("og_unpack_upsample_wgrad", _p(dwp), co, ci, c, kp, split, splitp, _p(gw), acc)
+    else:
+        _call("og_unpack_wgrad", _p(dwp), co, ci, kh, kw, c, kp, split, splitp, _p(gw), acc, transposed)
+    return gw if sink is None else None
+
+
+def _conv2d_geo(n, h, w, kh, kw, stride, pad, mode):
+    """The layer arguments of _tc_plan for a conv2d layer: its 3x3 layers' stride-1 taps run column by column."""
+    return n, h, w, kh, kw, stride, pad, pad, mode, kh == 3
+
+
+def _tc_fprop(x, cache, weight, kp, split, splitp, geo, bias_p, act):
+    """Returns (y, xs): the output and the fp16 operand triple of x (reused by the weight gradient)."""
+    plan = _tc_plan(FPROP, *geo)
+    ws = (cache.get_up_hilo if plan.up else cache.get_hilo)(weight, x.shape[3], kp, split, splitp, 1)
+    xs = _split(x, *plan.xsplit)
+    y = torch.empty((x.shape[0], *plan.out, kp), device=x.device, dtype=torch.float32)
+    _tc_launch(xs, x.shape[0], ws, plan, y, kp, bias_p, act)
+    return y, xs
+
+
+def _tc_dgrad(gs, cache, weight, c, kp, split, splitp, geo):
+    """Input gradient (N, h, w, c) on the tensor cores from gs, the hi/lo copies of g in the plan's gsplit layout."""
+    plan = _tc_plan(DGRAD, *geo)
+    n, h, w = geo[:3]
+    ws = (cache.get_up_hilo if plan.up else cache.get_hilo)(weight, c, kp, split, splitp, 0)
+    gx = torch.empty((n, *plan.out, c), device=gs[0].device, dtype=torch.float32)
+    _tc_launch(gs, n, ws, plan, gx, c)
+    if plan.out != (h, w):      # the reflection halo folds back onto the border
+        gpad, gx = gx, torch.empty((n, h, w, c), device=gx.device, dtype=torch.float32)
+        _call("og_reflect_pad_bwd", _p(gpad), n, h, w, c, _p(gx))
+    return gx
+
+
+def _tc_wgrad(xs, gs, weight, c, kp, split, splitp, geo, sink=None):
+    """Weight gradient on the tensor cores (og_conv2d_wgrad_tc) from the hi/lo copies of x and g; returns the OIHW
+    gradient (None with a sink)."""
+    plan = _tc_plan(WGRAD, *geo)
     xh, xl, ax = xs
     gh, gl, ag = gs
-    co, ci, kh_, kw_ = weight.shape
-    if kind == "s2":
-        ent = []
-        for kh in range(kh_):
-            dh, a = divmod(kh - 1, 2)
-            for kw in range(kw_):
-                dw, b = divmod(kw - 1, 2)
-                ent.append((0, dh, dw, (a * 2 + b) * n, kh * kw_ + kw))
-        nt = kh_ * kw_
-    elif mode == UPSAMPLE2X:
-        ent = [((p_ * 2 + q_) * n, _UP_OFF[p_][a], _UP_OFF[q_][b], 0, ((p_ * 2 + q_) * 2 + a) * 2 + b)
-               for p_ in range(2) for q_ in range(2) for a in range(2) for b in range(2)]
-        oh, ow, nt = h, w, 16
-    else:
-        off = 0 if mode == PAD_REFLECT else -1     # reflect: x copy carries the halo; zero pad: TMA fills
-        ent = [(0, kh + off, kw + off, 0, kh * kw_ + kw) for kh in range(kh_) for kw in range(kw_)]
-        nt = kh_ * kw_
-    arr = _int_array(ent)
-    dwp = torch.empty(nt * kp * c, device=xh.device, dtype=torch.float32)
-    _call("og_conv2d_wgrad_tc", _p(gh), _p(gl), _p(ag), n, gh.shape[0], oh, ow, kp, _p(xh), _p(xl), _p(ax),
-          xh.shape[0], xh.shape[1], xh.shape[2], c, _p(dwp), nt, ctypes.addressof(arr), len(ent))
-    if mode == UPSAMPLE2X and kind == "s1":
-        if sink is not None:
-            _call("og_unpack_upsample_wgrad", _p(dwp), co, ci, c, kp, split, splitp, _p(sink), 1)
-            return None
-        gw = torch.empty_like(weight)
-        _call("og_unpack_upsample_wgrad", _p(dwp), co, ci, c, kp, split, splitp, _p(gw), 0)
-        return gw
-    if sink is not None:
-        _call("og_unpack_wgrad", _p(dwp), co, ci, kh_, kw_, c, kp, split, splitp, _p(sink), 1, 1)
-        return None
-    gw = torch.empty_like(weight)
-    _call("og_unpack_wgrad", _p(dwp), co, ci, kh_, kw_, c, kp, split, splitp, _p(gw), 0, 1)
-    return gw
-
-
-def _out_hw(h, w, kh, kw, stride, pad, mode):
-    if mode == UPSAMPLE2X:
-        return 2 * h, 2 * w
-    return (h + 2 * pad - kh) // stride + 1, (w + 2 * pad - kw) // stride + 1
-
-
-def _conv_raw(x, wp, n, h, w, c, oh, ow, k, kh, kw, stride, pad, mode, bias, act, splitk=True):
-    y = torch.empty((n, oh, ow, k), device=x.device, dtype=torch.float32)
-    _call("og_conv2d_simt", _p(x), n, h, w, c, h * w * c, w * c, c, _p(wp), _p(y), oh, ow, k, oh * ow * k, ow * k, k,
-          kh, kw, stride, pad, pad, mode, _p(bias), act, LRELU_SLOPE, 1 if splitk else 0)
-    return y
+    (ents, oh, ow, _, _, _), = plan.launches
+    arr = _int_array(ents)
+    dwp = torch.empty(plan.ntaps * kp * c, device=xh.device, dtype=torch.float32)
+    _call("og_conv2d_wgrad_tc", _p(gh), _p(gl), _p(ag), geo[0], gh.shape[0], oh, ow, kp, _p(xh), _p(xl), _p(ax),
+          xh.shape[0], xh.shape[1], xh.shape[2], c, _p(dwp), plan.ntaps, ctypes.addressof(arr), len(ents))
+    return _unpack_wgrad(dwp, weight, c, kp, split, splitp, sink, 1, plan.up)
 
 
 class _Conv2d(torch.autograd.Function):
@@ -465,7 +471,11 @@ class _Conv2d(torch.autograd.Function):
             splitp, kp = 0, cpad(co)
         need_t = ctx.needs_input_grad[0]
         oh, ow = _out_hw(h, w, kh, kw, stride, pad, mode)
-        kind = _tc_kind(n, h, w, c, kh, kw, stride, pad, mode)
+        # a dry run keeps every layer on its CUDA-core form (the host-logic tests pin those call sequences)
+        kind = None if _lib.DRY_RUN else _tc_kind(n, h, w, c, kh, kw, stride, pad, mode)
+        path = kind or conv_path(n, h, w, kh, kw, stride, pad, pad, mode, kp, "simt")    # narrow or simt
+        tc = kind is not None
+        geo = _conv2d_geo(n, h, w, kh, kw, stride, pad, mode)
         bias_p = None
         if bias is not None:
             if kp == co:
@@ -474,29 +484,27 @@ class _Conv2d(torch.autograd.Function):
                 assert not split
                 bias_p = torch.zeros(kp, device=x.device, dtype=torch.float32)
                 bias_p[:co] = bias.detach()
-        narrow = kind is None and kp == 8 and mode == PAD_ZERO and n * oh * ow <= 65536
         f32_missing = getattr(x, "og_f32_invalid", False)
-        if f32_missing and not kind:
+        if f32_missing and not tc:
             raise RuntimeError("input exists only as tensor-core operand copies, but this convolution runs on the CUDA cores")
         xs = None
-        if kind:
-            y, xs = _tc_fprop(kind, x, cache, weight, kp, split, splitp, mode, bias_p, act)
+        if tc:
+            y, xs = _tc_fprop(x, cache, weight, kp, split, splitp, geo, bias_p, act)
             if not ctx.needs_input_grad[1] and not f32_missing:
                 xs = None
-        elif narrow:
+        elif path == "narrow":
             wf, _ = cache.get(weight, c, kp, split, splitp, False)
             y = torch.empty((n, oh, ow, 8), device=x.device, dtype=torch.float32)
             _call("og_conv2d_narrow_fwd", _p(x), n, h, w, c, _p(wf), _p(y), oh, ow, kh, kw, stride, pad, _p(bias_p), act,
                   LRELU_SLOPE)
         else:
             wf, _ = cache.get(weight, c, kp, split, splitp, False)
-            y = _conv_raw(x, wf, n, h, w, c, oh, ow, kp, kh, kw, stride, pad, mode, bias_p, act,
-                          splitk=(bias is None and act == ACT_NONE))
-        ctx.kind = kind
+            y = _simt_conv(x, wf, torch.empty((n, oh, ow, kp), device=x.device, dtype=torch.float32), kp, kh, kw,
+                           stride, pad, pad, mode, bias_p, act, splitk=(bias is None and act == ACT_NONE))
+        ctx.path, ctx.geo = path, geo
         ctx.wsink = _grad_sink(weight)
         ctx.bsink = _grad_sink(bias) if bias is not None else None
         ctx.xs = xs                      # hi/lo operand copies of x, reused by the weight gradient
-        ctx.narrow = narrow
         ctx.cfg = (stride, pad, mode, act, split, splitp, kp, need_t)
         ctx.cache = cache
         ctx.has_bias = bias is not None
@@ -523,51 +531,47 @@ class _Conv2d(torch.autograd.Function):
             else:
                 gb = torch.empty(co, device=g.device, dtype=torch.float32)
                 _call("og_channel_sum", _p(g), n * oh * ow, kp, _p(scratch), _p(gb), co, 0)
-        kind = ctx.kind
-        if ctx.narrow:
-            wf, _ = ctx.cache.get(weight, c, kp, split, splitp, False)
+        path, geo, cache = ctx.path, ctx.geo, ctx.cache
+        if path == "narrow":
+            wf, _ = cache.get(weight, c, kp, split, splitp, False)
             if ctx.needs_input_grad[0]:
                 gx = torch.empty_like(x)
                 _call("og_conv2d_narrow_dgrad", _p(g), n, h, w, c, _p(wf), _p(gx), oh, ow, kh, kw, stride, pad)
             if ctx.needs_input_grad[1]:
                 dwp = torch.empty(kh * kw * c * 8, device=g.device, dtype=torch.float32)
                 _call("og_conv2d_narrow_wgrad", _p(x), n, h, w, c, _p(g), _p(dwp), oh, ow, kh, kw, stride, pad)
-                if ctx.wsink is not None:
-                    _call("og_unpack_wgrad", _p(dwp), co, ci, kh, kw, c, kp, split, splitp, _p(ctx.wsink), 1, 0)
-                else:
-                    gw = torch.empty_like(weight)
-                    _call("og_unpack_wgrad", _p(dwp), co, ci, kh, kw, c, kp, split, splitp, _p(gw), 0, 0)
-            return gx, gw, gb, None, None, None, None, None, None
-        tc_w = bool(ctx.needs_input_grad[1] and kind)
-        gs = _split_g(kind, g, mode) if kind and (ctx.needs_input_grad[0] or tc_w) else None
-        if ctx.needs_input_grad[0] and kind:
-            gx = _tc_dgrad(kind, gs, n, ctx.cache, weight, c, kp, split, splitp, mode, h, w, oh, ow)
-        elif ctx.needs_input_grad[0]:
-            _, wt = ctx.cache.get(weight, c, kp, split, splitp, True)
-            if mode == PAD_ZERO:
-                gx = _conv_raw(g, wt, n, oh, ow, kp, h, w, c, kh, kw, stride, pad, TRANSPOSED, None, ACT_NONE)
-            elif mode == PAD_REFLECT:
-                assert stride == 1 and pad == 1
-                gpad = _conv_raw(g, wt, n, oh, ow, kp, h + 2, w + 2, c, kh, kw, 1, 0, TRANSPOSED, None, ACT_NONE)
-                gx = torch.empty_like(x)
-                _call("og_reflect_pad_bwd", _p(gpad), n, h, w, c, _p(gx))
-            else:  # UPSAMPLE2X
-                gu = _conv_raw(g, wt, n, oh, ow, kp, 2 * h, 2 * w, c, kh, kw, 1, pad, TRANSPOSED, None, ACT_NONE)
-                gx = torch.empty_like(x)
-                _call("og_upsample2x_bwd", _p(gu), n, h, w, c, _p(gx))
-        if tc_w:
-            xs = ctx.xs if ctx.xs is not None else _split_x(kind, x, mode)
-            ctx.xs = None
-            gw = _tc_wgrad(kind, xs, gs, n, h, w, oh, ow, weight, c, kp, split, splitp, mode, ctx.wsink)
-        elif ctx.needs_input_grad[1]:
-            dwp = torch.empty(kh * kw * c * kp, device=g.device, dtype=torch.float32)
-            _call("og_conv2d_wgrad_simt", _p(x), n, h, w, c, h * w * c, w * c, c, _p(g), oh, ow, kp, oh * ow * kp,
-                  ow * kp, kp, _p(dwp), kh, kw, stride, pad, mode)
-            if ctx.wsink is not None:
-                _call("og_unpack_wgrad", _p(dwp), co, ci, kh, kw, c, kp, split, splitp, _p(ctx.wsink), 1, 0)
-            else:
-                gw = torch.empty_like(weight)
-                _call("og_unpack_wgrad", _p(dwp), co, ci, kh, kw, c, kp, split, splitp, _p(gw), 0, 0)
+                gw = _unpack_wgrad(dwp, weight, c, kp, split, splitp, ctx.wsink)
+        elif path in ("s1", "s2"):
+            gs = None
+            if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+                gs = _split(g, *_tc_plan(DGRAD, *geo).gsplit)
+            if ctx.needs_input_grad[0]:
+                gx = _tc_dgrad(gs, cache, weight, c, kp, split, splitp, geo)
+            if ctx.needs_input_grad[1]:
+                xs = ctx.xs if ctx.xs is not None else _split(x, *_tc_plan(WGRAD, *geo).xsplit)
+                ctx.xs = None
+                gw = _tc_wgrad(xs, gs, weight, c, kp, split, splitp, geo, ctx.wsink)
+        else:
+            if ctx.needs_input_grad[0]:     # the adjoint as a TRANSPOSED convolution onto the padded / 2x extent
+                _, wt = cache.get(weight, c, kp, split, splitp, True)
+                if mode == PAD_ZERO:
+                    gx = _simt_conv(g, wt, torch.empty_like(x), c, kh, kw, stride, pad, pad, TRANSPOSED)
+                elif mode == PAD_REFLECT:
+                    assert stride == 1 and pad == 1
+                    gpad = _simt_conv(g, wt, torch.empty((n, h + 2, w + 2, c), device=g.device, dtype=torch.float32),
+                                      c, kh, kw, 1, 0, 0, TRANSPOSED)
+                    gx = torch.empty_like(x)
+                    _call("og_reflect_pad_bwd", _p(gpad), n, h, w, c, _p(gx))
+                else:  # UPSAMPLE2X
+                    gu = _simt_conv(g, wt, torch.empty((n, 2 * h, 2 * w, c), device=g.device, dtype=torch.float32),
+                                    c, kh, kw, 1, pad, pad, TRANSPOSED)
+                    gx = torch.empty_like(x)
+                    _call("og_upsample2x_bwd", _p(gu), n, h, w, c, _p(gx))
+            if ctx.needs_input_grad[1]:
+                dwp = torch.empty(kh * kw * c * kp, device=g.device, dtype=torch.float32)
+                _call("og_conv2d_wgrad_simt", _p(x), n, h, w, c, h * w * c, w * c, c, _p(g), oh, ow, kp, oh * ow * kp,
+                      ow * kp, kp, _p(dwp), kh, kw, stride, pad, mode)
+                gw = _unpack_wgrad(dwp, weight, c, kp, split, splitp, ctx.wsink)
         return gx, gw, gb, None, None, None, None, None, None
 
 
@@ -1661,8 +1665,9 @@ def linear_rows(x, w, bias, cache):
     co, ci = w.shape[:2]
     assert c == cpad(ci) and co % 4 == 0
     wf, _ = cache.get(w, c, co, 0, 0, False)
-    return _conv_raw(x.contiguous(), wf, n, 1, 1, c, 1, 1, co, 1, 1, 1, 0, PAD_ZERO, bias, ACT_NONE,
-                     splitk=False).view(n, co)
+    y = torch.empty((n, 1, 1, co), device=x.device, dtype=torch.float32)
+    return _simt_conv(x.contiguous().view(n, 1, 1, c), wf, y, co, 1, 1, 1, 0, 0, PAD_ZERO, bias,
+                      splitk=False).view(n, co)
 
 
 def lstm_bidir(gx, whh_f, whh_b, cap_lens, max_len):
@@ -1802,11 +1807,11 @@ def boxes_to_layout(labels, samples, steps, mean_std, label_to_class, count_stat
 
 
 # --------------------------------------------------------------------------------------------------
-# Inception-v3 image encoder (CNN_ENCODER, ref: model.py:182-287).  Its convolutions have their own dispatch: the
-# tap-list tensor-core launcher for every kernel shape (1x1, 1xN, Nx1, 3x3, 5x5, valid 3x3 stride 2), the exact-fp32
-# SIMT kernel under TC_MIN_PIXELS output pixels or with CONV_ENGINE = "simt".  _tc_kind and the routes of the other
-# layers are not involved.  Eval BatchNorm is folded into the weights and the bias (og_bn_fold), ReLU is the LeakyReLU
-# epilogue with slope 0.  The backward computes the input gradient only; the encoder is frozen.
+# Inception-v3 image encoder (CNN_ENCODER, ref: model.py:182-287).  Its convolutions take the tensor cores at every
+# kernel shape (1x1, 1xN, Nx1, 3x3, 5x5, valid 3x3 stride 2; conv_path's general form), the exact-fp32 SIMT kernel
+# under TC_MIN_PIXELS output pixels or with CONV_ENGINE = "simt".  Eval BatchNorm is folded into the weights and the
+# bias (og_bn_fold), ReLU is the LeakyReLU epilogue with slope 0.  The backward computes the input gradient only; the
+# encoder is frozen.
 # --------------------------------------------------------------------------------------------------
 class EncConv:
     """One BasicConv2d (conv without bias -> BatchNorm2d(eps=0.001) in eval mode -> ReLU), or several that read the
@@ -1850,23 +1855,9 @@ class EncConv:
     def out_hw(self, h, w):
         return ((h + 2 * self.padh - self.kh) // self.stride + 1, (w + 2 * self.padw - self.kw) // self.stride + 1)
 
-    def on_tc(self, n, h, w):
-        oh, ow = self.out_hw(h, w)
-        return CONV_ENGINE == "f16x3" and n * oh * ow >= TC_MIN_PIXELS
-
     def macs(self, h, w):
         oh, ow = self.out_hw(h, w)
         return oh * ow * self.cout * self.cin * self.kh * self.kw
-
-
-def _split_s2d_odd(x):
-    n, h, w, c = x.shape
-    shape = (4 * n, (h + 1) // 2, (w + 1) // 2, c)
-    xh = _empty_slack(shape, x.device)
-    xl = _empty_slack(shape, x.device)
-    amax = torch.empty(1, device=x.device, dtype=torch.int32)
-    _call("og_prep_split_s2d", _p(x), n, h, w, c, _p(amax), 0, _p(xh), _p(xl))
-    return xh, xl, amax
 
 
 def enc_conv_fwd(layer, x, y, yoff=0):
@@ -1878,28 +1869,15 @@ def enc_conv_fwd(layer, x, y, yoff=0):
     assert y.shape[1:3] == (oh, ow) and yoff + layer.cout <= cy
     wf, bias, cache = layer.folded()
     k = layer.cout
-    yptr = y.data_ptr() + yoff * 4
-    ystr = (oh * ow * cy, ow * cy, cy)
-    if layer.on_tc(n, h, w):
-        ws = cache.get_hilo(wf, c, k, 0, 0, 1)                    # [tap][co][ci]
-        kk = layer.kh * layer.kw
-        if layer.stride == 2:                                     # valid 3x3 stride 2 on the phase blocks
-            xs = _split_s2d_odd(x)
-            taps = []
-            for i in range(layer.kh):
-                dh, a = divmod(i, 2)
-                for j in range(layer.kw):
-                    dw, b = divmod(j, 2)
-                    taps.append((dh, dw, (a * 2 + b) * n, i * layer.kw + j))
-        else:
-            xs = _split(x, 0)
-            taps = [(i - layer.padh, j - layer.padw, 0, i * layer.kw + j) for i in range(layer.kh) for j in range(layer.kw)]
-        _tc_launch(xs, n, ws, kk, k, y, oh, ow, k, 1, (0, 0), taps, bias, layer.act, yoff=yoff, slope=0.0)
-    else:
+    geo = (n, h, w, layer.kh, layer.kw, layer.stride, layer.padh, layer.padw, PAD_ZERO)
+    if conv_path(*geo, k, CONV_ENGINE, general=True) == "simt":
         wp, _ = cache.get(wf, c, k, 0, 0, False)
-        _call("og_conv2d_simt", _p(x), n, h, w, c, h * w * c, w * c, c, _p(wp), yptr, oh, ow, k, ystr[0], ystr[1],
-              ystr[2], layer.kh, layer.kw, layer.stride, layer.padh, layer.padw, PAD_ZERO, _p(bias), layer.act, 0.0,
-              1 if (bias is None and layer.act == ACT_NONE and yoff == 0 and cy == k) else 0)
+        _simt_conv(x, wp, y, k, *geo[3:], bias, layer.act, 0.0,
+                   bias is None and layer.act == ACT_NONE and yoff == 0 and cy == k, yoff)
+    else:
+        plan = _tc_plan(FPROP, *geo)
+        ws = cache.get_hilo(wf, c, k, 0, 0, 1)                    # [tap][co][ci]
+        _tc_launch(_split(x, *plan.xsplit), n, ws, plan, y, k, bias, layer.act, yoff, 0.0)
 
 
 def enc_conv_dgrad(layer, gp, h, w):
@@ -1908,23 +1886,14 @@ def enc_conv_dgrad(layer, gp, h, w):
     c = cpad(layer.cin)
     wf, _, cache = layer.folded()
     gx = torch.empty((n, h, w, c), device=gp.device, dtype=torch.float32)
-    if layer.on_tc(n, h, w):
-        ws = cache.get_hilo(wf, c, k, 0, 0, 0)                    # [tap][ci][co]
-        gs = _split(gp, 0)
-        if layer.stride == 2:     # input pixel (2i + a, 2j + b) <- kernel taps with kh = a, kw = b (mod 2)
-            for a in range(2):
-                for b in range(2):
-                    taps = [(-((i - a) // 2), -((j - b) // 2), 0, i * layer.kw + j)
-                            for i in range(layer.kh) if (i - a) % 2 == 0 for j in range(layer.kw) if (j - b) % 2 == 0]
-                    _tc_launch(gs, n, ws, layer.kh * layer.kw, c, gx, (h + 1) // 2, (w + 1) // 2, c, 2, (a, b), taps,
-                               slope=0.0)
-        else:
-            taps = [(layer.padh - i, layer.padw - j, 0, i * layer.kw + j) for i in range(layer.kh) for j in range(layer.kw)]
-            _tc_launch(gs, n, ws, layer.kh * layer.kw, c, gx, h, w, c, 1, (0, 0), taps, slope=0.0)
-    else:
+    geo = (n, h, w, layer.kh, layer.kw, layer.stride, layer.padh, layer.padw, PAD_ZERO)
+    if conv_path(*geo, k, CONV_ENGINE, general=True) == "simt":
         _, wt = cache.get(wf, c, k, 0, 0, True)
-        _call("og_conv2d_simt", _p(gp), n, oh, ow, k, oh * ow * k, ow * k, k, _p(wt), _p(gx), h, w, c, h * w * c,
-              w * c, c, layer.kh, layer.kw, layer.stride, layer.padh, layer.padw, TRANSPOSED, 0, ACT_NONE, 0.0, 1)
+        _simt_conv(gp, wt, gx, c, *geo[3:8], TRANSPOSED, slope=0.0)
+    else:
+        plan = _tc_plan(DGRAD, *geo)
+        ws = cache.get_hilo(wf, c, k, 0, 0, 0)                    # [tap][ci][co]
+        _tc_launch(_split(gp, *plan.gsplit), n, ws, plan, gx, c, slope=0.0)
     return gx
 
 

@@ -7,11 +7,11 @@ A CASES / EDGE_CASES row is (N, H, W, Cin, Cout, k, stride, pad, mode, act, bias
   stride, pad   as nn.Conv2d;  mode  lib.PAD_ZERO / PAD_REFLECT / UPSAMPLE2X (nearest 2x upsample, then the conv)
   act           lib.ACT_NONE / ACT_LRELU / ACT_TANH / ACT_SIGMOID, applied in the epilogue
   bias          a bias is added in the epilogue;  split  GLU halves: Cout = 2 split, each half padded to cpad(split)
-  path          the path the f16x3 engine takes: "s1" / "s2" (tensor cores, ops._tc_kind), "narrow" (8 padded output
+  path          the path the f16x3 engine takes (ops.conv_path): "s1" / "s2" (tensor cores), "narrow" (8 padded output
                 channels on small maps: og_conv2d_narrow_*), "simt" (og_conv2d_simt / og_conv2d_wgrad_simt)
 An ENC_CASES row is (dir, N, H, W, Cin, Cout, kh, kw, stride, padh, padw, relu, bias, yoff, Cy, path): one call of
 ops.enc_conv_fwd (dir "fwd": output channels [yoff, yoff + Cout) of a Cy-channel destination) or ops.enc_conv_dgrad
-(dir "dgrad": yoff 0, Cy = cpad(Cin), the input gradient); path "tc" or "simt" (EncConv.on_tc).
+(dir "dgrad": yoff 0, Cy = cpad(Cin), the input gradient); path "tc" or "simt" (ops.conv_path).
 Rows are kept at the size the networks run them (no batch is cut), so a shape the networks issue must be in the table
 as it stands.
 """
@@ -270,28 +270,19 @@ ENC_CASES = [
 
 
 def path_of(N, H, W, Cin, Cout, k, stride, pad, mode, split):
-    """The path the f16x3 engine takes for this layer: ops._tc_kind (with lib.DRY_RUN lifted for the call: under a dry
-    run it always answers None) and ops._Conv2d's narrow condition."""
-    from objgan_b200 import lib, ops
+    """The path the f16x3 engine takes for this layer (ops.conv_path)."""
+    from objgan_b200 import ops
     from objgan_b200.ops import cpad
-    dry, engine = lib.DRY_RUN, ops.CONV_ENGINE
-    lib.DRY_RUN, ops.CONV_ENGINE = False, "f16x3"
-    try:
-        kind = ops._tc_kind(N, H, W, cpad(Cin), k, k, stride, pad, mode)
-    finally:
-        lib.DRY_RUN, ops.CONV_ENGINE = dry, engine
-    if kind:
-        return kind
-    oh, ow = ops._out_hw(H, W, k, k, stride, pad, mode)
     kp = 2 * cpad(split) if split else cpad(Cout)
-    return "narrow" if kp == 8 and mode == PAD_ZERO and N * oh * ow <= 65536 else "simt"
+    return ops.conv_path(N, H, W, k, k, stride, pad, pad, mode, kp, "f16x3")
 
 
 def enc_path(N, H, W, kh, kw, stride, padh, padw):
-    """EncConv.on_tc under the f16x3 engine."""
+    """ops.conv_path of an encoder layer (the general form, which has no narrow path: kp is not read) under the f16x3
+    engine, as "tc" or "simt"."""
     from objgan_b200 import ops
-    oh, ow = (H + 2 * padh - kh) // stride + 1, (W + 2 * padw - kw) // stride + 1
-    return "tc" if N * oh * ow >= ops.TC_MIN_PIXELS else "simt"
+    path = ops.conv_path(N, H, W, kh, kw, stride, padh, padw, PAD_ZERO, 0, "f16x3", general=True)
+    return "simt" if path == "simt" else "tc"
 
 
 def conv_needs(fn):

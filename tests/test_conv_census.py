@@ -69,7 +69,7 @@ def test_no_case_is_stale(dry):
 
 
 def test_paths_are_the_gpu_rule():
-    """The path column of every row is what ops._tc_kind and the narrow condition pick (EncConv.on_tc for ENC_CASES):
+    """The path column of every row is what ops.conv_path picks (its general form for ENC_CASES):
     a change of TC_MIN_PIXELS or of the dispatch moves rows, and shows up as a table edit."""
     assert [r for r in CASES + EDGE_CASES if path_of(*r[:9], r[11]) != r[12]] == []
     assert [r for r in ENC_CASES if enc_path(*r[1:4], *r[6:11]) != r[15]] == []
