@@ -71,9 +71,10 @@ class _Lib:
 
 
 _lib = None
-# Host-logic tracing switch used ONLY by the CPU unit tests (tests/test_host_logic.py): when True, operator
-# wrappers skip the kernel launch entirely (outputs are uninitialised memory), so shapes / autograd wiring /
-# state_dict plumbing can be exercised on a machine without a GPU.  It is not a compute path.
+# Dry run, for the CPU unit tests: the host code takes the same dispatch as on the GPU, ops._chk accepts host
+# tensors, and ops._call checks each call's argument count against the header and counts it instead of launching
+# (outputs stay uninitialised).  Nothing else reads it, so shapes / autograd wiring / call sequences / state_dict
+# plumbing are those of a device run, exercised on a machine without a GPU.  It is not a compute path.
 DRY_RUN = False
 
 

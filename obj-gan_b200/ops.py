@@ -171,7 +171,7 @@ class PackPlan:
 
     def run(self):
         """Call after the weights changed (and after the parameter epoch was bumped)."""
-        if not self.jobs or _lib.DRY_RUN:
+        if not self.jobs:
             return
         if self._tables is None or self._n_built != len(self.jobs):
             self._build(self.jobs[0][1].device)
@@ -471,8 +471,7 @@ class _Conv2d(torch.autograd.Function):
             splitp, kp = 0, cpad(co)
         need_t = ctx.needs_input_grad[0]
         oh, ow = _out_hw(h, w, kh, kw, stride, pad, mode)
-        # a dry run keeps every layer on its CUDA-core form (the host-logic tests pin those call sequences)
-        kind = None if _lib.DRY_RUN else _tc_kind(n, h, w, c, kh, kw, stride, pad, mode)
+        kind = _tc_kind(n, h, w, c, kh, kw, stride, pad, mode)
         path = kind or conv_path(n, h, w, kh, kw, stride, pad, pad, mode, kp, "simt")    # narrow or simt
         tc = kind is not None
         geo = _conv2d_geo(n, h, w, kh, kw, stride, pad, mode)
@@ -605,7 +604,7 @@ class _NormAct(torch.autograd.Function):
         if res is not None:
             res = res.contiguous()
             assert res.shape == out.shape
-        fused = (split_pad is not None and CONV_ENGINE == "f16x3" and not _lib.DRY_RUN
+        fused = (split_pad is not None and CONV_ENGINE == "f16x3"
                  and (res is None or _known_amax(res) is not None) and (split_pad == 0 or (h > 1 and w > 1)))
         if fused:
             # the consuming convolution's operand copies straight from this pass, scaled by an a-priori bound of max|out|
@@ -760,7 +759,7 @@ _CONST_CACHE_SLOTS = 12
 
 def cached_const(src, key, fn):
     import weakref
-    if src.requires_grad or _lib.DRY_RUN or not src.is_cuda or torch.cuda.is_current_stream_capturing():
+    if src.requires_grad or not src.is_cuda or torch.cuda.is_current_stream_capturing():
         return fn()
     for ref, ver, k, val in _CONST_CACHE:
         if k == key and ver == src._version and ref() is src:
@@ -1706,15 +1705,14 @@ def class_label_emb(glove_weight, cat_labels, cat_label_lens, order):
     "resort" indices).  Returns (N, E)."""
     lab, lens, order = _i64(cat_labels), _i64(cat_label_lens), _i64(order)
     n, e = order.shape[0], glove_weight.shape[1]
-    if not _lib.DRY_RUN:                       # built once per sampler: a host read of the tables is cheap here
-        lab_h, lens_h, order_h = lab.cpu(), lens.cpu(), order.cpu()
-        read = (torch.arange(lab_h.shape[1]).view(1, -1) < lens_h.view(-1, 1)) & (lens_h <= 2).view(-1, 1)
-        if lens_h.shape[0] != lab_h.shape[0] or bool(((lens_h == 2) & (lab_h.shape[1] < 2)).any()):
-            raise ValueError("cat_label_lens does not match cat_labels")
-        if bool(((lab_h < 0) | (lab_h >= glove_weight.shape[0]))[read].any()):
-            raise ValueError("a class label token is outside the GloVe table")
-        if bool(((order_h < 0) | (order_h >= lab_h.shape[0])).any()):
-            raise ValueError("cat_label_order indexes past the labels")
+    lab_h, lens_h, order_h = lab.cpu(), lens.cpu(), order.cpu()   # built once per sampler: a host read is cheap here
+    read = (torch.arange(lab_h.shape[1]).view(1, -1) < lens_h.view(-1, 1)) & (lens_h <= 2).view(-1, 1)
+    if lens_h.shape[0] != lab_h.shape[0] or bool(((lens_h == 2) & (lab_h.shape[1] < 2)).any()):
+        raise ValueError("cat_label_lens does not match cat_labels")
+    if bool(((lab_h < 0) | (lab_h >= glove_weight.shape[0]))[read].any()):
+        raise ValueError("a class label token is outside the GloVe table")
+    if bool(((order_h < 0) | (order_h >= lab_h.shape[0])).any()):
+        raise ValueError("cat_label_order indexes past the labels")
     _chk(glove_weight, lab, lens, order)
     out = torch.empty((n, e), device=glove_weight.device, dtype=torch.float32)
     _call("og_class_label_emb", _p(glove_weight.detach().contiguous()), e, _p(lab), lab.shape[1], _p(lens), _p(order),

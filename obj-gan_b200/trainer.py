@@ -20,7 +20,6 @@ import warnings
 import torch
 import torch.distributed as dist
 
-from . import lib as _lib
 from . import losses, model, ops, snapshots
 from .config import cfg
 
@@ -291,7 +290,7 @@ class StepATrainer:
 
     def _branch_streams(self):
         """Side streams for the three independent discriminator branches (None: run them in sequence)."""
-        if not torch.cuda.is_available() or _lib.DRY_RUN:
+        if self.device.type != "cuda":
             return None
         if not hasattr(self, "_dstreams"):
             self._dstreams = [torch.cuda.Stream() for _ in self.netsPatD]

@@ -1,5 +1,5 @@
 """Shapes of the attention and mask-paint kernels (csrc/attention.cu, csrc/attention_tc.cu), shared by
-tests/test_gpu_attention.py (which runs every row against a float64 restatement) and tests/test_attention_census.py
+tests/test_gpu_attention.py (which runs every row against a float64 restatement) and tests/test_census.py
 (which checks that the networks issue no shape missing here).
 
 One table of rows per C entry point:
@@ -126,15 +126,12 @@ def matches(need, row):
     return all(n is None or n == r for n, r in zip(need, row))
 
 
-def att_needs(fn):
-    """Runs ``fn()`` (which must issue its library calls under lib.DRY_RUN) and returns the set of (entry, pattern)
-    pairs its attention, paint and word-projection calls need: patterns shaped like a row of that entry's table, None
-    where the call does not fix the field."""
-    from objgan_b200 import ops
+def att_needs(work):
+    """The set of (entry, pattern) pairs the attention, paint and word-projection calls of a recorded workload
+    (tests/dry.py) need: patterns shaped like a row of that entry's table, None where the call does not fix the
+    field."""
     needs = set()
-    real = ops._call
-
-    def rec(name, *a):
+    for name, a in work.calls:
         if name == FWD:          # h, src, mask, B, Q, idf, cs, L, wc, attn
             needs.add((name, (a[3], a[4], a[5], a[6], a[7], bool(a[2]), False)))
         elif name == BWD:        # h, src, attn, g_wc, g_attn, B, Q, idf, cs, L, g_h, g_src
@@ -151,12 +148,6 @@ def att_needs(fn):
             needs.add((name, (a[2], a[3], a[4], a[5])))
         elif name == PROJ_BWD:   # words, W, gsrc, B, idf, cdf, L, gW, accumulate, gwords
             needs.add((name, (a[3], a[4], a[5], a[6])))
-        return real(name, *a)
-    ops._call = rec
-    try:
-        fn()
-    finally:
-        ops._call = real
     return needs
 
 

@@ -1,5 +1,5 @@
 """Shapes of the convolutions (csrc/conv_tc.cu, conv_simt.cu, wgmma.cuh), shared by tests/test_gpu_conv.py (which runs
-every row against float64 on both engines) and tests/test_conv_census.py (which checks that the networks issue no shape
+every row against float64 on both engines) and tests/test_census.py (which checks that the networks issue no shape
 missing here, that no row is stale, and that each row's path is the one the GPU takes).
 
 A CASES / EDGE_CASES row is (N, H, W, Cin, Cout, k, stride, pad, mode, act, bias, split, path):
@@ -285,41 +285,11 @@ def enc_path(N, H, W, kh, kw, stride, padh, padw):
     return "simt" if path == "simt" else "tc"
 
 
-def conv_needs(fn):
-    """Runs ``fn()`` (which must issue its library calls under lib.DRY_RUN) and returns the set of rows its convolutions
-    need: CASES-shaped tuples for ops.conv2d, ENC_CASES-shaped tuples for ops.enc_conv_fwd / enc_conv_dgrad."""
-    from objgan_b200 import ops
-    needs = set()
-    real_fwd, real_efwd, real_edgrad = ops._Conv2d.forward, ops.enc_conv_fwd, ops.enc_conv_dgrad
-
-    def fwd(ctx, x, weight, bias, cache, stride, pad, mode, act, split):
-        n, h, w, _ = x.shape
-        co, ci, k, _ = weight.shape
-        needs.add((n, h, w, ci, co, k, stride, pad, mode, act, bias is not None, split,
-                   path_of(n, h, w, ci, co, k, stride, pad, mode, split)))
-        return real_fwd(ctx, x, weight, bias, cache, stride, pad, mode, act, split)
-
-    def efwd(layer, x, y, yoff=0):
-        n, h, w, _ = x.shape
-        needs.add(_enc_row("fwd", layer, n, h, w, yoff, y.shape[3]))
-        return real_efwd(layer, x, y, yoff)
-
-    def edgrad(layer, gp, h, w):
-        needs.add(_enc_row("dgrad", layer, gp.shape[0], h, w, 0, ops.cpad(layer.cin)))
-        return real_edgrad(layer, gp, h, w)
-
-    ops._Conv2d.forward, ops.enc_conv_fwd, ops.enc_conv_dgrad = staticmethod(fwd), efwd, edgrad
-    try:
-        fn()
-    finally:
-        ops._Conv2d.forward, ops.enc_conv_fwd, ops.enc_conv_dgrad = staticmethod(real_fwd), real_efwd, real_edgrad
-    return needs
-
-
-def _enc_row(d, layer, n, h, w, yoff, cy):
-    return (d, n, h, w, layer.cin, layer.cout, layer.kh, layer.kw, layer.stride, layer.padh, layer.padw,
-            layer.act == ACT_LRELU, layer.bns is not None or len(layer.weights) > 1, yoff, cy,
-            enc_path(n, h, w, layer.kh, layer.kw, layer.stride, layer.padh, layer.padw))
+def conv_needs(work):
+    """The set of rows the convolutions of a recorded workload (tests/dry.py) need: CASES-shaped tuples for
+    ops.conv2d, ENC_CASES-shaped tuples for ops.enc_conv_fwd / enc_conv_dgrad."""
+    return ({r + (path_of(*r[:9], r[11]),) for r in work.convs} |
+            {r + (enc_path(*r[1:4], *r[6:11]),) for r in work.encs})
 
 
 def uncovered(needs):

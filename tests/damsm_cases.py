@@ -1,6 +1,6 @@
 """Shapes of the DAMSM matching kernels (csrc/words_pairs.cu, csrc/damsm.cu) and of the image encoder's backward
 gathers that carry the DAMSM gradient back to the image (csrc/inception.cu), shared by tests/test_gpu_damsm.py (which
-runs every row against a float64 restatement) and tests/test_damsm_census.py (which checks that the networks issue no
+runs every row against a float64 restatement) and tests/test_census.py (which checks that the networks issue no
 shape missing here).
 
 One table of rows per C entry point:
@@ -127,14 +127,11 @@ def _key(entry, row):
     return tuple(row)
 
 
-def damsm_needs(fn):
-    """Runs ``fn()`` (which must issue its library calls under lib.DRY_RUN) and returns the set of (entry, key) pairs
-    its DAMSM and encoder-gather calls need, keys as ``_key`` gives them for a row."""
-    from objgan_b200 import ops
+def damsm_needs(work):
+    """The set of (entry, key) pairs the DAMSM and encoder-gather calls of a recorded workload (tests/dry.py) need,
+    keys as ``_key`` gives them for a row."""
     needs = set()
-    real = ops._call
-
-    def rec(name, *a):
+    for name, a in work.calls:
         if name == WP_FWD:           # words, ctx, lens, B, NC, ndf, T, S, gamma1, gamma2, eps, wc, attn, sim
             needs.add((name, tuple(a[3:8])))
         elif name == WP_BWD:         # words, ctx, lens, wc, attn, g_sim, B, NC, ndf, T, S, gamma1, gamma2, eps, g_ctx
@@ -153,12 +150,6 @@ def damsm_needs(fn):
             needs.add((name, tuple(a[1:4])))
         elif name == RELU_SLICE:     # y, ldy, yoff, g, ldg, goff, out, ldo, ooff, nch, P, relu
             needs.add((name, tuple(a[1:3]) + tuple(a[4:6]) + tuple(a[7:12])))
-        return real(name, *a)
-    ops._call = rec
-    try:
-        fn()
-    finally:
-        ops._call = real
     return needs
 
 

@@ -21,7 +21,8 @@ import torch
 
 import reference_fixtures as fixtures
 import refimport
-from objgan_b200 import boxgen, lib, model, ops, synth
+from dry import dry, record  # noqa: F401
+from objgan_b200 import boxgen, model, synth
 from objgan_b200.config import cfg
 from objgan_b200.sampler import GSampler
 from oracle import box_oracle as O
@@ -367,15 +368,6 @@ def test_txt_round_trip_boundaries():
 # ---------------------------------------------------------------------------------------------------------------------
 # module API, layouts, loader
 # ---------------------------------------------------------------------------------------------------------------------
-@pytest.fixture()
-def dry():
-    lib.DRY_RUN = True
-    model.FAST_INIT = True
-    yield
-    lib.DRY_RUN = False
-    model.FAST_INIT = False
-
-
 def box_layouts():
     """{"decoder": [[key, shape]], "encoder": [[key, shape]], sha256s} of the reference's modules."""
     path = os.path.join(fixtures.GOLD, "box_layout.json")
@@ -623,30 +615,19 @@ def test_unsupported_and_input_checks(dry):
     assert out.shape == (2, 4, 256) and h_n.shape == c_n.shape == (2, 2, 128)
 
 
-def _trace(monkeypatch, fn):
-    calls = []
-    real = ops._call
-
-    def rec(name, *args):
-        calls.append(name)
-        return real(name, *args)
-    monkeypatch.setattr(ops, "_call", rec)
-    try:
-        fn()
-    finally:
-        monkeypatch.setattr(ops, "_call", real)
-    return calls
+def _trace(fn):
+    return [name for name, _ in record(fn)]
 
 
 @pytest.mark.parametrize("B,L", [(1, 1), (5, 40)])
-def test_box_stage_call_sequence(dry, monkeypatch, B, L):
+def test_box_stage_call_sequence(dry, B, L):
     """The box stage is five library calls whatever B and the caption length; the derived weights are made once."""
     bg = _gen()
     caps, lens = captions_for([L] * B, L, NTOK, 2)
     nb, nc = bg.draw_noise(B)
-    first = _trace(monkeypatch, lambda: bg.sample(caps, lens, L, nb, nc))
+    first = _trace(lambda: bg.sample(caps, lens, L, nb, nc))
     assert first.count("og_box_label_table") == 1
-    calls = _trace(monkeypatch, lambda: bg.sample(caps, lens, L, nb, nc))
+    calls = _trace(lambda: bg.sample(caps, lens, L, nb, nc))
     assert calls == ["og_gather_rows", "og_conv2d_simt", "og_lstm_bidir_state", "og_box_decode", "og_box_layout"]
     out = bg.sample(caps, lens, L, nb, nc)
     assert [r.shape for r in out["rois"]] == [(B, 10, 6)] * 3 and out["fm_rois"].shape == (B, 10, 6)

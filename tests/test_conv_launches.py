@@ -1,7 +1,7 @@
 """CPU record of every library call the convolutions issue, byte for byte, at every row of tests/conv_cases.py.
 
-The host code runs its real dispatch (lib.DRY_RUN off, so the tensor-core forms are taken as on the device) on CPU
-tensors from torch.empty: ops._call records instead of launching and ops._chk accepts host tensors.  A record holds,
+The host code runs a dry run (lib.DRY_RUN: the GPU's dispatch, and ops._chk accepts host tensors) on CPU tensors from
+torch.empty, with ops._call replaced by a recorder that launches nothing.  A record holds,
 per call, the entry name, every non-pointer argument (floats exactly), each pointer as the order in which its address
 first appeared in the run (0 stays null), and the tap quadruples of og_conv2d_tc / entry quintuples of
 og_conv2d_wgrad_tc read from their host arrays during the call.  Tap order is summation order, so a reordered tap list
@@ -63,9 +63,8 @@ class _Recorder:
 
 def _recorder(setattr):
     """run(fn) -> the record of the library calls fn issues, with the GPU dispatch on CPU tensors."""
-    setattr(lib, "DRY_RUN", False)
+    setattr(lib, "DRY_RUN", True)
     setattr(model, "FAST_INIT", True)
-    setattr(ops, "_chk", lambda *ts: None)
 
     def run(fn):
         r = _Recorder()

@@ -15,7 +15,8 @@ import torch
 import oracle_eval
 import reference_fixtures as fixtures
 import refimport
-from objgan_b200 import lib, model, ops, synth
+from dry import dry, record  # noqa: F401
+from objgan_b200 import model, synth
 
 CAP = fixtures.CAP
 TRAIN_PASSES = 10
@@ -134,29 +135,11 @@ def test_g_net_forward_eval(B, monkeypatch):
 # ---------------------------------------------------------------------------------------------------
 # library calls (DRY_RUN: no kernels run, the call sequence and argument counts are what is checked)
 # ---------------------------------------------------------------------------------------------------
-@pytest.fixture()
-def dry():
-    lib.DRY_RUN = True
-    model.FAST_INIT = True
-    yield
-    lib.DRY_RUN = False
-    model.FAST_INIT = False
+def _trace(fn):
+    return [(name, len(args)) for name, args in record(fn)]
 
 
-def _trace(monkeypatch, fn):
-    calls = []
-    real = ops._call
-
-    def rec(name, *args):
-        calls.append((name, len(args)))
-        return real(name, *args)
-    monkeypatch.setattr(ops, "_call", rec)
-    fn()
-    monkeypatch.setattr(ops, "_call", real)
-    return calls
-
-
-def test_eval_call_sequence(dry, monkeypatch):
+def test_eval_call_sequence(dry):
     g = model.G_NET(80)
     inp = synth.make_inputs(2, parity=True)
 
@@ -166,10 +149,10 @@ def test_eval_call_sequence(dry, monkeypatch):
               inp["hmaps"], inp["rois"], inp["fm_rois"], inp["num_rois"], inp["bt_masks"], inp["fm_bt_masks"],
               inp["glb_max_num_roi"])
     fwd()                                   # the first pass also packs the weights
-    train = _trace(monkeypatch, fwd)
+    train = _trace(fwd)
     bufs = {k: v.clone() for k, v in g.named_buffers()}
     g.eval()
-    ev = _trace(monkeypatch, fwd)
+    ev = _trace(fwd)
     count = lambda calls, name: sum(1 for n, _ in calls if n == name)
     assert count(train, "og_norm_stats") == 35 and count(ev, "og_norm_stats") == 29
     assert count(train, "og_bn_eval_coef") == 0 and count(ev, "og_bn_eval_coef") == 6
@@ -177,7 +160,7 @@ def test_eval_call_sequence(dry, monkeypatch):
     for k, v in g.named_buffers():
         assert torch.equal(v, bufs[k]), k
     g.train()
-    assert _trace(monkeypatch, fwd) == train
+    assert _trace(fwd) == train
 
 
 def test_eval_backward_wiring(dry):

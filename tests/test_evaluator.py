@@ -15,21 +15,13 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
+from dry import dry, record  # noqa: F401
 from objgan_b200 import evaluator, lib, losses, model, ops, synth, trainer
 from objgan_b200.config import cfg
 from objgan_b200.sampler import GSampler
 
 N_WORDS = 120
 DIMS = 64
-
-
-@pytest.fixture()
-def dry():
-    lib.DRY_RUN = True
-    model.FAST_INIT = True
-    yield
-    lib.DRY_RUN = False
-    model.FAST_INIT = False
 
 
 @pytest.fixture(scope="module")
@@ -177,15 +169,13 @@ def test_batch_call_sequence(mode, dry, eval_cfg, tmp_path, monkeypatch):
     rp, is_, fid = losses.RPrecision(4), losses.InceptionScore(2), losses.FrechetDistance(DIMS)
     e.evaluate_batch(e.data_loader[0], rp, is_, fid)          # first batch: derived weight copies built
     events = []
-    real_call = ops._call
-    monkeypatch.setattr(ops, "_call", lambda name, *a: (events.append(name), real_call(name, *a))[1])
     for cls, meth, tag in ((model.SHP_G_NET, "forward_nhwc", "<shp_g>"), (model.G_NET, "forward", "<g>"),
                            (model.CNN_ENCODER, "forward", "<cnn>"), (model.INCEPTION_V3, "forward", "<inception>"),
                            (model.INCEPTION_V3_FID, "activations", "<inception_fid>")):
         real = getattr(cls, meth)
-        monkeypatch.setattr(cls, meth, (lambda r, t: lambda self, *a, **k: (events.append(t), r(self, *a, **k))[1])(
-            real, tag))
-    e.evaluate_batch(e.data_loader[1], rp, is_, fid)
+        monkeypatch.setattr(cls, meth, (lambda r, t: lambda self, *a, **k: (events.append((t, ())),
+                                                                            r(self, *a, **k))[1])(real, tag))
+    events = [name for name, _ in record(lambda: e.evaluate_batch(e.data_loader[1], rp, is_, fid), events)]
     marks = ["og_gather_rows", "og_form_bbox_maps", "og_gen_hmaps", "og_form_hmaps", "<shp_g>", "<g>", "<cnn>",
              "<inception>", "<inception_fid>"]
     seq = [x for x in events if x in marks]

@@ -29,6 +29,7 @@ import torch
 import torch.nn.functional as F
 
 from conv_cases import CASES, EDGE_CASES, ENC_CASES
+from dry import record
 from objgan_b200 import model, ops, synth, trainer
 from objgan_b200.lib import ACT_LRELU, ACT_SIGMOID, ACT_TANH, PAD_REFLECT, PAD_ZERO, UPSAMPLE2X
 
@@ -102,22 +103,9 @@ def _ref_conv(x, w, b, k, stride, pad, mode):
     return F.conv2d(x, w, b, stride, pad)
 
 
-class _Recorder:
-    """Wraps ops._call: the og_* names issued (and the og_prep_split calls' s2d flags)."""
-
-    def __init__(self, monkeypatch):
-        self.names, self.s2d = set(), []
-        real = ops._call
-
-        def rec(name, *a):
-            self.names.add(name)
-            if name == "og_prep_split":
-                self.s2d.append(a[6])
-            return real(name, *a)
-        monkeypatch.setattr(ops, "_call", rec)
-
-    def convs(self):
-        return {n for n in self.names if n.startswith("og_conv2d")}
+def _convs(calls):
+    """The og_conv2d* names among recorded library calls."""
+    return {n for n, _ in calls if n.startswith("og_conv2d")}
 
 
 def _zero_lo(monkeypatch):
@@ -135,7 +123,7 @@ def _zero_lo(monkeypatch):
 
 
 def _run_conv(row, engine, monkeypatch, seed=0, sinks=False):
-    """Runs the row through model.Conv2dP; returns {quantity: error} and the recorder."""
+    """Runs the row through model.Conv2dP; returns {quantity: error} and the library calls it issued."""
     N, H, W, Cin, Cout, k, stride, pad, mode, act, bias, split, path = row
     monkeypatch.setattr(ops, "CONV_ENGINE", engine)
     torch.manual_seed(seed)
@@ -163,11 +151,16 @@ def _run_conv(row, engine, monkeypatch, seed=0, sinks=False):
             prefill[p_] = torch.linspace(-1, 1, p_.numel(), device=DEV).view(p_.shape)
             p_.og_grad_sink = prefill[p_].clone()
 
-    rec = _Recorder(monkeypatch)
-    for _ in range(2 if sinks else 1):
-        xg = x.clone().requires_grad_(True)
-        y = m(xg)
-        y.backward(gfull)
+    last = []
+
+    def passes():
+        for _ in range(2 if sinks else 1):
+            xg = x.clone().requires_grad_(True)
+            y = m(xg)
+            y.backward(gfull)
+        last.extend((xg, y))
+    calls = record(passes)
+    xg, y = last
     assert y.shape == (N, oh, ow, kp)
     assert (y[..., pad_ch] == pad_value).all(), "padding channels of the output are not act(0)"
     assert (xg.grad[..., Cin:] == 0).all(), "padding channels of the input gradient are not 0"
@@ -190,26 +183,26 @@ def _run_conv(row, engine, monkeypatch, seed=0, sinks=False):
     err["wgrad"] = _per_channel(gw, grads[1], 0)
     if bias:
         err["bgrad"] = (gb.double() - grads[2]).abs().max().item() / grads[2].abs().max().item()
-    return err, rec
+    return err, calls
 
 
-def _check_path(row, engine, rec):
+def _check_path(row, engine, calls):
     """The og_conv2d* names issued are the row's path (f16x3), or the CUDA-core path of the same layer (simt)."""
     N, H, W, Cin, Cout, k, stride, pad, mode, act, bias, split, want = row
     if engine == "simt":
         oh, ow = ops._out_hw(H, W, k, k, stride, pad, mode)
         kp = 2 * ops.cpad(split) if split else ops.cpad(Cout)
         want = "narrow" if kp == 8 and mode == PAD_ZERO and N * oh * ow <= 65536 else "simt"
-    assert rec.convs() == NAMES[want], (rec.convs(), want)
-    if want in ("s1", "s2"):
-        assert rec.s2d[0] == (want == "s2")      # the forward's operand split of x
+    assert _convs(calls) == NAMES[want], (_convs(calls), want)
+    if want in ("s1", "s2"):                     # the forward's operand split of x
+        assert next(a[6] for n, a in calls if n == "og_prep_split") == (want == "s2")
 
 
 @pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("row", CASES + EDGE_CASES, ids=_rid)
 def test_conv(row, engine, monkeypatch):
-    err, rec = _run_conv(row, engine, monkeypatch)
-    _check_path(row, engine, rec)
+    err, calls = _run_conv(row, engine, monkeypatch)
+    _check_path(row, engine, calls)
     worst = max(err.values())
     _note((engine, row[-1]), worst)
     assert worst <= BAR[engine], err
@@ -243,12 +236,11 @@ def _run_enc(row, engine, monkeypatch, seed=0):
     oh, ow = layer.out_hw(H, W)
     cp = ops.cpad(Cin)
     gen = torch.Generator(device=DEV).manual_seed(seed + 1)
-    rec = _Recorder(monkeypatch)
     if d == "fwd":
         x = torch.randn(N, H, W, cp, device=DEV, generator=gen)
         x[..., Cin:] = 0
         y = torch.full((N, oh, ow, Cy), float("nan"), device=DEV)
-        ops.enc_conv_fwd(layer, x, y, yoff)
+        calls = record(lambda: ops.enc_conv_fwd(layer, x, y, yoff))
         outside = torch.ones(Cy, dtype=torch.bool, device=DEV)
         outside[yoff:yoff + Cout] = False
         assert torch.isnan(y[..., outside]).all(), "a channel outside the output slice was written"
@@ -257,21 +249,23 @@ def _run_enc(row, engine, monkeypatch, seed=0):
         err = {"fwd": _per_channel(y[..., yoff:yoff + Cout].permute(0, 3, 1, 2), ref, 1)}
     else:
         gp = torch.randn(N, oh, ow, Cout, device=DEV, generator=gen)
-        gx = ops.enc_conv_dgrad(layer, gp, H, W)
+        out = []
+        calls = record(lambda: out.append(ops.enc_conv_dgrad(layer, gp, H, W)))
+        gx, = out
         assert gx.shape == (N, H, W, cp) and (gx[..., Cin:] == 0).all()
         x64 = torch.zeros(N, Cin, H, W, device=DEV, dtype=torch.float64, requires_grad=True)
         z = F.conv2d(x64, w64, None, stride, (padh, padw))
         ref, = torch.autograd.grad(z, x64, gp.permute(0, 3, 1, 2).double())
         err = {"dgrad": _per_channel(gx[..., :Cin].permute(0, 3, 1, 2), ref, 1)}
-    return err, rec
+    return err, calls
 
 
 @pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("row", ENC_CASES, ids=_rid)
 def test_enc_conv(row, engine, monkeypatch):
-    err, rec = _run_enc(row, engine, monkeypatch)
+    err, calls = _run_enc(row, engine, monkeypatch)
     want = "og_conv2d_tc" if engine == "f16x3" and row[-1] == "tc" else "og_conv2d_simt"
-    assert rec.convs() == {want}
+    assert _convs(calls) == {want}
     worst = max(err.values())
     _note((engine, "enc_" + row[-1]), worst)
     assert worst <= BAR[engine], err
@@ -312,8 +306,8 @@ def test_gradient_sink(row, engine, monkeypatch):
     """``param.og_grad_sink`` set on the weight and the bias: two backward passes accumulate into it (og_unpack_wgrad /
     og_unpack_upsample_wgrad / og_channel_sum with accumulate=1) and hand autograd no gradient."""
     assert row in CASES + EDGE_CASES
-    err, rec = _run_conv(row, engine, monkeypatch, sinks=True)
-    _check_path(row, engine, rec)
+    err, calls = _run_conv(row, engine, monkeypatch, sinks=True)
+    _check_path(row, engine, calls)
     assert max(err.values()) <= BAR[engine], err
 
 

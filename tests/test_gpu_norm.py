@@ -1,5 +1,5 @@
 """The normalisation kernels (csrc/norm.cu) against a float64 restatement of their math, at every shape the networks
-run them (tests/norm_cases.py: CASES) and at rows that pin each code path (EDGE_CASES, SPLIT_CASES).
+run them (tests/norm_cases.py: CASES, SPLIT_CASES) and at rows that pin each code path (EDGE_CASES, SPLIT_EDGE_CASES).
 
 The reference is computed on the device in float64 from the same fp32 inputs the kernels get: two-pass biased variance,
 eps 1e-5 inside the square root, running statistics with momentum 0.1 and the unbiased variance.  It is NOT the CPU
@@ -29,7 +29,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from norm_cases import CASES, EDGE_CASES, SPLIT_CASES
+from norm_cases import CASES, EDGE_CASES, SPLIT_CASES, SPLIT_EDGE_CASES
 from objgan_b200 import ops
 from objgan_b200.lib import NA_GLU, NA_LRELU, NA_NONE
 
@@ -314,7 +314,7 @@ def _split_run(instance, N, H, W, Cy, act, residual, pad, y=None, gamma=None, be
     return out_apply, out, xh, xl, bound
 
 
-@pytest.mark.parametrize("case", SPLIT_CASES, ids=lambda c: "-".join(map(str, c)))
+@pytest.mark.parametrize("case", SPLIT_CASES + SPLIT_EDGE_CASES, ids=lambda c: "-".join(map(str, c)))
 def test_norm_apply_split(case):
     instance, N, H, W, Cy, act, residual, pad = case
     out_apply, out, xh, xl, bound = _split_run(*case)

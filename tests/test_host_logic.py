@@ -1,20 +1,12 @@
-"""CPU tests of the host-side logic (no kernels run: lib.DRY_RUN skips the launches, outputs are
-uninitialised).  Checks shapes, autograd wiring, flat-bucket plumbing and state_dict compatibility."""
-import pytest
+"""CPU tests of the host-side logic in a dry run (tests/dry.py: the host code takes the GPU's dispatch on CPU tensors,
+every library call is checked against the header and counted instead of launched, outputs are uninitialised).  Checks
+shapes, autograd wiring, flat-bucket plumbing and state_dict compatibility."""
 import torch
 
 import refimport
+from dry import dry  # noqa: F401
 from objgan_b200 import lib, model, synth, trainer
 from objgan_b200.config import cfg
-
-
-@pytest.fixture()
-def dry():
-    lib.DRY_RUN = True
-    model.FAST_INIT = True        # DRY_RUN never looks at values: skip the QR-based orthogonal initialisation
-    yield
-    lib.DRY_RUN = False
-    model.FAST_INIT = False
 
 
 def test_step_a_wiring(dry):

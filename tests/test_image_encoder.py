@@ -16,6 +16,7 @@ import torch
 
 import reference_fixtures as fixtures
 import refimport
+from dry import dry  # noqa: F401
 from objgan_b200 import lib, losses, model
 from oracle import image_encoder_oracle as E
 
@@ -133,7 +134,7 @@ def test_guards():
         net(x)
 
 
-def test_dry_run_call_sequence():
+def test_dry_run_call_sequence(dry):
     """One forward issues a fixed list of library calls and no torch compute; with the input requiring grad the
     backward adds the input-gradient calls."""
     net = model.CNN_ENCODER(256)
@@ -142,25 +143,21 @@ def test_dry_run_call_sequence():
     # 94 BasicConv2d + emb_features, with 11 groups of sibling 1x1 convs fused (3 x 3 + 4 x 3 + 2 + 2 x 3 -> 11)
     assert sum(len(st[1].weights) for st in convs) == 95
     assert len(convs) == 95 - (3 * 2 + 4 * 2 + 1 + 2 * 2)
-    lib.DRY_RUN = True
-    try:
-        first = lib.get().launches
-        net(torch.zeros(2, 3, 256, 256))                     # folds BatchNorm and packs the weights
-        first = lib.get().launches - first
-        n0 = lib.get().launches
-        with mock.patch("torch.nn.functional.conv2d", side_effect=AssertionError("torch compute")):
-            f, code = net(torch.zeros(2, 3, 256, 256))
-        fwd = lib.get().launches - n0
-        assert first - fwd >= 94                             # one og_bn_fold per BasicConv2d, once
-        assert f.shape == (2, 256, 17, 17) and code.shape == (2, 256)
-        x = torch.zeros(2, 3, 256, 256, requires_grad=True)
-        n0 = lib.get().launches
-        f, code = net(x)
-        (f.sum() + code.sum()).backward()
-        assert x.grad.shape == x.shape
-        assert lib.get().launches - n0 > 2 * fwd          # the input gradient costs more calls than the forward
-    finally:
-        lib.DRY_RUN = False
+    first = lib.get().launches
+    net(torch.zeros(2, 3, 256, 256))                     # folds BatchNorm and packs the weights
+    first = lib.get().launches - first
+    n0 = lib.get().launches
+    with mock.patch("torch.nn.functional.conv2d", side_effect=AssertionError("torch compute")):
+        f, code = net(torch.zeros(2, 3, 256, 256))
+    fwd = lib.get().launches - n0
+    assert first - fwd >= 94                             # one og_bn_fold per BasicConv2d, once
+    assert f.shape == (2, 256, 17, 17) and code.shape == (2, 256)
+    x = torch.zeros(2, 3, 256, 256, requires_grad=True)
+    n0 = lib.get().launches
+    f, code = net(x)
+    (f.sum() + code.sum()).backward()
+    assert x.grad.shape == x.shape
+    assert lib.get().launches - n0 > 2 * fwd          # the input gradient costs more calls than the forward
 
 
 class _RecordingRP(losses.RPrecision):

@@ -19,7 +19,8 @@ import torch
 import inception_oracle as I
 import reference_fixtures as fixtures
 import refimport
-from objgan_b200 import lib, losses, model, ops
+from dry import dry, record  # noqa: F401
+from objgan_b200 import losses, model, ops
 
 LAYOUT = os.path.join(fixtures.GOLD, "inception_layout.json")
 ENCODER_CALLS = os.path.join(os.path.dirname(fixtures.GOLD), "cnn_encoder_calls.json")
@@ -179,62 +180,50 @@ def test_cpu_input_raises_before_any_launch():
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# library calls (DRY_RUN)
+# library calls (dry run)
 # ---------------------------------------------------------------------------------------------------------------------
 def _record_calls(fn):
-    log = []
-    orig = ops._call
-
-    def rec(name, *args):
-        log.append([name] + [a for a in args if isinstance(a, int) and abs(a) < 2 ** 20])
-        return orig(name, *args)
-
-    with mock.patch.object(ops, "_call", rec):
-        fn()
-    return log
+    """The library calls of fn() with their small integer arguments (sizes and flags, not addresses)."""
+    return [[name] + [a for a in args if isinstance(a, int) and abs(a) < 2 ** 20] for name, args in record(fn)]
 
 
-def test_dry_run_library_calls():
+def test_dry_run_library_calls(dry):
     """The forwards issue library calls only; the FID program stops at its last block; CNN_ENCODER's forward and
     input-gradient calls are the ones recorded before the trunk builder was shared."""
-    lib.DRY_RUN = True
+    torch.manual_seed(0)
+    enc = model.CNN_ENCODER(256)
+    enc(torch.zeros(2, 3, 256, 256))                      # folds BatchNorm and packs the weights
+
+    def enc_fwd_bwd():
+        enc(torch.zeros(2, 3, 256, 256))
+        x = torch.zeros(1, 3, 200, 200, requires_grad=True)
+        f, c = enc(x)
+        (f.sum() + c.sum()).backward()
+    assert _record_calls(enc_fwd_bwd) == json.load(open(ENCODER_CALLS))
+
+    forbid = [mock.patch(f, side_effect=AssertionError("torch compute")) for f in
+              ("torch.nn.functional.conv2d", "torch.nn.functional.interpolate", "torch.nn.functional.softmax",
+               "torch.softmax", "torch.nn.functional.linear")]
+    isnet = model.INCEPTION_V3()
+    isnet(torch.zeros(2, 3, 256, 256))
+    for p in forbid:
+        p.start()
     try:
-        torch.manual_seed(0)
-        enc = model.CNN_ENCODER(256)
-        enc(torch.zeros(2, 3, 256, 256))                      # folds BatchNorm and packs the weights
-
-        def enc_fwd_bwd():
-            enc(torch.zeros(2, 3, 256, 256))
-            x = torch.zeros(1, 3, 200, 200, requires_grad=True)
-            f, c = enc(x)
-            (f.sum() + c.sum()).backward()
-        assert _record_calls(enc_fwd_bwd) == json.load(open(ENCODER_CALLS))
-
-        forbid = [mock.patch(f, side_effect=AssertionError("torch compute")) for f in
-                  ("torch.nn.functional.conv2d", "torch.nn.functional.interpolate", "torch.nn.functional.softmax",
-                   "torch.softmax", "torch.nn.functional.linear")]
-        isnet = model.INCEPTION_V3()
-        isnet(torch.zeros(2, 3, 256, 256))
-        for p in forbid:
-            p.start()
-        try:
-            calls = _record_calls(lambda: isnet(torch.zeros(2, 3, 256, 256)))
-            names = [c[0] for c in calls]
-            assert names[0] == "og_inception_input" and names[-1] == "og_softmax_rows"
-            assert "og_bilinear_fwd" not in names and "og_nchw_to_nhwc" not in names
-            convs = {}
-            for dims in (64, 2048):
-                fid = model.INCEPTION_V3_FID([model.INCEPTION_V3_FID.BLOCK_INDEX_BY_DIM[dims]])
-                fid.activations(torch.zeros(2, 3, 256, 256))
-                calls = _record_calls(lambda: fid.activations(torch.zeros(2, 3, 256, 256)))
-                assert calls[0][0] == "og_inception_input" and calls[-1][0] == "og_global_avg_fwd"
-                convs[dims] = sum(1 for c in calls if c[0].startswith("og_conv2d"))
-        finally:
-            for p in forbid:
-                p.stop()
-        assert convs == {64: 3, 2048: 75}, convs
+        calls = _record_calls(lambda: isnet(torch.zeros(2, 3, 256, 256)))
+        names = [c[0] for c in calls]
+        assert names[0] == "og_inception_input" and names[-1] == "og_softmax_rows"
+        assert "og_bilinear_fwd" not in names and "og_nchw_to_nhwc" not in names
+        convs = {}
+        for dims in (64, 2048):
+            fid = model.INCEPTION_V3_FID([model.INCEPTION_V3_FID.BLOCK_INDEX_BY_DIM[dims]])
+            fid.activations(torch.zeros(2, 3, 256, 256))
+            calls = _record_calls(lambda: fid.activations(torch.zeros(2, 3, 256, 256)))
+            assert calls[0][0] == "og_inception_input" and calls[-1][0] == "og_global_avg_fwd"
+            convs[dims] = sum(1 for c in calls if c[0].startswith("og_conv2d"))
     finally:
-        lib.DRY_RUN = False
+        for p in forbid:
+            p.stop()
+    assert convs == {64: 3, 2048: 75}, convs
 
 
 # ---------------------------------------------------------------------------------------------------------------------

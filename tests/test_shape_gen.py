@@ -17,7 +17,8 @@ import torch
 
 import reference_fixtures as fixtures
 import refimport
-from objgan_b200 import lib, model, ops, synth
+from dry import dry, record  # noqa: F401
+from objgan_b200 import model, ops, synth
 from objgan_b200.sampler import GSampler, strip_module_prefix
 from oracle import shape_oracle as S
 
@@ -241,15 +242,6 @@ def test_bbox_maps_hand_worked():
 # ---------------------------------------------------------------------------------------------------------------------
 # module API
 # ---------------------------------------------------------------------------------------------------------------------
-@pytest.fixture()
-def dry():
-    lib.DRY_RUN = True
-    model.FAST_INIT = True
-    yield
-    lib.DRY_RUN = False
-    model.FAST_INIT = False
-
-
 def test_shp_g_net_state_dict_matches_reference(dry):
     ref = shp_layout()
     net = model.SHP_G_NET(80)
@@ -290,25 +282,17 @@ def test_inference_only(dry):
                            torch.tensor([2]))
 
 
-def _trace(monkeypatch, fn):
-    calls = []
-    real = ops._call
-
-    def rec(name, *args):
-        calls.append(name)
-        return real(name, *args)
-    monkeypatch.setattr(ops, "_call", rec)
-    try:
-        fn()
-    finally:
-        monkeypatch.setattr(ops, "_call", real)
-    return calls
+def _trace(fn):
+    return [name for name, _ in record(fn)]
 
 
 @pytest.mark.parametrize("R", [1, 4])
-def test_shape_call_sequence(dry, monkeypatch, R):
+def test_shape_tensor_core_call_sequence(dry, R):
     """The recurrence: the x-part of Gates once per direction for all steps, then per step the h-part of both
-    directions (not at t = 0, where h = 0) and ONE cell launch for both; no concat pass; one crop."""
+    directions (not at t = 0, where h = 0) and ONE cell launch for both; no concat pass; one crop.  Every 3x3 layer
+    takes the tensor cores (ops.conv_path: the smallest, gates_h, has B x 16 x 16 >= TC_MIN_PIXELS output pixels):
+    the split of its input, then one og_conv2d_tc per output phase.  No normalisation feeds a convolution's operand
+    copies directly (no split_pad), so each is og_norm_stats + og_norm_apply."""
     net = model.SHP_G_NET(80)
     B = 2
     maps, fmaps = ops.form_bbox_maps(torch.zeros(B, 10, 6, dtype=torch.float64), torch.zeros(B, 10, 6, dtype=torch.float64),
@@ -317,26 +301,28 @@ def test_shape_call_sequence(dry, monkeypatch, R):
     z = torch.randn(B, R, 320)
     with torch.no_grad():
         net.forward_nhwc(z, maps, fmaps)                  # first pass packs the weights
-        calls = _trace(monkeypatch, lambda: net.forward_nhwc(z, maps, fmaps))
-    conv = "og_conv2d_simt"
-    want = [conv, "og_norm_stats", "og_norm_apply", conv, "og_norm_stats", "og_norm_apply",     # downsample1, 2
-            conv, conv, "og_broadcast_channels"]                                                # gates_x fwd, bwd; z
+        calls = _trace(lambda: net.forward_nhwc(z, maps, fmaps))
+    conv = ["og_prep_split", "og_conv2d_tc"]                # "s1" / "s2": one launch
+    up = ["og_prep_split"] + ["og_conv2d_tc"] * 4           # upsample + conv3x3: one launch per output phase
+    norm = ["og_norm_stats", "og_norm_apply"]
+    want = conv + norm + conv + norm                                            # downsample1, 2 ("s2")
+    want += conv + conv + ["og_broadcast_channels"]                             # gates_x fwd, bwd; z
     for t in range(R):
-        want += ([] if t == 0 else [conv, conv]) + ["og_clstm_cell"]
-    want += [conv, "og_norm_stats", "og_norm_apply", "og_mul_pixels",                          # jointConv, crop
-             conv, "og_norm_stats", "og_norm_apply", conv, "og_norm_stats", "og_norm_apply", conv, "og_add",
-             conv, "og_norm_stats", "og_norm_apply", conv, "og_norm_stats", "og_norm_apply",    # upsample1, 2
-             "og_conv2d_narrow_fwd" if B * R * 4096 <= 65536 else conv]
+        want += ([] if t == 0 else conv + conv) + ["og_clstm_cell"]
+    want += conv + norm + ["og_mul_pixels"]                                     # jointConv, crop
+    want += conv + norm + conv + norm + conv + ["og_add"]                       # the residual block
+    want += up + norm + up + norm                                               # upsample1, 2
+    want += ["og_conv2d_narrow_fwd" if B * R * 4096 <= 65536 else "og_conv2d_simt"]   # the 1x1 head: 8 padded channels
     assert calls == want
 
 
-def test_sampler_generated_shape_path(dry, monkeypatch):
+def test_sampler_generated_shape_path(dry):
     g, shp = model.G_NET(80), model.SHP_G_NET(80)
     s = GSampler(g, shp)
     batch = synth.compact(synth.make_inputs(2, seed=5, parity=True))
     for k in ("bt_masks", "fm_bt_masks"):
         batch.pop(k)
-    calls = _trace(monkeypatch, lambda: s.sample_eager(batch))
+    calls = _trace(lambda: s.sample_eager(batch))
     count = lambda name: sum(1 for c in calls if c == name)
     rmax = batch["glb_max_num_roi"]
     assert count("og_form_bbox_maps") == 1 and count("og_gen_hmaps") == 1 and count("og_clstm_cell") == rmax

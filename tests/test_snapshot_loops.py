@@ -1,4 +1,4 @@
-"""CPU tests of the snapshot PNGs in the two loops, without a GPU (lib.DRY_RUN: no kernel runs, the canvases hold
+"""CPU tests of the snapshot PNGs in the two loops, without a GPU (a dry run: no kernel runs, the canvases hold
 whatever memory they were given): the trainer's epoch-numbered file set in Image/ through train(), on display steps
 only, one og_snapshot_canvas call and one device -> host read per PNG, the writer drained before train() returns, its
 errors surfaced without replacing the loop's own, the warning without a font, and in a gloo world of two only rank 0
@@ -14,6 +14,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 from PIL import ImageFont
 
+from dry import dry, record  # noqa: F401
 from objgan_b200 import evaluator, lib, model, ops, snapshots, synth, trainer
 from objgan_b200.config import cfg
 from objgan_b200.sampler import GSampler
@@ -21,15 +22,6 @@ from objgan_b200.sampler import GSampler
 N_WORDS = 120
 DIMS = 64
 FONT = ImageFont.load_default(size=50)
-
-
-@pytest.fixture()
-def dry():
-    lib.DRY_RUN = True
-    model.FAST_INIT = True
-    yield
-    lib.DRY_RUN = False
-    model.FAST_INIT = False
 
 
 @pytest.fixture(scope="module")
@@ -70,14 +62,10 @@ def _trainer(out, files, font, batches=2):
                                   font=font)
 
 
-def _count(monkeypatch):
-    """Counts og_snapshot_canvas calls, canvas reads and writer closes."""
-    n = dict(canvas=0, read=0, close=0)
-    real_call, real_read, real_close = ops._call, snapshots._to_host, snapshots.PngWriter.close
-
-    def call(name, *a):
-        n["canvas"] += name == "og_snapshot_canvas"
-        return real_call(name, *a)
+def _count(monkeypatch, fn):
+    """Runs ``fn()`` and returns (its result, its og_snapshot_canvas calls, canvas reads and writer closes)."""
+    n = dict(read=0, close=0)
+    real_read, real_close = snapshots._to_host, snapshots.PngWriter.close
 
     def read(t):
         n["read"] += 1
@@ -86,23 +74,23 @@ def _count(monkeypatch):
     def close(self, *a, **k):
         n["close"] += 1
         return real_close(self, *a, **k)
-    monkeypatch.setattr(ops, "_call", call)
     monkeypatch.setattr(snapshots, "_to_host", read)
     monkeypatch.setattr(snapshots.PngWriter, "close", close)
-    return n
+    out = []
+    n["canvas"] = sum(name == "og_snapshot_canvas" for name, _ in record(lambda: out.append(fn())))
+    return out[0], n
 
 
 # ------------------------------------------------------------------------------------------------------ trainer
 def test_trainer_files_on_display_steps(dry, cfg_restore, files, tmp_path, monkeypatch):
     """2 epochs x 2 steps, DISPLAY_INTERVAL 3: one display, at step 3 (epoch 1), five PNGs named by the epoch."""
-    n = _count(monkeypatch)
     t = _trainer(tmp_path, files, FONT)
     displays = []
     real = trainer.condGANTrainer.save_img_results
     monkeypatch.setattr(trainer.condGANTrainer, "save_img_results",
                         lambda self, epoch, w: (displays.append(epoch), real(self, epoch, w))[1])
     with np.errstate(all="ignore"):
-        t.train()
+        _, n = _count(monkeypatch, t.train)
     assert displays == [1]
     assert sorted(os.listdir(tmp_path / "Image")) == sorted(
         ["G_average_1_0.png", "G_average_1_1.png", "bt_G_average_1_0.png", "bt_G_average_1_1.png",
@@ -112,12 +100,11 @@ def test_trainer_files_on_display_steps(dry, cfg_restore, files, tmp_path, monke
 
 
 def test_trainer_without_font_warns_once_and_writes_nothing(dry, cfg_restore, files, tmp_path, monkeypatch):
-    n = _count(monkeypatch)
     t = _trainer(tmp_path, files, None)
     cfg.TRAIN.DISPLAY_INTERVAL = 1
     t.display_interval = 1
     with np.errstate(all="ignore"), pytest.warns(UserWarning, match="attention-map PNGs") as rec:
-        t.train()
+        _, n = _count(monkeypatch, t.train)
     assert len([w for w in rec if "attention-map" in str(w.message)]) == 1
     assert os.listdir(tmp_path / "Image") == [] and n["canvas"] == 0 and n["read"] == 0
     assert t.fixed_noise is None
@@ -160,14 +147,11 @@ def _worker(rank, world, port, files, outdirs, res):
     lib.DRY_RUN = True
     model.FAST_INIT = True
     cfg.DATA_DIR = "/nonexistent"
-    counted = []
-    real = ops._call
-    ops._call = lambda name, *a: (counted.append(name == "og_snapshot_canvas"), real(name, *a))[1]
     torch.manual_seed(300 + rank)
     t = _trainer(outdirs[rank], files, FONT)
     with np.errstate(all="ignore"):
-        t.train()
-    res[rank] = (t.rank, sum(counted), t.fixed_noise is not None)
+        calls = record(t.train)
+    res[rank] = (t.rank, sum(name == "og_snapshot_canvas" for name, _ in calls), t.fixed_noise is not None)
     dist.destroy_process_group()
 
 
@@ -223,8 +207,7 @@ def _evaluate(out, files, mode, options, font, monkeypatch):
 def test_evaluator_snapshot_files(dry, cfg_restore, files, tmp_path, mode, monkeypatch):
     """SNAPSHOT, DISPLAY_INTERVAL 2 over 4 batches: displays at 0 and 2.  G_ / bt_G_ per stage; ShapeG_ in modes 1
     and 2; ShapeD_ in mode 1.  One canvas and one read per PNG, drained before evaluate() returns."""
-    n = _count(monkeypatch)
-    got = _evaluate(tmp_path, files, mode, "SNAPSHOT", FONT, monkeypatch)
+    got, n = _count(monkeypatch, lambda: _evaluate(tmp_path, files, mode, "SNAPSHOT", FONT, monkeypatch))
     want = []
     for it in (0, 2):
         want += ["G_%d_0.png" % it, "G_%d_1.png" % it, "bt_G_%d_0.png" % it, "bt_G_%d_1.png" % it]
@@ -243,7 +226,6 @@ def test_evaluator_shape_files_in_image_mode(dry, cfg_restore, files, tmp_path, 
 
 @pytest.mark.parametrize("mode", [1, 2])
 def test_evaluator_without_font_writes_no_png(dry, cfg_restore, files, tmp_path, mode, monkeypatch):
-    n = _count(monkeypatch)
     with pytest.warns(UserWarning, match="attention-map PNGs"):
-        got = _evaluate(tmp_path, files, mode, "SNAPSHOT", None, monkeypatch)
+        got, n = _count(monkeypatch, lambda: _evaluate(tmp_path, files, mode, "SNAPSHOT", None, monkeypatch))
     assert got == [] and n["canvas"] == 0

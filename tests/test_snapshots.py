@@ -13,6 +13,7 @@ from PIL import Image, ImageFont
 
 import refimport
 import snapshot_cases as C
+from dry import dry  # noqa: F401
 from objgan_b200 import lib, snapshots
 from objgan_b200.config import cfg
 from oracle import snapshot_oracle as O
@@ -137,13 +138,6 @@ def test_pyramid_expand_boundary_rules():
 
 
 # ----------------------------------------------------------------------------- host logic without a GPU
-@pytest.fixture()
-def dry():
-    lib.DRY_RUN = True
-    yield
-    lib.DRY_RUN = False
-
-
 def test_one_call_per_png_and_geometry(dry, monkeypatch):
     monkeypatch.setitem(cfg.TEXT, "WORDS_NUM", 18)
     n0 = lib.get().launches

@@ -17,7 +17,8 @@ import torch
 
 import reference_fixtures as fixtures
 import refimport
-from objgan_b200 import lib, model, ops, synth
+from dry import dry, record  # noqa: F401
+from objgan_b200 import model, ops, synth
 from objgan_b200.config import cfg
 from objgan_b200.sampler import GSampler, strip_module_prefix
 from oracle import text_oracle as T
@@ -126,15 +127,6 @@ def test_rnn_encoder_oracle_is_per_sample():
 # ---------------------------------------------------------------------------------------------------------------------
 # module API
 # ---------------------------------------------------------------------------------------------------------------------
-@pytest.fixture()
-def dry():
-    lib.DRY_RUN = True
-    model.FAST_INIT = True
-    yield
-    lib.DRY_RUN = False
-    model.FAST_INIT = False
-
-
 def test_rnn_encoder_state_dict_matches_reference():
     ref = enc_layout()
     net = model.RNN_ENCODER(NTOK, nhidden=256)
@@ -236,42 +228,31 @@ def test_sampler_caption_input_checks(dry):
         GSampler(model.G_NET(80)).encode_text(good)
 
 
-def _trace(monkeypatch, fn):
-    calls = []
-    real = ops._call
-
-    def rec(name, *args):
-        calls.append(name)
-        return real(name, *args)
-    monkeypatch.setattr(ops, "_call", rec)
-    try:
-        fn()
-    finally:
-        monkeypatch.setattr(ops, "_call", real)
-    return calls
+def _trace(fn):
+    return [name for name, _ in record(fn)]
 
 
 @pytest.mark.parametrize("lens", [[1], [7, 18, 3, 1, 12]])
-def test_text_stage_call_sequence(dry, monkeypatch, lens):
+def test_text_stage_call_sequence(dry, lens):
     """The text stage is four library calls whatever B and max_len: the token lookup, the x-part of the gates of both
     directions for all steps, the recurrence, and the GloVe lookups + mask; the padded weight copies are made once."""
     s = _text_sampler()
     x = caption_batch(len(lens), 4, lens, NTOK, 40)
-    first = _trace(monkeypatch, lambda: s.encode_text(x))
+    first = _trace(lambda: s.encode_text(x))
     assert first.count("og_zero_bytes") == 1 and first.count("og_add") == 2 and first.count("og_pack_weights") == 1
-    calls = _trace(monkeypatch, lambda: s.encode_text(x))
+    calls = _trace(lambda: s.encode_text(x))
     assert calls == ["og_gather_rows", "og_conv2d_simt", "og_lstm_bidir", "og_text_inputs"]
     out = s.encode_text(x)
     n = max(lens)
     assert out["words_embs"].shape == (len(lens), 256, n) and out["sent_emb"].shape == (len(lens), 256)
     assert out["mask"].shape == (len(lens), n) and out["mask"].dtype == torch.bool
     assert out["glove_words_embs"].shape == (len(lens), 50, n)
-    full = _trace(monkeypatch, lambda: s.sample_eager(x))
+    full = _trace(lambda: s.sample_eager(x))
     i = full.index("og_lstm_bidir")                 # the text stage runs inside the same forward, once
     assert full[i - 2:i + 2] == calls and full.count("og_lstm_bidir") == 1 and i < full.index("og_words_proj")
     with torch.no_grad():
         s.text_encoder.rnn.bias_hh_l0.add_(1.0)       # a weight change refreshes the derived copies
-    again = _trace(monkeypatch, lambda: s.encode_text(x))
+    again = _trace(lambda: s.encode_text(x))
     assert again == ["og_zero_bytes", "og_copy_channels", "og_add", "og_add", "og_gather_rows", "og_pack_weights",
                      *calls[1:]]
 

@@ -1,7 +1,7 @@
 """CPU tests of the training loop (trainer.condGANTrainer) and its batch intake (trainer.prepare_reference_batch): the
 caption-length sort, the dtype conversions and the dropped heat maps of the intake; the order of the library calls in
 one step; the reference's snapshot and score files, and resuming; and, in a gloo world of two, that only rank 0 writes
-and that the Inception predictions are gathered once per epoch.  No kernel runs (lib.DRY_RUN)."""
+and that the Inception predictions are gathered once per epoch.  No kernel runs (a dry run)."""
 import os
 import re
 import socket
@@ -11,19 +11,11 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
+from dry import dry, record  # noqa: F401
 from objgan_b200 import lib, model, synth, trainer
 from objgan_b200.config import cfg
 
 N_WORDS = 120
-
-
-@pytest.fixture()
-def dry():
-    lib.DRY_RUN = True
-    model.FAST_INIT = True
-    yield
-    lib.DRY_RUN = False
-    model.FAST_INIT = False
 
 
 @pytest.fixture(scope="module")
@@ -97,21 +89,20 @@ def _trainer(tmp_path, files, batches=2, b=2, seed=20):
 
 def test_step_call_sequence(dry, loop_cfg, tmp_path, monkeypatch):
     """Intake -> heat maps -> text stage -> the complete step -> INCEPTION_V3, in that order, and nothing read back."""
-    from objgan_b200 import ops
     t = _trainer(tmp_path, loop_cfg)
     t.setup()
     data = t.data_loader[0]
     t.train_step(data)                        # first step: the text encoder's derived weight copies are built
     events = []
-    real_call, real_step, real_inc = ops._call, trainer.StepBTrainer.step, model.INCEPTION_V3.forward
-    monkeypatch.setattr(ops, "_call", lambda name, *a: (events.append(name), real_call(name, *a))[1])
+    real_step, real_inc = trainer.StepBTrainer.step, model.INCEPTION_V3.forward
     monkeypatch.setattr(trainer.StepBTrainer, "step",
-                        lambda self, *a, **k: (events.append("<step>"), real_step(self, *a, **k))[1])
+                        lambda self, *a, **k: (events.append(("<step>", ())), real_step(self, *a, **k))[1])
     monkeypatch.setattr(model.INCEPTION_V3, "forward",
-                        lambda self, x: (events.append("<inception>"), real_inc(self, x))[1])
-    reads = []
+                        lambda self, x: (events.append(("<inception>", ())), real_inc(self, x))[1])
+    reads, out = [], []
     monkeypatch.setattr(trainer.condGANTrainer, "host_losses", staticmethod(lambda out: reads.append(1)))
-    out = t.train_step(data)
+    events = [name for name, _ in record(lambda: out.append(t.train_step(data)), events)]
+    out = out[0]
     s, i = events.index("<step>"), events.index("<inception>")
     text = [e for e in events[:s] if e in ("og_gather_rows", "og_conv2d_simt", "og_lstm_bidir", "og_text_inputs")]
     assert text == ["og_gather_rows", "og_conv2d_simt", "og_lstm_bidir", "og_text_inputs"]
