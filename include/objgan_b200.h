@@ -79,10 +79,10 @@ int og_conv2d_narrow_dgrad(const float* g, int N, int H, int W, int C, const flo
                            int KH, int KW, int stride, int pad, cudaStream_t stream);
 int og_conv2d_narrow_wgrad(const float* x, int N, int H, int W, int C, const float* g, float* dw_packed, int OH, int OW,
                            int KH, int KW, int stride, int pad, cudaStream_t stream);
-/* OIHW parameter (state_dict layout, SURVEY 8b) <-> kernel-native matrices.  split/splitp: GLU halves of the
- * output channels are each padded to splitp.  transposed=1 gives the dgrad operand ([tap][co][ci] instead of
- * [tap][ci][co]).  og_pack_weights_f16 writes the same matrices as the fp16 hi/lo operand pair of the tensor-core
- * path, scaled by the power of two derived from *amax (og_amax over the parameter; see og_prep_split). */
+/* OIHW parameter (state_dict layout, SURVEY 8b) <-> kernel-native matrices (csrc/operands.cu).  split/splitp: GLU
+ * halves of the output channels are each padded to splitp.  transposed=1 gives the dgrad operand ([tap][co][ci]
+ * instead of [tap][ci][co]).  og_pack_weights_f16 writes the same matrices as the fp16 hi/lo operand pair of the
+ * tensor-core path, scaled by the power of two derived from *amax (og_amax over the parameter; see og_prep_split). */
 int og_pack_weights(const float* w_oihw, int Co, int Ci, int KH, int KW, int Cip, int Kp, int split, int splitp,
                     int transposed, float* out, cudaStream_t stream);
 int og_pack_weights_f16(const float* w_oihw, int Co, int Ci, int KH, int KW, int Cip, int Kp, int split, int splitp,
@@ -91,9 +91,9 @@ int og_unpack_wgrad(const float* dw_packed, int Co, int Ci, int KH, int KW, int 
                     float* grad_oihw, int accumulate, int transposed, cudaStream_t stream);
 
 /* upBlock (nearest 2x upsample + conv3x3, ref: model.py:43-49) as four 2x2 phase convolutions with pre-summed
- * weights: Wp[16][..] (tap t = ((p*2+q)*2+a)*2+b) from the OIHW parameter as fp16 hi/lo operands (scale word
- * *amax_up = 4 * *amax, the bound of the pre-sums), and the adjoint map for the gradient (accumulate = 1 adds it to
- * grad_oihw, a persistent gradient buffer, like og_unpack_wgrad). */
+ * weights (csrc/operands.cu): Wp[16][..] (tap t = ((p*2+q)*2+a)*2+b) from the OIHW parameter as fp16 hi/lo operands
+ * (scale word *amax_up = 4 * *amax, the bound of the pre-sums), and the adjoint map for the gradient (accumulate = 1
+ * adds it to grad_oihw, a persistent gradient buffer, like og_unpack_wgrad). */
 int og_pack_upsample_weights(const float* w_oihw, int Co, int Ci, int Cip, int Kp, int split, int splitp,
                              int transposed, const unsigned* amax, unsigned* amax_up, void* hi, void* lo,
                              cudaStream_t stream);
@@ -104,9 +104,10 @@ int og_unpack_upsample_wgrad(const float* dwp, int Co, int Ci, int Cip, int Kp, 
  * contractions that dominate the step (HmapResBlock / upBlock / jointConv / discriminator convs: forward, input
  * and weight gradients).  Operands are fp16 hi/lo pairs (22 mantissa bits; "3xFP16": a*b ~ ah*bh + al*bh + ah*bl)
  * of x * 2^k, k = og_scale_exp(max|x|) per tensor; the word *amax holds max|x| as float bits and travels with the
- * operand.  og_prep_split computes *amax and writes the pair for an activation tensor (pad=1 also materialises
- * the nn.ReflectionPad2d(1) halo, ref: model.py:67; s2d=1 writes the four space-to-depth phase blocks used by
- * the stride-2 convs of the discriminators and by the adjoint of the 2x upsampling); og_conv2d_tc computes
+ * operand (the format: csrc/operand.cuh).  og_prep_split (csrc/operands.cu) computes *amax and writes the pair for
+ * an activation tensor (pad=1 also materialises the nn.ReflectionPad2d(1) halo, ref: model.py:67; s2d=1 writes the
+ * four space-to-depth phase blocks used by the stride-2 convs of the discriminators and by the adjoint of the 2x
+ * upsampling); og_conv2d_tc computes
  *     y[n, osy*h+opy, osx*w+opx, :] = act(bias + sum_t x[n+dn_t, h+dh_t, w+dw_t, :] * W[widx_t])   (x OOB = 0)
  * with taps = ntaps host quadruples (dh, dw, dn, widx), as the error-compensated product (fp32-level accuracy).
  * Every entry point that takes a hi / lo pair returns cudaErrorInvalidValue if either pointer is null. */
@@ -275,7 +276,7 @@ int og_form_clabels_feat(const float* emb, const long long* cls, const long long
                          int ncls, float* out, cudaStream_t stream);
 
 /* Whole-network weight re-packing after an optimiser step: og_amax + og_pack_weights_f16 for EVERY registered
- * (weight, layout) of a network in one launch each, from a device-resident int64 job table.
+ * (weight, layout) of a network in one launch each, from a device-resident int64 job table (csrc/operands.cu).
  *  amax job (4 fields): x, n, out word, first block index;  a block covers 4096 elements
  *  pack job (14 fields): w (OIHW), hi, lo (or 0), amax word, Co, Ci, taps, Cip, Kp, split, splitp, transposed, total,
  *                        first block index */
@@ -381,9 +382,9 @@ int og_zero_bytes(float* p, long long bytes, cudaStream_t stream);
  * gradient slice the same way), avg_pool2d(3, 1, 1, count_include_pad=True), the global average over P pixels; every
  * backward is a deterministic gather.  og_bilinear_bwd_gather: adjoint of og_bilinear_fwd without atomics.
  * og_bn_fold: eval BatchNorm folded into a bias-free conv (wout = w * s, bout = beta - mean * s, s = gamma /
- * sqrt(var + eps), R = Ci * KH * KW).  og_prep_split_s2d: og_prep_split(s2d=1) for any H, W (phase blocks of
- * ceil(H/2) x ceil(W/2), zero past an odd edge).  og_relu_grad_slice: out[p, ooff + c] = g[p, goff + c] masked by
- * y[p, yoff + c] > 0 (relu = 1) or copied (relu = 0), c < nch.
+ * sqrt(var + eps), R = Ci * KH * KW).  og_prep_split_s2d (csrc/operands.cu): og_prep_split(s2d=1) for any H, W
+ * (phase blocks of ceil(H/2) x ceil(W/2), zero past an odd edge).  og_relu_grad_slice: out[p, ooff + c] =
+ * g[p, goff + c] masked by y[p, yoff + c] > 0 (relu = 1) or copied (relu = 0), c < nch.
  * ---------------------------------------------------------------------------------------------------- */
 int og_maxpool3s2_fwd(const float* x, int N, int H, int W, int C, float* y, int ldy, int yoff, cudaStream_t stream);
 int og_maxpool3s2_bwd(const float* x, const float* g, int ldg, int goff, int N, int H, int W, int C, float* gx,

@@ -30,6 +30,12 @@ static inline int og_num_sms() {
   return sms > 0 ? sms : 1;
 }
 
+// blocks of 256 threads for a grid-stride walk over total items: one per 256 items, at least one, at most per_sm per SM
+static inline int og_grid(long long total, int per_sm = 32) {
+  const long long b = (total + 255) / 256, cap = (long long)og_num_sms() * per_sm;
+  return (int)(b < 1 ? 1 : (b > cap ? cap : b));
+}
+
 // Stream-ordered scratch memory (also valid inside CUDA graph capture).  The device's default pool keeps what is
 // freed for the next call instead of returning it to the driver at every synchronisation.
 static inline cudaError_t og_work_alloc(float** p, size_t elems, cudaStream_t stream) {

@@ -12,7 +12,6 @@
 // with the addressing mode (zero pad / reflection pad / nearest-2x-upsample-then-zero-pad /
 // transposed); B is a pre-packed [(kh,kw,ci)][co] matrix (og_pack_weights).
 #include "common.cuh"
-#include <cuda_fp16.h>
 
 struct ConvArgs {
   const float* x;  // source NHWC
@@ -321,79 +320,6 @@ __global__ void __launch_bounds__(256) conv_wgrad_kernel(WgradArgs a) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// weight (re)packing between the reference's OIHW parameter layout (state_dict shapes, SURVEY 8b)
-// and the kernel-native K-major matrices.
-//   co_map(co) = co < split ? co : co + (splitp - split)   (GLU halves each padded to splitp)
-// ---------------------------------------------------------------------------------------------
-// output-major: one thread per element of the packed matrix (coalesced writes, zero padding written in place; the
-// strided OIHW reads hit the same 32-byte sectors for neighbouring taps and stay in L1/L2)
-// F16 = true: fp16 hi/lo operands of the tensor-core path, scaled by the power of two derived from *amax
-__device__ __forceinline__ void store_hilo_f16(float v, float scale, __half* hi, __half* lo, long long o) {
-  v *= scale;
-  const __half h = __float2half_rn(v);
-  hi[o] = h;
-  lo[o] = __float2half_rn(v - __half2float(h));
-}
-
-template <bool F16>
-__global__ void pack_weights_kernel(const float* __restrict__ w, int Co, int Ci, int KH, int KW, int Cip, int Kp,
-                                    int split, int splitp, int transposed, void* __restrict__ out_v,
-                                    void* __restrict__ out_lo_v, const unsigned* __restrict__ amax) {
-  float* out = (float*)out_v;
-  float scale = 1.f;
-  if (F16) scale = og_exp2i(og_scale_exp(__ldg(amax)));
-  const long long total = (long long)KH * KW * Cip * Kp;
-  const int taps = KH * KW;
-  for (long long o = blockIdx.x * (long long)blockDim.x + threadIdx.x; o < total;
-       o += (long long)gridDim.x * blockDim.x) {
-    int cm, ci, tap;
-    if (!transposed) {            // [(tap, ci)][cm]
-      cm = (int)(o % Kp);
-      long long t = o / Kp;
-      ci = (int)(t % Cip);
-      tap = (int)(t / Cip);
-    } else {                      // [(tap, cm)][ci]
-      ci = (int)(o % Cip);
-      long long t = o / Cip;
-      cm = (int)(t % Kp);
-      tap = (int)(t / Kp);
-    }
-    // inverse of the GLU-half padding map: cm -> co (or a padding lane)
-    int co;
-    if (split > 0) {
-      if (cm < split) co = cm;
-      else if (cm >= splitp && cm < splitp + split) co = cm - (splitp - split);
-      else co = -1;
-    } else {
-      co = cm < Co ? cm : -1;
-    }
-    float v = 0.f;
-    if (co >= 0 && co < Co && ci < Ci) v = __ldg(w + ((long long)co * Ci + ci) * taps + tap);
-    if (F16) store_hilo_f16(v, scale, (__half*)out_v, (__half*)out_lo_v, o);
-    else out[o] = v;
-  }
-}
-
-__global__ void unpack_wgrad_kernel(const float* __restrict__ dw, int Co, int Ci, int KH, int KW, int Cip, int Kp,
-                                    int split, int splitp, float* __restrict__ grad, int accumulate,
-                                    int transposed) {
-  long long total = (long long)Co * Ci * KH * KW;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    int kw = (int)(i % KW);
-    long long t = i / KW;
-    int kh = (int)(t % KH);
-    t /= KH;
-    int ci = (int)(t % Ci);
-    int co = (int)(t / Ci);
-    int cm = (split > 0 && co >= split) ? co + (splitp - split) : co;
-    float v = transposed ? dw[((long long)(kh * KW + kw) * Kp + cm) * Cip + ci]
-                         : dw[((long long)(kh * KW + kw) * Cip + ci) * Kp + cm];
-    grad[i] = accumulate ? grad[i] + v : v;
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
 // "narrow" convolutions: at most 8 output channels and a long reduction (the k4 s2 p0 logit heads of
 // D_GET_LOGITS, model.py:1031-1033: 768 -> 1 on 16x16 / 8x8 / 4x4 maps).  A GEMM tile is the wrong shape for
 // them (7 CTAs, 1536 k-steps each); these are dot products: one warp per output pixel in the forward,
@@ -678,38 +604,6 @@ OG_API int og_conv2d_wgrad_simt(const float* x, int N, int H, int W, int C, long
   return rc;
 }
 
-OG_API int og_pack_weights(const float* w_oihw, int Co, int Ci, int KH, int KW, int Cip, int Kp, int split,
-                           int splitp, int transposed, float* out, cudaStream_t stream) {
-  long long total = (long long)KH * KW * Cip * Kp;
-  int blocks = (int)((total + 255) / 256);
-  if (blocks > og_num_sms() * 16) blocks = og_num_sms() * 16;
-  pack_weights_kernel<false><<<blocks, 256, 0, stream>>>(w_oihw, Co, Ci, KH, KW, Cip, Kp, split, splitp, transposed,
-                                                         out, nullptr, nullptr);
-  OG_RETURN_LAST_ERROR();
-}
-// fp16 hi/lo operands for og_conv2d_tc: same matrices, scaled by 2^og_scale_exp(*amax) (amax from og_amax over w)
-OG_API int og_pack_weights_f16(const float* w_oihw, int Co, int Ci, int KH, int KW, int Cip, int Kp, int split,
-                               int splitp, int transposed, const unsigned* amax, void* hi, void* lo,
-                               cudaStream_t stream) {
-  if (!hi || !lo) return (int)cudaErrorInvalidValue;
-  long long total = (long long)KH * KW * Cip * Kp;
-  int blocks = (int)((total + 255) / 256);
-  if (blocks > og_num_sms() * 16) blocks = og_num_sms() * 16;
-  pack_weights_kernel<true><<<blocks, 256, 0, stream>>>(w_oihw, Co, Ci, KH, KW, Cip, Kp, split, splitp, transposed,
-                                                        hi, lo, amax);
-  OG_RETURN_LAST_ERROR();
-}
-
-OG_API int og_unpack_wgrad(const float* dw_packed, int Co, int Ci, int KH, int KW, int Cip, int Kp, int split,
-                           int splitp, float* grad_oihw, int accumulate, int transposed, cudaStream_t stream) {
-  long long total = (long long)Co * Ci * KH * KW;
-  int blocks = (int)((total + 255) / 256);
-  if (blocks > og_num_sms() * 16) blocks = og_num_sms() * 16;
-  unpack_wgrad_kernel<<<blocks, 256, 0, stream>>>(dw_packed, Co, Ci, KH, KW, Cip, Kp, split, splitp, grad_oihw,
-                                                  accumulate, transposed);
-  OG_RETURN_LAST_ERROR();
-}
-
 // contiguous NHWC tensors, zero padding, output channels padded to exactly 8; wpacked = [(kh,kw,ci)][8]
 OG_API int og_conv2d_narrow_fwd(const float* x, int N, int H, int W, int C, const float* wpacked, float* y, int OH,
                                 int OW, int KH, int KW, int stride, int pad, const float* bias, int act, float slope,
@@ -758,184 +652,4 @@ OG_API int og_conv2d_narrow_wgrad(const float* x, int N, int H, int W, int C, co
     if (!rc) rc = (int)e;
   }
   return rc;
-}
-
-// ---------------------------------------------------------------------------------------------
-// nearest-2x-upsample + conv3x3 as four 2x2 "phase" convolutions on the low-resolution tensor (upBlock,
-// model.py:43-49).  Output pixel (2i+p, 2j+q) reads low-res rows i + {-1,0} (p = 0) or i + {0,+1} (p = 1), and the
-// three kernel rows collapse onto those two offsets, so the weights can be pre-summed:
-//     Wp[p][q][a][b] = sum_{kh in Sh(p,a)} sum_{kw in Sw(q,b)} W[kh][kw]      (2.25x fewer MACs, same result up to
-// fp32 rounding of the pre-sums).  Tap index t = ((p*2+q)*2+a)*2+b.  up_row(p, k) = which of the two offsets
-// kernel row k falls on: p = 0: {0,1,1}, p = 1: {0,0,1}.
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ int up_row(int p, int k) { return p == 0 ? (k >= 1) : (k >= 2); }
-
-// amax_up receives 4 * amax(w): the pre-sums of up to four taps are bounded by it, and it is the scale word the conv
-// kernel is given for this operand
-__global__ void pack_upsample_weights_kernel(const float* __restrict__ w, int Co, int Ci, int Cip, int Kp, int split,
-                                             int splitp, int transposed, const unsigned* __restrict__ amax,
-                                             unsigned* __restrict__ amax_up, __half* __restrict__ out,
-                                             __half* __restrict__ out_lo) {
-  long long total = (long long)16 * Co * Ci;
-  const float bound = 4.f * __uint_as_float(__ldg(amax));
-  const float scale = og_exp2i(og_scale_exp(__float_as_uint(bound)));
-  if (blockIdx.x == 0 && threadIdx.x == 0) *amax_up = __float_as_uint(bound);
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    int ci = (int)(i % Ci);
-    long long t2 = i / Ci;
-    int co = (int)(t2 % Co);
-    int t = (int)(t2 / Co);
-    int b = t & 1, a = (t >> 1) & 1, q = (t >> 2) & 1, p = (t >> 3) & 1;
-    float v = 0.f;
-    for (int kh = 0; kh < 3; ++kh) {
-      if (up_row(p, kh) != a) continue;
-      for (int kw = 0; kw < 3; ++kw)
-        if (up_row(q, kw) == b) v += w[(((long long)co * Ci + ci) * 3 + kh) * 3 + kw];
-    }
-    int cm = (split > 0 && co >= split) ? co + (splitp - split) : co;
-    long long o = transposed ? ((long long)t * Kp + cm) * Cip + ci : ((long long)t * Cip + ci) * Kp + cm;
-    store_hilo_f16(v, scale, out, out_lo, o);
-  }
-}
-// dW[kh][kw] = sum_{p,q} dWp[p][q][up_row(p,kh)][up_row(q,kw)]   (dWp packed [16][Kp][Cip], i.e. "transposed" layout)
-__global__ void unpack_upsample_wgrad_kernel(const float* __restrict__ dwp, int Co, int Ci, int Cip, int Kp, int split,
-                                             int splitp, float* __restrict__ grad, int accumulate) {
-  long long total = (long long)Co * Ci * 9;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    int kw = (int)(i % 3);
-    long long t2 = i / 3;
-    int kh = (int)(t2 % 3);
-    t2 /= 3;
-    int ci = (int)(t2 % Ci);
-    int co = (int)(t2 / Ci);
-    int cm = (split > 0 && co >= split) ? co + (splitp - split) : co;
-    float v = 0.f;
-    for (int p = 0; p < 2; ++p)
-      for (int q = 0; q < 2; ++q) {
-        int t = ((p * 2 + q) * 2 + up_row(p, kh)) * 2 + up_row(q, kw);
-        v += dwp[((long long)t * Kp + cm) * Cip + ci];
-      }
-    grad[i] = accumulate ? grad[i] + v : v;
-  }
-}
-OG_API int og_pack_upsample_weights(const float* w_oihw, int Co, int Ci, int Cip, int Kp, int split, int splitp,
-                                    int transposed, const unsigned* amax, unsigned* amax_up, void* hi, void* lo,
-                                    cudaStream_t stream) {
-  if (!hi || !lo) return (int)cudaErrorInvalidValue;
-  long long n = (long long)16 * Cip * Kp;
-  OG_CHECK(cudaMemsetAsync(hi, 0, sizeof(__half) * n, stream));
-  OG_CHECK(cudaMemsetAsync(lo, 0, sizeof(__half) * n, stream));
-  long long total = (long long)16 * Co * Ci;
-  int blocks = (int)((total + 255) / 256);
-  if (blocks > og_num_sms() * 16) blocks = og_num_sms() * 16;
-  pack_upsample_weights_kernel<<<blocks, 256, 0, stream>>>(w_oihw, Co, Ci, Cip, Kp, split, splitp, transposed, amax,
-                                                           amax_up, (__half*)hi, (__half*)lo);
-  OG_RETURN_LAST_ERROR();
-}
-OG_API int og_unpack_upsample_wgrad(const float* dwp, int Co, int Ci, int Cip, int Kp, int split, int splitp,
-                                    float* grad_oihw, int accumulate, cudaStream_t stream) {
-  long long total = (long long)Co * Ci * 9;
-  int blocks = (int)((total + 255) / 256);
-  if (blocks > og_num_sms() * 16) blocks = og_num_sms() * 16;
-  unpack_upsample_wgrad_kernel<<<blocks, 256, 0, stream>>>(dwp, Co, Ci, Cip, Kp, split, splitp, grad_oihw, accumulate);
-  OG_RETURN_LAST_ERROR();
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Multi-tensor weight re-packing: after an optimiser step EVERY convolution weight of a network needs its max|w| and
-// its fp16 hi/lo operand matrices again (og_amax + og_pack_weights_f16 per layer and layout: ~300 tiny launches per
-// training step).  These two kernels do the whole network in one launch each from a device-resident job table
-// (int64 fields), a block being assigned to (job, chunk) by its index.
-//   amax job : [x, n, out, block_start]                                  (blocks of 256 threads x 16 floats)
-//   pack job : [w, hi, lo, amax, Co, Ci, taps, Cip, Kp, split, splitp, transposed, total, block_start]
-// ---------------------------------------------------------------------------------------------------------------
-namespace {
-constexpr int MJ_AMAX_FIELDS = 4, MJ_PACK_FIELDS = 14, MJ_CHUNK = 4096;
-
-__device__ __forceinline__ int mj_find(const long long* __restrict__ jobs, int njobs, int fields, int start_field,
-                                       long long blk) {
-  int lo = 0, hi = njobs - 1;
-  while (lo < hi) {                       // last job whose block_start <= blk
-    const int mid = (lo + hi + 1) >> 1;
-    if (jobs[(long long)mid * fields + start_field] <= blk) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
-__global__ void __launch_bounds__(256) amax_multi_kernel(const long long* __restrict__ jobs, int njobs) {
-  const int j = mj_find(jobs, njobs, MJ_AMAX_FIELDS, 3, blockIdx.x);
-  const long long* f = jobs + (long long)j * MJ_AMAX_FIELDS;
-  const float* x = reinterpret_cast<const float*>(f[0]);
-  const long long n = f[1];
-  unsigned* out = reinterpret_cast<unsigned*>(f[2]);
-  const long long base = ((long long)blockIdx.x - f[3]) * MJ_CHUNK;
-  float m = 0.f;
-  for (long long i = base + threadIdx.x; i < n && i < base + MJ_CHUNK; i += 256) m = fmaxf(m, fabsf(__ldg(x + i)));
-  m = warp_max(m);
-  __shared__ float sm[8];
-  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int k = 1; k < 8; ++k) m = fmaxf(m, sm[k]);
-    atomicMax(out, __float_as_uint(m));
-  }
-}
-__global__ void amax_zero_multi_kernel(const long long* __restrict__ jobs, int njobs) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j < njobs) *reinterpret_cast<unsigned*>(jobs[(long long)j * MJ_AMAX_FIELDS + 2]) = 0u;
-}
-
-__global__ void __launch_bounds__(256) pack_multi_kernel(const long long* __restrict__ jobs, int njobs) {
-  const int j = mj_find(jobs, njobs, MJ_PACK_FIELDS, 13, blockIdx.x);
-  const long long* f = jobs + (long long)j * MJ_PACK_FIELDS;
-  const float* w = reinterpret_cast<const float*>(f[0]);
-  __half* hi = reinterpret_cast<__half*>(f[1]);
-  __half* lo = reinterpret_cast<__half*>(f[2]);
-  const float scale = og_exp2i(og_scale_exp(__ldg(reinterpret_cast<const unsigned*>(f[3]))));
-  const int Co = (int)f[4], Ci = (int)f[5], taps = (int)f[6], Cip = (int)f[7], Kp = (int)f[8];
-  const int split = (int)f[9], splitp = (int)f[10], transposed = (int)f[11];
-  const long long total = f[12];
-  const long long base = ((long long)blockIdx.x - f[13]) * MJ_CHUNK;
-  for (long long o = base + threadIdx.x; o < total && o < base + MJ_CHUNK; o += 256) {
-    int cm, ci, tap;
-    if (!transposed) {            // [(tap, ci)][cm]
-      cm = (int)(o % Kp);
-      const long long t = o / Kp;
-      ci = (int)(t % Cip);
-      tap = (int)(t / Cip);
-    } else {                      // [(tap, cm)][ci]
-      ci = (int)(o % Cip);
-      const long long t = o / Cip;
-      cm = (int)(t % Kp);
-      tap = (int)(t / Kp);
-    }
-    int co;
-    if (split > 0) {
-      if (cm < split) co = cm;
-      else if (cm >= splitp && cm < splitp + split) co = cm - (splitp - split);
-      else co = -1;
-    } else {
-      co = cm < Co ? cm : -1;
-    }
-    float v = 0.f;
-    if (co >= 0 && co < Co && ci < Ci) v = __ldg(w + ((long long)co * Ci + ci) * taps + tap);
-    store_hilo_f16(v, scale, hi, lo, o);
-  }
-}
-}  // namespace
-
-// jobs: device table of njobs x 4 int64 (see above), total_blocks = sum of ceil(n / 4096)
-OG_API int og_amax_multi(const long long* jobs, int njobs, int total_blocks, cudaStream_t stream) {
-  if (njobs <= 0) return 0;
-  amax_zero_multi_kernel<<<og_cdiv(njobs, 128), 128, 0, stream>>>(jobs, njobs);
-  if (total_blocks > 0) amax_multi_kernel<<<total_blocks, 256, 0, stream>>>(jobs, njobs);
-  OG_RETURN_LAST_ERROR();
-}
-// jobs: device table of njobs x 14 int64, total_blocks = sum of ceil(total / 4096)
-OG_API int og_pack_weights_f16_multi(const long long* jobs, int njobs, int total_blocks, cudaStream_t stream) {
-  if (njobs <= 0 || total_blocks <= 0) return 0;
-  pack_multi_kernel<<<total_blocks, 256, 0, stream>>>(jobs, njobs);
-  OG_RETURN_LAST_ERROR();
 }

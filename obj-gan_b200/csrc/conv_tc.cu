@@ -826,104 +826,3 @@ OG_API int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* am
   }
   return rc;
 }
-
-
-// max|x| over a tensor as float bits (non-negative floats order like unsigned integers)
-__global__ void __launch_bounds__(256) amax_kernel(const float* __restrict__ x, long long n4, int tail,
-                                                   unsigned* __restrict__ out) {
-  float m = 0.f;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
-    float4 v = ldg4(x + i * 4);
-    m = fmaxf(fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
-  }
-  if (blockIdx.x == 0 && (int)threadIdx.x < tail) m = fmaxf(m, fabsf(x[n4 * 4 + threadIdx.x]));
-  m = warp_max(m);
-  __shared__ float sm[8];
-  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x < 8) {
-    m = sm[threadIdx.x];
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffu, m, o));
-    if (threadIdx.x == 0) atomicMax(out, __float_as_uint(m));
-  }
-}
-
-__device__ __forceinline__ void split_f16(float v, float scale, __half& hi, __half& lo) {
-  v *= scale;
-  hi = __float2half_rn(v);
-  lo = __float2half_rn(v - __half2float(hi));
-}
-
-__global__ void __launch_bounds__(256) prep_split_kernel(const float* __restrict__ x, int N, int H, int W, int C8, int pad,
-                                                         int s2d, long long total, const unsigned* __restrict__ amax,
-                                                         __half* __restrict__ xh, __half* __restrict__ xl) {
-  // output: [N][H+2p][W+2p][C] or, for s2d, [4][N][H/2][W/2][C] with phase block (a*2+b) = x[:, a::2, b::2]
-  const int Hp = s2d ? H / 2 : H + 2 * pad, Wp = s2d ? W / 2 : W + 2 * pad;
-  const float scale = og_exp2i(og_scale_exp(__ldg(amax)));
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    int c = (int)(i % C8);
-    long long t = i / C8;
-    int w = (int)(t % Wp);
-    t /= Wp;
-    int h = (int)(t % Hp);
-    long long n = t / Hp;
-    int sh, sw;
-    if (s2d) {
-      int ph = (int)(n / N);
-      n -= (long long)ph * N;
-      sh = 2 * h + (ph >> 1);
-      sw = 2 * w + (ph & 1);
-    } else {
-      sh = h - pad;
-      sw = w - pad;
-      if (sh < 0) sh = -sh;
-      if (sh >= H) sh = 2 * H - 2 - sh;
-      if (sw < 0) sw = -sw;
-      if (sw >= W) sw = 2 * W - 2 - sw;
-    }
-    const float* src = x + (((n * H + sh) * W + sw) * C8 + c) * 8;
-    const float4 v0 = ldg4(src), v1 = ldg4(src + 4);
-    const float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-    __align__(16) __half hi[8], lo[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) split_f16(v[j], scale, hi[j], lo[j]);
-    *reinterpret_cast<uint4*>(xh + i * 8) = *reinterpret_cast<const uint4*>(hi);
-    *reinterpret_cast<uint4*>(xl + i * 8) = *reinterpret_cast<const uint4*>(lo);
-  }
-}
-
-// fp16 hi/lo operand copies of an NHWC fp32 tensor, scaled by the power of two that og_scale_exp derives from
-// max|x| (*amax as float bits: computed here, or, with amax_ready, left there by the kernel that produced x --
-// any upper bound of max|x| is valid, it only positions the 22-bit window).  pad = 0: plain; pad = 1: nn.ReflectionPad2d(1) halo (model.py:67)
-// materialised while splitting; s2d = 1: four space-to-depth phase blocks.
-OG_API int og_prep_split(const float* x, int N, int H, int W, int C, int pad, int s2d, unsigned* amax, int amax_ready,
-                         void* xh, void* xl, cudaStream_t stream) {
-  if (!xh || !xl || C % 8 || pad < 0 || pad > 1 || (s2d && (pad || (H & 1) || (W & 1)))) return (int)cudaErrorInvalidValue;
-  const long long n4 = (long long)N * H * W * C / 4;
-  if (!amax_ready) OG_CHECK(cudaMemsetAsync(amax, 0, sizeof(unsigned), stream));
-  if (n4 == 0) return 0;
-  if (!amax_ready) {      // the producer of x did not leave max|x| behind: one extra read pass
-    long long ab = (n4 + 255) / 256;
-    if (ab > (long long)og_num_sms() * 8) ab = (long long)og_num_sms() * 8;
-    amax_kernel<<<(int)ab, 256, 0, stream>>>(x, n4, 0, amax);
-  }
-  long long total = s2d ? (long long)N * H * W * (C / 8) : (long long)N * (H + 2 * pad) * (W + 2 * pad) * (C / 8);
-  long long b = (total + 255) / 256;
-  if (b > (long long)og_num_sms() * 32) b = (long long)og_num_sms() * 32;
-  prep_split_kernel<<<(int)b, 256, 0, stream>>>(x, N, H, W, C / 8, pad, s2d, total, amax, (__half*)xh, (__half*)xl);
-  OG_RETURN_LAST_ERROR();
-}
-
-// *amax = float bits of max|x[0..n)| (x 16-byte aligned); used for the weight tensors before og_pack_weights_f16
-OG_API int og_amax(const float* x, long long n, unsigned* amax, cudaStream_t stream) {
-  OG_CHECK(cudaMemsetAsync(amax, 0, sizeof(unsigned), stream));
-  if (n == 0) return 0;
-  const long long n4 = n / 4;
-  long long ab = (n4 + 255) / 256;
-  if (ab < 1) ab = 1;
-  if (ab > (long long)og_num_sms() * 8) ab = (long long)og_num_sms() * 8;
-  amax_kernel<<<(int)ab, 256, 0, stream>>>(x, n4, (int)(n - n4 * 4), amax);
-  OG_RETURN_LAST_ERROR();
-}

@@ -3,12 +3,6 @@
 // Reference semantics cited per kernel (paths under /root/reference/image_generation/).
 #include "common.cuh"
 
-static int eblocks(long long total, int per = 256) {
-  long long b = (total + per - 1) / per;
-  long long cap = (long long)og_num_sms() * 32;
-  return (int)(b < cap ? (b < 1 ? 1 : b) : cap);
-}
-
 // ---------------------------------------------------------------------------------------------
 // NCHW <-> NHWC(+channel padding).  Public tensors are NCHW fp32 like the reference's; kernels run NHWC.
 // ---------------------------------------------------------------------------------------------
@@ -86,7 +80,7 @@ OG_API int og_act_backward(const float* out, const float* g, long long n, int ac
                            cudaStream_t stream) {
   if (n % 4) return (int)cudaErrorInvalidValue;
   if (n == 0) return 0;
-  act_backward_kernel<<<eblocks(n / 4), 256, 0, stream>>>(out, g, n / 4, act, slope, gin);
+  act_backward_kernel<<<og_grid(n / 4), 256, 0, stream>>>(out, g, n / 4, act, slope, gin);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -160,7 +154,7 @@ OG_API int og_upsample2x_bwd(const float* gu, int N, int H, int W, int C, float*
   if (C % 4) return (int)cudaErrorInvalidValue;
   long long total = (long long)N * H * W * (C / 4);
   if (total == 0) return 0;
-  upsample2x_bwd_kernel<<<eblocks(total), 256, 0, stream>>>(gu, H, W, C / 4, total, gx);
+  upsample2x_bwd_kernel<<<og_grid(total), 256, 0, stream>>>(gu, H, W, C / 4, total, gx);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -188,7 +182,7 @@ OG_API int og_reflect_pad_fwd(const float* x, int N, int H, int W, int C, float*
   if (C % 4) return (int)cudaErrorInvalidValue;
   long long total = (long long)N * (H + 2) * (W + 2) * (C / 4);
   if (total == 0) return 0;
-  reflect_pad_fwd_kernel<<<eblocks(total), 256, 0, stream>>>(x, H, W, C / 4, total, xp);
+  reflect_pad_fwd_kernel<<<og_grid(total), 256, 0, stream>>>(x, H, W, C / 4, total, xp);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -224,7 +218,7 @@ OG_API int og_reflect_pad_bwd(const float* gpad, int N, int H, int W, int C, flo
   if (C % 4) return (int)cudaErrorInvalidValue;
   long long total = (long long)N * H * W * (C / 4);
   if (total == 0) return 0;
-  reflect_pad_bwd_kernel<<<eblocks(total), 256, 0, stream>>>(gpad, H, W, C / 4, total, gx);
+  reflect_pad_bwd_kernel<<<og_grid(total), 256, 0, stream>>>(gpad, H, W, C / 4, total, gx);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -246,7 +240,7 @@ __global__ void copy_channels_kernel(const float* __restrict__ src, int sstride,
 OG_API int og_copy_channels(const float* src, int sstride, int soff, float* dst, int dstride, int doff, int nch,
                             long long P, int accumulate, cudaStream_t stream) {
   if (P * nch == 0) return 0;
-  copy_channels_kernel<<<eblocks(P * nch), 256, 0, stream>>>(src, sstride, soff, dst, dstride, doff, nch, P, accumulate);
+  copy_channels_kernel<<<og_grid(P * nch), 256, 0, stream>>>(src, sstride, soff, dst, dstride, doff, nch, P, accumulate);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -268,7 +262,7 @@ OG_API int og_broadcast_channels_bwd(const float* g, int B, int Cc, int gstride,
                                      float* gc, cudaStream_t stream) {
   long long total = (long long)B * Cc;
   if (total == 0) return 0;
-  broadcast_channels_bwd_kernel<<<eblocks(total), 256, 0, stream>>>(g, Cc, gstride, goff, pix_per_img, total, gc);
+  broadcast_channels_bwd_kernel<<<og_grid(total), 256, 0, stream>>>(g, Cc, gstride, goff, pix_per_img, total, gc);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -295,7 +289,7 @@ __global__ void scatter_rows_add_kernel(const float* __restrict__ g, const long 
 OG_API int og_gather_rows(const float* x, const long long* idx, long long n_out, long long rowlen, float* out,
                           cudaStream_t stream) {
   if (n_out * rowlen == 0) return 0;
-  gather_rows_kernel<<<eblocks(n_out * rowlen), 256, 0, stream>>>(x, idx, n_out, rowlen, out);
+  gather_rows_kernel<<<og_grid(n_out * rowlen), 256, 0, stream>>>(x, idx, n_out, rowlen, out);
   OG_RETURN_LAST_ERROR();
 }
 // gx ([n_in][rowlen]) is zero-filled here, then receives the scattered rows
@@ -303,7 +297,7 @@ OG_API int og_scatter_rows_add(const float* g, const long long* idx, long long n
                                float* gx, cudaStream_t stream) {
   OG_CHECK(cudaMemsetAsync(gx, 0, sizeof(float) * (size_t)(n_in * rowlen), stream));
   if (n_out * rowlen == 0) return 0;
-  scatter_rows_add_kernel<<<eblocks(n_out * rowlen), 256, 0, stream>>>(g, idx, n_out, rowlen, gx);
+  scatter_rows_add_kernel<<<og_grid(n_out * rowlen), 256, 0, stream>>>(g, idx, n_out, rowlen, gx);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -322,7 +316,7 @@ OG_API int og_broadcast_channels(const float* c, int B, int Cc, float* dst, int 
                                  long long pix_per_img, cudaStream_t stream) {
   long long total = (long long)B * pix_per_img * Cc;
   if (total == 0) return 0;
-  broadcast_channels_kernel<<<eblocks(total), 256, 0, stream>>>(c, Cc, dst, dstride, doff, pix_per_img, total);
+  broadcast_channels_kernel<<<og_grid(total), 256, 0, stream>>>(c, Cc, dst, dstride, doff, pix_per_img, total);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -337,7 +331,7 @@ __global__ void add_kernel(const float* __restrict__ a, const float* __restrict_
 OG_API int og_add(const float* a, const float* b, float* out, long long n, cudaStream_t stream) {
   if (n % 4) return (int)cudaErrorInvalidValue;
   if (n == 0) return 0;
-  add_kernel<<<eblocks(n / 4), 256, 0, stream>>>(a, b, out, n / 4);
+  add_kernel<<<og_grid(n / 4), 256, 0, stream>>>(a, b, out, n / 4);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -365,12 +359,12 @@ __global__ void glu_bwd_kernel(const float* __restrict__ x, const float* __restr
 }
 OG_API int og_glu_fwd(const float* x, long long P, int Ch, float* out, cudaStream_t stream) {
   if (P * Ch == 0) return 0;
-  glu_fwd_kernel<<<eblocks(P * Ch), 256, 0, stream>>>(x, Ch, P * Ch, out);
+  glu_fwd_kernel<<<og_grid(P * Ch), 256, 0, stream>>>(x, Ch, P * Ch, out);
   OG_RETURN_LAST_ERROR();
 }
 OG_API int og_glu_bwd(const float* x, const float* g, long long P, int Ch, float* gx, cudaStream_t stream) {
   if (P * Ch == 0) return 0;
-  glu_bwd_kernel<<<eblocks(P * Ch), 256, 0, stream>>>(x, g, Ch, P * Ch, gx);
+  glu_bwd_kernel<<<og_grid(P * Ch), 256, 0, stream>>>(x, g, Ch, P * Ch, gx);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -401,13 +395,13 @@ __global__ void reparam_bwd_kernel(const float* __restrict__ x, int xs, const fl
 }
 OG_API int og_reparam_fwd(const float* x, int xs, const float* eps, int B, int D, float* c, int cs,
                           cudaStream_t stream) {
-  reparam_fwd_kernel<<<eblocks((long long)B * D), 256, 0, stream>>>(x, xs, eps, D, (long long)B * D, c, cs);
+  reparam_fwd_kernel<<<og_grid((long long)B * D), 256, 0, stream>>>(x, xs, eps, D, (long long)B * D, c, cs);
   OG_RETURN_LAST_ERROR();
 }
 // accumulates into gx (caller zero-fills or pre-loads it with the KL gradient)
 OG_API int og_reparam_bwd(const float* x, int xs, const float* eps, const float* gc, int gcs, int B, int D, float* gx,
                           cudaStream_t stream) {
-  reparam_bwd_kernel<<<eblocks((long long)B * D), 256, 0, stream>>>(x, xs, eps, gc, gcs, D, (long long)B * D, gx);
+  reparam_bwd_kernel<<<og_grid((long long)B * D), 256, 0, stream>>>(x, xs, eps, gc, gcs, D, (long long)B * D, gx);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -510,7 +504,7 @@ OG_API int og_adam_ema(float* p, const float* g, float* m, float* v, float* avg,
                        double b2, double eps, int step, const long long* step_dev, float gscale, float decay,
                        cudaStream_t stream) {
   if (n == 0) return 0;
-  adam_ema_kernel<<<eblocks(n), 256, 0, stream>>>(p, g, m, v, avg, n, (float)lr, (float)b1, (float)b2, (float)eps, b1, b2,
+  adam_ema_kernel<<<og_grid(n), 256, 0, stream>>>(p, g, m, v, avg, n, (float)lr, (float)b1, (float)b2, (float)eps, b1, b2,
                                                    step, step_dev, gscale, decay);
   OG_RETURN_LAST_ERROR();
 }
@@ -577,7 +571,7 @@ OG_API int og_bilinear_fwd(const float* x, int N, int IH, int IW, int C, int OH,
   long long total = (long long)N * OH * OW * (C / 4);
   if (total == 0) return 0;
   float rh = OH > 1 ? (float)(IH - 1) / (float)(OH - 1) : 0.f, rw = OW > 1 ? (float)(IW - 1) / (float)(OW - 1) : 0.f;
-  bilinear_fwd_kernel<<<eblocks(total), 256, 0, stream>>>(x, IH, IW, OH, OW, C / 4, rh, rw, total, y);
+  bilinear_fwd_kernel<<<og_grid(total), 256, 0, stream>>>(x, IH, IW, OH, OW, C / 4, rh, rw, total, y);
   OG_RETURN_LAST_ERROR();
 }
 // gx is zero-filled here
@@ -586,7 +580,7 @@ OG_API int og_bilinear_bwd(const float* g, int N, int IH, int IW, int C, int OH,
   long long total = (long long)N * OH * OW * C;
   if (total == 0) return 0;
   float rh = OH > 1 ? (float)(IH - 1) / (float)(OH - 1) : 0.f, rw = OW > 1 ? (float)(IW - 1) / (float)(OW - 1) : 0.f;
-  bilinear_bwd_kernel<<<eblocks(total), 256, 0, stream>>>(g, IH, IW, OH, OW, C, rh, rw, total, gx);
+  bilinear_bwd_kernel<<<og_grid(total), 256, 0, stream>>>(g, IH, IW, OH, OW, C, rh, rw, total, gx);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -703,6 +697,6 @@ __global__ void __launch_bounds__(256) images_to_u8_kernel(const float* __restri
 OG_API int og_images_to_u8(const float* x, int N, int H, int W, unsigned char* out, cudaStream_t stream) {
   const long long total = (long long)N * H * W;
   if (total == 0) return 0;
-  images_to_u8_kernel<<<eblocks(total), 256, 0, stream>>>(x, (long long)H * W, total, out);
+  images_to_u8_kernel<<<og_grid(total), 256, 0, stream>>>(x, (long long)H * W, total, out);
   OG_RETURN_LAST_ERROR();
 }

@@ -5,24 +5,13 @@
 //   * the final 8x8 average, forward and backward;
 //   * the adjoint of F.interpolate(bilinear, align_corners=True) as a gather (og_bilinear_fwd is the forward);
 //   * eval BatchNorm folded into the convolution: W' = W * s, b' = beta - mean * s, s = gamma / sqrt(var + eps);
-//   * the space-to-depth split of an odd-sized tensor for the valid stride-2 convolutions;
 //   * the gradient through a conv's ReLU epilogue between channel slices of concatenated block outputs.
 //
 // Every backward here is a gather: each input element sums its (at most a few) contributions in a fixed order, so two
 // runs give the same bits.  No atomics.
-#include <cuda_fp16.h>
-
 #include "common.cuh"
 
-extern "C" int og_amax(const float* x, long long n, unsigned* amax, cudaStream_t stream);
-
 namespace {
-
-int grid_for(long long total) {
-  long long b = (total + 255) / 256;
-  const long long cap = (long long)og_num_sms() * 32;
-  return (int)(b < 1 ? 1 : (b > cap ? cap : b));
-}
 
 #define GRID_STRIDE(i, total) \
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < (total); i += (long long)gridDim.x * blockDim.x)
@@ -227,46 +216,6 @@ __global__ void __launch_bounds__(256) bn_fold_kernel(const float* __restrict__ 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// space-to-depth fp16 hi / lo split of a tensor of any H, W: phase block (a*2+b) holds x[:, a::2, b::2] on a
-// ceil(H/2) x ceil(W/2) grid, the row / column past an odd edge zero (what og_prep_split(s2d=1) writes for even sizes)
-// ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) split_s2d_kernel(const float* __restrict__ x, int N, int H, int W, int C8,
-                                                        long long total, const unsigned* __restrict__ amax,
-                                                        __half* __restrict__ xh, __half* __restrict__ xl) {
-  const int Hp = (H + 1) / 2, Wp = (W + 1) / 2;
-  const float scale = og_exp2i(og_scale_exp(__ldg(amax)));
-  GRID_STRIDE(i, total) {
-    const int c = (int)(i % C8);
-    long long t = i / C8;
-    const int w = (int)(t % Wp);
-    t /= Wp;
-    const int h = (int)(t % Hp);
-    long long n = t / Hp;
-    const int ph = (int)(n / N);
-    n -= (long long)ph * N;
-    const int sh = 2 * h + (ph >> 1), sw = 2 * w + (ph & 1);
-    float v[8];
-    if (sh < H && sw < W) {
-      const float* src = x + (((n * H + sh) * W + sw) * C8 + c) * 8;
-      const float4 v0 = ldg4(src), v1 = ldg4(src + 4);
-      v[0] = v0.x; v[1] = v0.y; v[2] = v0.z; v[3] = v0.w; v[4] = v1.x; v[5] = v1.y; v[6] = v1.z; v[7] = v1.w;
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = 0.f;
-    }
-    __align__(16) __half hi[8], lo[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float s = v[j] * scale;
-      hi[j] = __float2half_rn(s);
-      lo[j] = __float2half_rn(s - __half2float(hi[j]));
-    }
-    *reinterpret_cast<uint4*>(xh + i * 8) = *reinterpret_cast<const uint4*>(hi);
-    *reinterpret_cast<uint4*>(xl + i * 8) = *reinterpret_cast<const uint4*>(lo);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
 // out[p, ooff + c] = (relu ? (y[p, yoff + c] > 0 ? g[p, goff + c] : 0) : g[p, goff + c]) for c < nch: the gradient
 // through a conv's ReLU epilogue (torch's threshold_backward masks y > 0), between channel slices
 // ---------------------------------------------------------------------------------------------------------------
@@ -438,7 +387,7 @@ OG_API int og_maxpool3s2_fwd(const float* x, int N, int H, int W, int C, float* 
   const int OH = (H - 3) / 2 + 1, OW = (W - 3) / 2 + 1;
   const long long total = (long long)N * OH * OW * (C / 4);
   if (total == 0) return 0;
-  maxpool3s2_fwd_kernel<<<grid_for(total), 256, 0, stream>>>(x, H, W, C / 4, OH, OW, total, y, ldy, yoff);
+  maxpool3s2_fwd_kernel<<<og_grid(total), 256, 0, stream>>>(x, H, W, C / 4, OH, OW, total, y, ldy, yoff);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -448,7 +397,7 @@ OG_API int og_maxpool3s2_bwd(const float* x, const float* g, int ldg, int goff, 
   const int OH = (H - 3) / 2 + 1, OW = (W - 3) / 2 + 1;
   const long long total = (long long)N * H * W * C;
   if (total == 0) return 0;
-  maxpool3s2_bwd_kernel<<<grid_for(total), 256, 0, stream>>>(x, g, ldg, goff, H, W, C, OH, OW, total, gx);
+  maxpool3s2_bwd_kernel<<<og_grid(total), 256, 0, stream>>>(x, g, ldg, goff, H, W, C, OH, OW, total, gx);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -456,7 +405,7 @@ OG_API int og_avgpool3s1_fwd(const float* x, int N, int H, int W, int C, float* 
   if (C % 4) return (int)cudaErrorInvalidValue;
   const long long total = (long long)N * H * W * (C / 4);
   if (total == 0) return 0;
-  avgpool3s1_kernel<<<grid_for(total), 256, 0, stream>>>(x, H, W, C / 4, total, y);
+  avgpool3s1_kernel<<<og_grid(total), 256, 0, stream>>>(x, H, W, C / 4, total, y);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -464,21 +413,21 @@ OG_API int og_avgpool3s1_bwd(const float* g, int N, int H, int W, int C, float* 
   if (C % 4) return (int)cudaErrorInvalidValue;
   const long long total = (long long)N * H * W * (C / 4);
   if (total == 0) return 0;
-  avgpool3s1_bwd_kernel<<<grid_for(total), 256, 0, stream>>>(g, H, W, C / 4, total, gx);
+  avgpool3s1_bwd_kernel<<<og_grid(total), 256, 0, stream>>>(g, H, W, C / 4, total, gx);
   OG_RETURN_LAST_ERROR();
 }
 
 OG_API int og_global_avg_fwd(const float* x, int N, int P, int C, float* y, cudaStream_t stream) {
   const long long total = (long long)N * C;
   if (total == 0 || P == 0) return 0;
-  global_avg_kernel<<<grid_for(total), 256, 0, stream>>>(x, P, C, total, y);
+  global_avg_kernel<<<og_grid(total), 256, 0, stream>>>(x, P, C, total, y);
   OG_RETURN_LAST_ERROR();
 }
 
 OG_API int og_global_avg_bwd(const float* g, int N, int P, int C, float* gx, cudaStream_t stream) {
   const long long total = (long long)N * P * C;
   if (total == 0) return 0;
-  global_avg_bwd_kernel<<<grid_for(total), 256, 0, stream>>>(g, P, C, total, gx);
+  global_avg_bwd_kernel<<<og_grid(total), 256, 0, stream>>>(g, P, C, total, gx);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -488,7 +437,7 @@ OG_API int og_bilinear_bwd_gather(const float* g, int N, int IH, int IW, int C, 
   const long long total = (long long)N * IH * IW * C;
   if (total == 0) return 0;
   const float rh = OH > 1 ? (float)(IH - 1) / (float)(OH - 1) : 0.f, rw = OW > 1 ? (float)(IW - 1) / (float)(OW - 1) : 0.f;
-  bilinear_bwd_gather_kernel<<<grid_for(total), 256, 0, stream>>>(g, IH, IW, OH, OW, C, rh, rw, rh > 0.f ? 1.f / rh : 0.f,
+  bilinear_bwd_gather_kernel<<<og_grid(total), 256, 0, stream>>>(g, IH, IW, OH, OW, C, rh, rw, rh > 0.f ? 1.f / rh : 0.f,
                                                                    rw > 0.f ? 1.f / rw : 0.f, total, gx);
   OG_RETURN_LAST_ERROR();
 }
@@ -496,21 +445,7 @@ OG_API int og_bilinear_bwd_gather(const float* g, int N, int IH, int IW, int C, 
 OG_API int og_bn_fold(const float* w, int Co, long long R, const float* gamma, const float* beta, const float* mean,
                       const float* var, float eps, float* wout, float* bout, cudaStream_t stream) {
   if ((long long)Co * R == 0) return 0;
-  bn_fold_kernel<<<grid_for((long long)Co * R), 256, 0, stream>>>(w, Co, R, gamma, beta, mean, var, eps, wout, bout);
-  OG_RETURN_LAST_ERROR();
-}
-
-// xh / xl: [4N][ceil(H/2)][ceil(W/2)][C]; *amax as in og_prep_split
-OG_API int og_prep_split_s2d(const float* x, int N, int H, int W, int C, unsigned* amax, int amax_ready, void* xh,
-                             void* xl, cudaStream_t stream) {
-  if (!xh || !xl || C % 8) return (int)cudaErrorInvalidValue;
-  if (!amax_ready) {
-    const int rc = og_amax(x, (long long)N * H * W * C, amax, stream);
-    if (rc) return rc;
-  }
-  const long long total = 4LL * N * ((H + 1) / 2) * ((W + 1) / 2) * (C / 8);
-  if (total == 0) return 0;
-  split_s2d_kernel<<<grid_for(total), 256, 0, stream>>>(x, N, H, W, C / 8, total, amax, (__half*)xh, (__half*)xl);
+  bn_fold_kernel<<<og_grid((long long)Co * R), 256, 0, stream>>>(w, Co, R, gamma, beta, mean, var, eps, wout, bout);
   OG_RETURN_LAST_ERROR();
 }
 
@@ -519,7 +454,7 @@ OG_API int og_relu_grad_slice(const float* y, int ldy, int yoff, const float* g,
   if (nch % 4 || ldy % 4 || yoff % 4 || ldg % 4 || goff % 4 || ldo % 4 || ooff % 4) return (int)cudaErrorInvalidValue;
   const long long total = P * (nch / 4);
   if (total == 0) return 0;
-  relu_grad_slice_kernel<<<grid_for(total), 256, 0, stream>>>(y, ldy, yoff, g, ldg, goff, out, ldo, ooff, nch / 4, relu,
+  relu_grad_slice_kernel<<<og_grid(total), 256, 0, stream>>>(y, ldy, yoff, g, ldg, goff, out, ldo, ooff, nch / 4, relu,
                                                               total);
   OG_RETURN_LAST_ERROR();
 }
@@ -543,7 +478,7 @@ OG_API int og_inception_input(const float* x, int N, int H, int W, int OS, int m
     rh = (float)H / (float)OS;
     rw = (float)W / (float)OS;
   }
-  inception_input_kernel<<<grid_for(total), 256, 0, stream>>>(x, H, W, OS, mode, rh, rw, af, total, y);
+  inception_input_kernel<<<og_grid(total), 256, 0, stream>>>(x, H, W, OS, mode, rh, rw, af, total, y);
   OG_RETURN_LAST_ERROR();
 }
 

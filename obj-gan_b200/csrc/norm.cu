@@ -12,8 +12,7 @@
 //
 // Layout: contiguous NHWC, rows = pixels, C % 4 == 0.  "groups" = N for instance norm, 1 for batch norm;
 // each group covers P pixels (H*W, resp. N*H*W).
-#include "common.cuh"
-#include <cuda_fp16.h>
+#include "operand.cuh"
 
 // grid: (ceil(C4/32), chunks, groups)   block: (32, 8)
 // A thread owns one channel quad and walks the rows p0 + ty, p0 + ty + 8, ...: four rows are loaded back to back (four
@@ -146,24 +145,8 @@ __global__ void __launch_bounds__(256) norm_stats_exact_kernel(const float* __re
 
 // forward apply.  y: conv output [G*P][Cy];  out: [G*P][Co] where Co = Cy (none / lrelu) or Cy/2 (GLU).
 // gamma/beta (BatchNorm affine) may be null (InstanceNorm).  res (same shape as out) is added when non-null.
-// max|.| of the values a 256-thread block has written, merged into *amax (float bits; non-negative floats order like
-// unsigned integers).  The consumer convolution scales its fp16 operand copies by it (og_prep_split).
-__device__ __forceinline__ float amax4(float m, const float4& o) {
-  return fmaxf(fmaxf(m, fmaxf(fabsf(o.x), fabsf(o.y))), fmaxf(fabsf(o.z), fabsf(o.w)));
-}
-__device__ __forceinline__ void block_amax_256(float m, unsigned* amax) {
-  __shared__ float sm_amax[8];
-  const int tid = threadIdx.y * blockDim.x + threadIdx.x;       // 256 threads as (256) or (32, 8)
-  m = warp_max(m);
-  if ((tid & 31) == 0) sm_amax[tid >> 5] = m;
-  __syncthreads();
-  if (tid < 8) {
-    m = sm_amax[tid];
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffu, m, o));
-    if (tid == 0) atomicMax(amax, __float_as_uint(m));
-  }
-}
+// amax (optional) receives max|out| as float bits (block_amax_256): the consumer convolution scales its fp16 operand
+// copies by it (og_prep_split).
 
 // sigmoid on the SFU: ex2.approx + rcp.approx (~2 ulp; the libm expf + IEEE division it replaces made the GLU passes
 // issue bound at half of the HBM bandwidth).  exp(-x) overflowing to +inf gives exactly 0.
@@ -486,7 +469,7 @@ __global__ void __launch_bounds__(256) norm_apply_split_kernel(
   const int Co = (ACT == OG_NA_GLU) ? Cy / 2 : Cy;
   const int C8 = Co >> 3;
   const int Hp = H + 2 * pad, Wp = W + 2 * pad;
-  const float scale = og_exp2i(og_scale_exp(__ldg(bound_word)));
+  const float scale = og_operand_scale(__ldg(bound_word));
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
     const int c = (int)(i % C8) * 8;
@@ -495,13 +478,8 @@ __global__ void __launch_bounds__(256) norm_apply_split_kernel(
     t /= Wp;
     const int h = (int)(t % Hp);
     const long long n = t / Hp;
-    int sh = h - pad, sw = w - pad;
-    const bool interior = sh >= 0 && sh < H && sw >= 0 && sw < W;
-    if (sh < 0) sh = -sh;
-    if (sh >= H) sh = 2 * H - 2 - sh;
-    if (sw < 0) sw = -sw;
-    if (sw >= W) sw = 2 * W - 2 - sw;
-    const long long p = (n * H + sh) * W + sw;
+    const bool interior = h >= pad && h < H + pad && w >= pad && w < W + pad;
+    const long long p = (n * H + og_reflect(h - pad, H)) * W + og_reflect(w - pad, W);
     const long long g = instance ? n : 0;
     const float* yp = y + p * Cy + c;
     const float* mrow = mean + g * Cy + c;
@@ -537,15 +515,7 @@ __global__ void __launch_bounds__(256) norm_apply_split_kernel(
       st4(out + p * Co + c, make_float4(o[0], o[1], o[2], o[3]));
       st4(out + p * Co + c + 4, make_float4(o[4], o[5], o[6], o[7]));
     }
-    __align__(16) __half hi[8], lo[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float v = o[j] * scale;
-      hi[j] = __float2half_rn(v);
-      lo[j] = __float2half_rn(v - __half2float(hi[j]));
-    }
-    *reinterpret_cast<uint4*>(xh + i * 8) = *reinterpret_cast<const uint4*>(hi);
-    *reinterpret_cast<uint4*>(xl + i * 8) = *reinterpret_cast<const uint4*>(lo);
+    og_encode8_store(o, scale, xh, xl, i);
   }
 }
 
@@ -655,11 +625,6 @@ __global__ void bn_eval_param_grad_kernel(const double* __restrict__ part, int S
   dbeta[i] = accumulate ? dbeta[i] + (float)sb : (float)sb;
 }
 
-static int elem_blocks(long long total) {
-  long long b = (total + 255) / 256;
-  long long cap = (long long)og_num_sms() * 32;
-  return (int)(b < cap ? (b < 1 ? 1 : b) : cap);
-}
 static int pix_chunk(long long P, int cgroups, int groups) {
   // aim for >= ~4 blocks per SM overall, at least 64 pixels per block
   long long want = (long long)og_num_sms() * 8;
@@ -694,7 +659,7 @@ OG_API int og_norm_apply(const float* y, int groups, long long P, int Cy, const 
   int Co = act == OG_NA_GLU ? Cy / 2 : Cy;
   if (Cy % 4 || Co % 4) return (int)cudaErrorInvalidValue;
   if (amax_out) OG_CHECK(cudaMemsetAsync(amax_out, 0, sizeof(unsigned), stream));
-  int blocks = elem_blocks(tp * (Co / 4));
+  int blocks = og_grid(tp * (Co / 4));
   if (act == OG_NA_GLU)
     norm_apply_kernel<OG_NA_GLU><<<blocks, 256, 0, stream>>>(y, Cy, P, tp, mean, rstd, gamma, beta, res, slope, out, amax_out);
   else if (act == OG_NA_LRELU)
@@ -807,10 +772,9 @@ OG_API int og_norm_apply_split(const float* y, int N, int H, int W, int Cy, int 
   if (!xh || !xl || Co % 8 || pad < 0 || pad > 1 || (pad && (H < 2 || W < 2))) return (int)cudaErrorInvalidValue;
   const long long total = (long long)N * (H + 2 * pad) * (W + 2 * pad) * (Co / 8);
   if (total == 0) return 0;
-  long long b = (total + 255) / 256;
-  if (b > (long long)og_num_sms() * 32) b = (long long)og_num_sms() * 32;
+  const int b = og_grid(total);
 #define OG_LAUNCH_AS(A)                                                                                              \
-  norm_apply_split_kernel<A><<<(int)b, 256, 0, stream>>>(y, N, H, W, Cy, instance, mean, rstd, gamma, beta, res, slope, \
+  norm_apply_split_kernel<A><<<b, 256, 0, stream>>>(y, N, H, W, Cy, instance, mean, rstd, gamma, beta, res, slope, \
                                                          out, bound_word, pad, total, (__half*)xh, (__half*)xl)
   if (act == OG_NA_GLU) OG_LAUNCH_AS(OG_NA_GLU);
   else if (act == OG_NA_LRELU) OG_LAUNCH_AS(OG_NA_LRELU);

@@ -9,6 +9,8 @@ pad lanes kept at exactly zero.
 """
 from __future__ import annotations
 
+from collections import namedtuple
+
 import torch
 
 from . import lib as _lib
@@ -75,10 +77,20 @@ class PackedWeights:
         self.hl = {}
         self.amax = None
 
+    @staticmethod
+    def _key(w, cip, kp, split):
+        """What the cached copies were derived from: the parameter's storage, its version and epochs, and the layout."""
+        return (w.data_ptr(), w._version, _epoch_of(w), cip, kp, split)
+
     def _refresh(self, w, cip, kp, split):
-        key = (w.data_ptr(), w._version, _epoch_of(w), cip, kp, split)
+        key = self._key(w, cip, kp, split)
         if key != self.key:
             self.key, self.f, self.t, self.hl, self.amax = key, None, None, {}, None
+
+    def install(self, w, cip, kp, split, amax, hl):
+        """Re-validate the cache for the current w with the fp16 copies PackPlan.run re-packed in place
+        (hl: {transposed: (hi, lo, amax)}); every other copy is dropped."""
+        self.key, self.f, self.t, self.hl, self.amax = self._key(w, cip, kp, split), None, None, hl, amax
 
     def _amax(self, w):
         """Device word with the float bits of max|w| (the power-of-two scale of the fp16 operand copies)."""
@@ -132,6 +144,9 @@ class PackedWeights:
         return self.hl[transposed]
 
 
+_PackJob = namedtuple("_PackJob", "cache w cip kp split splitp transposed hi lo amax")
+
+
 class PackPlan:
     """All (weight, layout) fp16 operand copies of ONE network, re-derived by two launches (og_amax_multi +
     og_pack_weights_f16_multi) right after the network's optimiser step instead of lazily, layer by layer, at the next
@@ -139,14 +154,14 @@ class PackPlan:
     ``run`` refreshes the SAME buffers and re-validates the layers' caches."""
 
     def __init__(self):
-        self.jobs = []              # (cache, w, cip, kp, split, splitp, transposed, hi, lo, amax)
+        self.jobs = []              # _PackJob
         self._tables = None
         self._n_built = 0
 
     def record(self, cache, w, cip, kp, split, splitp, transposed, hi, lo, amax):
-        job = (cache, w, cip, kp, split, splitp, transposed, hi, lo, amax)
+        job = _PackJob(cache, w, cip, kp, split, splitp, transposed, hi, lo, amax)
         for i, j in enumerate(self.jobs):
-            if j[0] is cache and j[6] == transposed:      # same layer and layout packed again: new buffers
+            if j.cache is cache and j.transposed == transposed:      # same layer and layout packed again: new buffers
                 self.jobs[i] = job
                 self._tables = None
                 return
@@ -155,15 +170,16 @@ class PackPlan:
     def _build(self, device):
         CH = 4096
         arows, prows, ab, pb, seen = [], [], 0, 0, {}
-        for cache, w, cip, kp, split, splitp, tr, hi, lo, amax in self.jobs:
-            if id(amax) not in seen:
-                seen[id(amax)] = True
-                arows.append([w.data_ptr(), w.numel(), amax.data_ptr(), ab])
+        for j in self.jobs:
+            w = j.w
+            if id(j.amax) not in seen:
+                seen[id(j.amax)] = True
+                arows.append([w.data_ptr(), w.numel(), j.amax.data_ptr(), ab])
                 ab += (w.numel() + CH - 1) // CH
             co, ci, kh, kw = w.shape
-            total = kh * kw * cip * kp
-            prows.append([w.data_ptr(), hi.data_ptr(), lo.data_ptr(), amax.data_ptr(), co, ci,
-                          kh * kw, cip, kp, split, splitp, tr, total, pb])
+            total = kh * kw * j.cip * j.kp
+            prows.append([w.data_ptr(), j.hi.data_ptr(), j.lo.data_ptr(), j.amax.data_ptr(), co, ci,
+                          kh * kw, j.cip, j.kp, j.split, j.splitp, j.transposed, total, pb])
             pb += (total + CH - 1) // CH
         mk = lambda rows: h2d(rows, device, torch.int64)
         self._tables = (mk(arows), len(arows), ab, mk(prows), len(prows), pb)
@@ -174,19 +190,15 @@ class PackPlan:
         if not self.jobs:
             return
         if self._tables is None or self._n_built != len(self.jobs):
-            self._build(self.jobs[0][1].device)
+            self._build(self.jobs[0].w.device)
         at, an, ab, pt, pn, pb = self._tables
         _call("og_amax_multi", _p(at), an, ab)
         _call("og_pack_weights_f16_multi", _p(pt), pn, pb)
-        touched = {}
-        for cache, w, cip, kp, split, splitp, tr, hi, lo, amax in self.jobs:
-            if id(cache) not in touched:
-                touched[id(cache)] = cache
-                cache.key = (w.data_ptr(), w._version, _epoch_of(w), cip, kp, split)
-                cache.f = cache.t = None
-                cache.hl = {}
-                cache.amax = amax
-            cache.hl[tr] = (hi, lo, amax)
+        per_cache = {}              # id(cache) -> (its first job, {transposed: (hi, lo, amax)})
+        for j in self.jobs:
+            per_cache.setdefault(id(j.cache), (j, {}))[1][j.transposed] = (j.hi, j.lo, j.amax)
+        for j, hl in per_cache.values():
+            j.cache.install(j.w, j.cip, j.kp, j.split, j.amax, hl)
 
 
 # Contraction engine for the convolutions: "f16x3" = wgmma tensor cores with the error-compensated
@@ -195,7 +207,6 @@ class PackPlan:
 import ctypes
 import functools
 import os as _os
-from collections import namedtuple
 CONV_ENGINE = _os.environ.get("OBJGAN_CONV", "f16x3")
 if CONV_ENGINE not in ("f16x3", "simt"):
     raise ValueError("OBJGAN_CONV=%r: the convolution engine is 'f16x3' or 'simt'" % CONV_ENGINE)

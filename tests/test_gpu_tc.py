@@ -1,6 +1,7 @@
-"""GPU tests of the tensor-core convolution path's operand handling (conv_tc.cu): the exact hi/lo operand split, the
-producer-side operand copies of the normalisation pass, and the refusal of a missing lo copy.  The convolutions
-themselves are compared with float64 at every layer shape in tests/test_gpu_conv.py."""
+"""GPU tests of the tensor-core convolution path's operand handling (operands.cu, norm.cu): the exact hi/lo operand
+split, the producer-side operand copies of the normalisation pass, and the refusal of a missing lo copy.  Every writer
+is compared bit for bit with a numpy restatement in tests/test_gpu_operands.py; the convolutions themselves are
+compared with float64 at every layer shape in tests/test_gpu_conv.py."""
 import pytest
 import torch
 import torch.nn.functional as F
