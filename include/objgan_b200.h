@@ -175,8 +175,8 @@ int og_words_proj_bwd(const float* words, const float* W, const float* gsrc, int
                       int accumulate, float* gwords, cudaStream_t stream);
 int og_att_general_fwd(const float* h, const float* src, const unsigned char* mask, int B, int Q, int idf, int cs,
                        int L, float* wc, float* attn, cudaStream_t stream);
-int og_att_general_bwd(const float* h, const float* src, const float* attn, const float* g_wc, const float* g_attn,
-                       int B, int Q, int idf, int cs, int L, float* g_h, float* g_src, cudaStream_t stream);
+int og_att_general_bwd(const float* h, const float* src, const float* attn, const float* g_wc, int B, int Q, int idf,
+                       int cs, int L, float* g_h, float* g_src, cudaStream_t stream);
 int og_bu_att_fwd(const float* labels, const float* glove, const float* src, const unsigned char* mask, int B, int E,
                   int R, int L, int idf, int norm, float eps, float* wc, float* attn, cudaStream_t stream);
 int og_bu_att_bwd(const float* attn, const float* g_wc, int B, int R, int L, int idf, float* g_src,

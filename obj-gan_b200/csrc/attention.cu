@@ -19,6 +19,35 @@ __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
 }
 constexpr int ATT_Q = 128; // queries per block
 
+// The grid-attention kernels stage rows of `cs` floats (row stride cs, cs % 4 == 0) in shared tiles of pitch cs + 1.
+// Both walks move 16 bytes per thread and step, and advance the thread's (row, quad) position by ATT_Q quads without
+// a division.
+// Rows [0, nq) of g -> tile rows [0, nq); with ZERO_TAIL, tile rows [nq, ATT_Q) become zeros.
+template <bool ZERO_TAIL>
+__device__ __forceinline__ void rows_to_tile(float* tile, const float* __restrict__ g, int cs, int nq) {
+  const int pitch = cs + 1, cs4 = cs >> 2, t = threadIdx.x;
+  for (int r = t / cs4, c4 = t - (t / cs4) * cs4, i = t; i < (ZERO_TAIL ? ATT_Q : nq) * cs4; i += ATT_Q) {
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (!ZERO_TAIL || r < nq) v = ldg4(g + i * 4);
+    float* d = tile + r * pitch + c4 * 4;
+    d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
+    c4 += ATT_Q % cs4;
+    r += ATT_Q / cs4;
+    if (c4 >= cs4) { c4 -= cs4; ++r; }
+  }
+}
+// Tile rows [0, nq) -> rows [0, nq) of g.
+__device__ __forceinline__ void tile_to_rows(float* __restrict__ g, const float* tile, int cs, int nq) {
+  const int pitch = cs + 1, cs4 = cs >> 2, t = threadIdx.x;
+  for (int r = t / cs4, c4 = t - (t / cs4) * cs4, i = t; i < nq * cs4; i += ATT_Q) {
+    const float* d = tile + r * pitch + c4 * 4;
+    st4(g + i * 4, make_float4(d[0], d[1], d[2], d[3]));
+    c4 += ATT_Q % cs4;
+    r += ATT_Q / cs4;
+    if (c4 >= cs4) { c4 -= cs4; ++r; }
+  }
+}
+
 // src[b][c][l] = sum_k W[c][k] * words[b][k][l]
 __global__ void words_proj_kernel(const float* __restrict__ words, const float* __restrict__ W, int idf, int cdf,
                                   int L, float* __restrict__ src) {
@@ -79,71 +108,48 @@ OG_API int og_words_proj_bwd(const float* words, const float* W, const float* gs
 // mask: [B][L] bytes (1 = padding word) or null.  wc: [B][Q][cs] (pad lanes zeroed), attn: [B][L][Q].
 // Mask quirk (ref: GlobalAttention.py:108): row (b, q) uses the caption mask of sample (b*Q + q) mod B.
 // ---------------------------------------------------------------------------------------------
-// QPT queries per thread (rows t, t + ATT_Q, ... of the block's tile): every 128-bit broadcast load of a word-projection
-// row feeds QPT queries.  With one query per thread the kernel is bound by the shared-memory return path (each
-// LDS.128 writes 512 bytes of registers per warp: 5 of them per 20 FMAs), not by HBM; QPT = 2 halves that.
-template <int LM, int QPT>
-__global__ void __launch_bounds__(ATT_Q, (QPT == 1 ? 7 : 4))
+template <int LM>
+__global__ void __launch_bounds__(ATT_Q, 7)
 att_general_fwd_kernel(const float* __restrict__ h, const float* __restrict__ src,
                        const unsigned char* __restrict__ mask, int B, int Q, int idf, int cs, int L,
                        float* __restrict__ wc, float* __restrict__ attn) {
   // The word projections src[c][0..L) live in shared memory as rows of LM floats (zero padded) and are read with
-  // 128-bit broadcast loads: one LDS.128 feeds four FMAs per query.
+  // 128-bit broadcast loads: one LDS.128 feeds four FMAs.
   extern __shared__ __align__(16) float smem[];
-  constexpr int TQ = ATT_Q * QPT;        // queries per block
   const int pitch = cs + 1;
   float* ssrc = smem;                    // [idf][LM]
-  float* tile = smem + idf * LM;         // [TQ][pitch]
-  const int b = blockIdx.y, q0 = blockIdx.x * TQ, t = threadIdx.x;
-  const int nq = min(TQ, Q - q0);
+  float* tile = smem + idf * LM;         // [ATT_Q][pitch]
+  const int b = blockIdx.y, q0 = blockIdx.x * ATT_Q, t = threadIdx.x;
+  const int nq = min(ATT_Q, Q - q0);
   for (int i = t; i < idf * LM; i += ATT_Q) {
     int c = i / LM, l = i - c * LM;
     ssrc[i] = l < L ? src[((long long)b * idf + c) * L + l] : 0.f;
   }
-  const float* hb = h + ((long long)b * Q + q0) * cs;
-  const int cs4 = cs >> 2;
-  for (int r = t / cs4, c4 = t - (t / cs4) * cs4, i = t; i < nq * cs4; i += ATT_Q) {
-    float4 v = ldg4(hb + i * 4);
-    float* d = tile + r * pitch + c4 * 4;
-    d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
-    c4 += ATT_Q % cs4;                   // advance (r, c4) by ATT_Q elements without a division
-    r += ATT_Q / cs4;
-    if (c4 >= cs4) { c4 -= cs4; ++r; }
-  }
+  rows_to_tile<false>(tile, h + ((long long)b * Q + q0) * cs, cs, nq);
   __syncthreads();
-  float2 s2[QPT][LM / 2];
+  float2 s2[LM / 2];
 #pragma unroll
-  for (int u = 0; u < QPT; ++u)
-#pragma unroll
-    for (int l = 0; l < LM / 2; ++l) s2[u][l] = make_float2(0.f, 0.f);
+  for (int l = 0; l < LM / 2; ++l) s2[l] = make_float2(0.f, 0.f);
   // rows past nq hold stale shared memory: they are computed but never stored
   for (int c = 0; c < idf; ++c) {
-    float2 hv2[QPT];
-#pragma unroll
-    for (int u = 0; u < QPT; ++u) {
-      const float hv = tile[(t + u * ATT_Q) * pitch + c];
-      hv2[u] = make_float2(hv, hv);
-    }
+    const float hv = tile[t * pitch + c];
+    const float2 hv2 = make_float2(hv, hv);
     const float4* sr = reinterpret_cast<const float4*>(ssrc + c * LM);
 #pragma unroll
     for (int l4 = 0; l4 < LM / 4; ++l4) {
       const float4 w = sr[l4];
-#pragma unroll
-      for (int u = 0; u < QPT; ++u) {
-        s2[u][2 * l4] = ffma2(hv2[u], make_float2(w.x, w.y), s2[u][2 * l4]);
-        s2[u][2 * l4 + 1] = ffma2(hv2[u], make_float2(w.z, w.w), s2[u][2 * l4 + 1]);
-      }
+      s2[2 * l4] = ffma2(hv2, make_float2(w.x, w.y), s2[2 * l4]);
+      s2[2 * l4 + 1] = ffma2(hv2, make_float2(w.z, w.w), s2[2 * l4 + 1]);
     }
   }
-#pragma unroll
-  for (int u = 0; u < QPT; ++u) {
-    const int q = q0 + t + u * ATT_Q;
-    const bool live = t + u * ATT_Q < nq;
+  {
+    const int q = q0 + t;
+    const bool live = t < nq;
     float s[LM];
 #pragma unroll
     for (int l = 0; l < LM / 2; ++l) {
-      s[2 * l] = s2[u][l].x;
-      s[2 * l + 1] = s2[u][l].y;
+      s[2 * l] = s2[l].x;
+      s[2 * l + 1] = s2[l].y;
     }
     float mx = -INFINITY;
     if (mask && live) {
@@ -168,41 +174,25 @@ att_general_fwd_kernel(const float* __restrict__ h, const float* __restrict__ sr
       if (l < L && live) attn[((long long)b * L + l) * Q + q] = s[l];
     }
 #pragma unroll
-    for (int l = 0; l < LM / 2; ++l) s2[u][l] = make_float2(s[2 * l], s[2 * l + 1]);
+    for (int l = 0; l < LM / 2; ++l) s2[l] = make_float2(s[2 * l], s[2 * l + 1]);
   }
   for (int c = 0; c < cs; ++c) {
-    float acc[QPT];
-#pragma unroll
-    for (int u = 0; u < QPT; ++u) acc[u] = 0.f;
+    float acc = 0.f;
     if (c < idf) {
       const float4* sr = reinterpret_cast<const float4*>(ssrc + c * LM);
-      float2 a2[QPT], b2[QPT];             // four interleaved partial sums per query: short dependent FMA chains
-#pragma unroll
-      for (int u = 0; u < QPT; ++u) a2[u] = b2[u] = make_float2(0.f, 0.f);
+      float2 a2 = make_float2(0.f, 0.f), b2 = a2;   // four interleaved partial sums: short dependent FMA chains
 #pragma unroll
       for (int l4 = 0; l4 < LM / 4; ++l4) {
         const float4 w = sr[l4];
-#pragma unroll
-        for (int u = 0; u < QPT; ++u) {
-          a2[u] = ffma2(make_float2(w.x, w.y), s2[u][2 * l4], a2[u]);
-          b2[u] = ffma2(make_float2(w.z, w.w), s2[u][2 * l4 + 1], b2[u]);
-        }
+        a2 = ffma2(make_float2(w.x, w.y), s2[2 * l4], a2);
+        b2 = ffma2(make_float2(w.z, w.w), s2[2 * l4 + 1], b2);
       }
-#pragma unroll
-      for (int u = 0; u < QPT; ++u) acc[u] = (a2[u].x + b2[u].x) + (a2[u].y + b2[u].y);
+      acc = (a2.x + b2.x) + (a2.y + b2.y);
     }
-#pragma unroll
-    for (int u = 0; u < QPT; ++u) tile[(t + u * ATT_Q) * pitch + c] = acc[u];
+    tile[t * pitch + c] = acc;
   }
   __syncthreads();
-  float* wb = wc + ((long long)b * Q + q0) * cs;
-  for (int r = t / cs4, c4 = t - (t / cs4) * cs4, i = t; i < nq * cs4; i += ATT_Q) {
-    const float* d = tile + r * pitch + c4 * 4;
-    st4(wb + i * 4, make_float4(d[0], d[1], d[2], d[3]));
-    c4 += ATT_Q % cs4;
-    r += ATT_Q / cs4;
-    if (c4 >= cs4) { c4 -= cs4; ++r; }
-  }
+  tile_to_rows(wc + ((long long)b * Q + q0) * cs, tile, cs, nq);
 }
 
 // attention_tc.cu: the tensor-core (wgmma) kernel for the large maps of the hot path; -1 = shape outside its envelope
@@ -217,39 +207,26 @@ OG_API int og_att_general_fwd(const float* h, const float* src, const unsigned c
     const int rc = og_att_general_fwd_tc(h, src, mask, B, Q, idf, cs, L, wc, attn, stream);
     if (rc >= 0) return rc;
   }
-  if (L <= 20 && Q >= 4096) {   // the large maps of the hot path: two queries per thread
-    constexpr int QPT = 2;
-    const size_t sm = sizeof(float) * (ATT_Q * QPT * (cs + 1) + idf * 20);
-    static size_t configured = 0;
-    if (sm > configured) {
-      OG_CHECK(cudaFuncSetAttribute(att_general_fwd_kernel<20, QPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-      configured = sm;
-    }
-    dim3 grid2(og_cdiv(Q, ATT_Q * QPT), B);
-    att_general_fwd_kernel<20, QPT><<<grid2, ATT_Q, sm, stream>>>(h, src, mask, B, Q, idf, cs, L, wc, attn);
-    OG_RETURN_LAST_ERROR();
-  }
   const int LMsel = L <= 20 ? 20 : LMAX;
   size_t sm = sizeof(float) * (ATT_Q * (cs + 1) + idf * LMsel);
   dim3 grid(og_cdiv(Q, ATT_Q), B);
   if (L <= 20) {   // captions of the hot path have 12..18 words: keep the per-thread score vector small
     if (sm > 48 * 1024)
-      OG_CHECK(cudaFuncSetAttribute(att_general_fwd_kernel<20, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    att_general_fwd_kernel<20, 1><<<grid, ATT_Q, sm, stream>>>(h, src, mask, B, Q, idf, cs, L, wc, attn);
+      OG_CHECK(cudaFuncSetAttribute(att_general_fwd_kernel<20>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    att_general_fwd_kernel<20><<<grid, ATT_Q, sm, stream>>>(h, src, mask, B, Q, idf, cs, L, wc, attn);
   } else {
-    OG_CHECK(cudaFuncSetAttribute(att_general_fwd_kernel<LMAX, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    att_general_fwd_kernel<LMAX, 1><<<grid, ATT_Q, sm, stream>>>(h, src, mask, B, Q, idf, cs, L, wc, attn);
+    OG_CHECK(cudaFuncSetAttribute(att_general_fwd_kernel<LMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    att_general_fwd_kernel<LMAX><<<grid, ATT_Q, sm, stream>>>(h, src, mask, B, Q, idf, cs, L, wc, attn);
   }
   OG_RETURN_LAST_ERROR();
 }
 
 // backward: g_h [B][Q][cs], g_src [B][idf][L] (accumulated atomically; zeroed by the launcher).
-// g_attn ([B][L][Q]) may be null (the attention maps are only visualised in training).
+// The attention map is an output the networks only visualise, so no gradient flows into it.
 __global__ void __launch_bounds__(ATT_Q) att_general_bwd_kernel(const float* __restrict__ h,
                                                                 const float* __restrict__ src,
                                                                 const float* __restrict__ attn,
-                                                                const float* __restrict__ g_wc,
-                                                                const float* __restrict__ g_attn, int B, int Q,
+                                                                const float* __restrict__ g_wc, int B, int Q,
                                                                 int idf, int cs, int L, float* __restrict__ g_h,
                                                                 float* __restrict__ g_src) {
   extern __shared__ float smem[];
@@ -262,20 +239,10 @@ __global__ void __launch_bounds__(ATT_Q) att_general_bwd_kernel(const float* __r
   const int b = blockIdx.y, q0 = blockIdx.x * ATT_Q, t = threadIdx.x;
   const int nq = min(ATT_Q, Q - q0);
   for (int i = t; i < idf * L; i += ATT_Q) ssrc[i] = src[(long long)b * idf * L + i];
-  const float* hb = h + ((long long)b * Q + q0) * cs;
-  const float* gb = g_wc + ((long long)b * Q + q0) * cs;
-  for (int i = t; i < nq * cs / 4; i += ATT_Q) {
-    int r = (i * 4) / cs, c = (i * 4) - r * cs;
-    float4 v = ldg4(hb + i * 4), w = ldg4(gb + i * 4);
-    float* d = th + r * pitch + c;
-    d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
-    float* e = tg + r * pitch + c;
-    e[0] = w.x; e[1] = w.y; e[2] = w.z; e[3] = w.w;
-  }
+  rows_to_tile<false>(th, h + ((long long)b * Q + q0) * cs, cs, nq);
+  rows_to_tile<false>(tg, g_wc + ((long long)b * Q + q0) * cs, cs, nq);
   __syncthreads();
   float gS[LMAX];
-  float hrow_keep = 0.f;
-  (void)hrow_keep;
   if (t < nq) {
     const int q = q0 + t;
     float A[LMAX], gA[LMAX];
@@ -283,10 +250,7 @@ __global__ void __launch_bounds__(ATT_Q) att_general_bwd_kernel(const float* __r
     for (int l = 0; l < LMAX; ++l) {
       A[l] = 0.f;
       gA[l] = 0.f;
-      if (l < L) {
-        A[l] = attn[((long long)b * L + l) * Q + q];
-        if (g_attn) gA[l] = g_attn[((long long)b * L + l) * Q + q];
-      }
+      if (l < L) A[l] = attn[((long long)b * L + l) * Q + q];
     }
     const float* grow = tg + t * pitch;
     for (int c = 0; c < idf; ++c) {
@@ -343,12 +307,7 @@ __global__ void __launch_bounds__(ATT_Q) att_general_bwd_kernel(const float* __r
     }
   }
   __syncthreads();
-  float* ob = g_h + ((long long)b * Q + q0) * cs;
-  for (int i = t; i < nq * cs / 4; i += ATT_Q) {
-    int r = (i * 4) / cs, c = (i * 4) - r * cs;
-    const float* d = th + r * pitch + c;
-    st4(ob + i * 4, make_float4(d[0], d[1], d[2], d[3]));
-  }
+  tile_to_rows(g_h + ((long long)b * Q + q0) * cs, th, cs, nq);
 }
 
 // Backward for L <= 20 (the hot path): same arithmetic as above with the forward kernel's register blocking --
@@ -357,8 +316,8 @@ __global__ void __launch_bounds__(ATT_Q) att_general_bwd_kernel(const float* __r
 // ([48 c x 2 halves of 10 words] threads, reduction over the block's 128 queries from shared memory); (B) g_h rows.
 __global__ void __launch_bounds__(ATT_Q, 3)
 att_general_bwd20_kernel(const float* __restrict__ h, const float* __restrict__ src, const float* __restrict__ attn,
-                         const float* __restrict__ g_wc, const float* __restrict__ g_attn, int B, int Q, int idf,
-                         int cs, int L, float* __restrict__ g_h, float* __restrict__ g_src) {
+                         const float* __restrict__ g_wc, int B, int Q, int idf, int cs, int L,
+                         float* __restrict__ g_h, float* __restrict__ g_src) {
   constexpr int LM = 20;
   extern __shared__ __align__(16) float smem[];
   const int pitch = cs + 1;
@@ -373,23 +332,8 @@ att_general_bwd20_kernel(const float* __restrict__ h, const float* __restrict__ 
     const int c = i / LM, l = i - c * LM;
     ssrc[i] = l < L ? src[((long long)b * idf + c) * L + l] : 0.f;
   }
-  const float* hb = h + ((long long)b * Q + q0) * cs;
-  const float* gb = g_wc + ((long long)b * Q + q0) * cs;
-  const int cs4 = cs >> 2;
-  for (int r = t / cs4, c4 = t - (t / cs4) * cs4, i = t; i < ATT_Q * cs4; i += ATT_Q) {
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f), w = v;
-    if (r < nq) {
-      v = ldg4(hb + i * 4);
-      w = ldg4(gb + i * 4);
-    }
-    float* d = th + r * pitch + c4 * 4;
-    d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
-    float* e = tg + r * pitch + c4 * 4;
-    e[0] = w.x; e[1] = w.y; e[2] = w.z; e[3] = w.w;
-    c4 += ATT_Q % cs4;
-    r += ATT_Q / cs4;
-    if (c4 >= cs4) { c4 -= cs4; ++r; }
-  }
+  rows_to_tile<true>(th, h + ((long long)b * Q + q0) * cs, cs, nq);
+  rows_to_tile<true>(tg, g_wc + ((long long)b * Q + q0) * cs, cs, nq);
   __syncthreads();
   // (A) gA[l] = sum_c g_wc[q][c] * src[c][l]
   float2 s2[LM / 2];
@@ -422,10 +366,7 @@ att_general_bwd20_kernel(const float* __restrict__ h, const float* __restrict__ 
 #pragma unroll
     for (int l = 0; l < LM; ++l) {
       A[l] = 0.f;
-      if (l < L && live) {
-        A[l] = attn[((long long)b * L + l) * Q + q];
-        if (g_attn) gA[l] += g_attn[((long long)b * L + l) * Q + q];
-      }
+      if (l < L && live) A[l] = attn[((long long)b * L + l) * Q + q];
       dot = fmaf(gA[l], A[l], dot);
     }
 #pragma unroll
@@ -483,26 +424,18 @@ att_general_bwd20_kernel(const float* __restrict__ h, const float* __restrict__ 
     }
   }
   __syncthreads();
-  float* ob = g_h + ((long long)b * Q + q0) * cs;
-  for (int r = t / cs4, c4 = t - (t / cs4) * cs4, i = t; i < nq * cs4; i += ATT_Q) {
-    const float* d = th + r * pitch + c4 * 4;
-    st4(ob + i * 4, make_float4(d[0], d[1], d[2], d[3]));
-    c4 += ATT_Q % cs4;
-    r += ATT_Q / cs4;
-    if (c4 >= cs4) { c4 -= cs4; ++r; }
-  }
+  tile_to_rows(g_h + ((long long)b * Q + q0) * cs, th, cs, nq);
 }
 
 extern "C" int og_att_general_bwd_tc(const float* h, const float* src, const float* attn, const float* g_wc, int B, int Q,
                                      int idf, int cs, int L, float* g_h, float* g_src, cudaStream_t stream);
 
-OG_API int og_att_general_bwd(const float* h, const float* src, const float* attn, const float* g_wc,
-                              const float* g_attn, int B, int Q, int idf, int cs, int L, float* g_h, float* g_src,
-                              cudaStream_t stream) {
+OG_API int og_att_general_bwd(const float* h, const float* src, const float* attn, const float* g_wc, int B, int Q,
+                              int idf, int cs, int L, float* g_h, float* g_src, cudaStream_t stream) {
   if (L > LMAX || cs % 4 || idf > cs) return (int)cudaErrorInvalidValue;
   OG_CHECK(cudaMemsetAsync(g_src, 0, sizeof(float) * (size_t)B * idf * L, stream));
   if (B == 0 || Q == 0) return 0;
-  if (!g_attn && Q >= 4096) {
+  if (Q >= 4096) {
     const int rc = og_att_general_bwd_tc(h, src, attn, g_wc, B, Q, idf, cs, L, g_h, g_src, stream);
     if (rc >= 0) return rc;
   }
@@ -514,13 +447,13 @@ OG_API int og_att_general_bwd(const float* h, const float* src, const float* att
       configured20 = sm20;
     }
     dim3 grid20(og_cdiv(Q, ATT_Q), B);
-    att_general_bwd20_kernel<<<grid20, ATT_Q, sm20, stream>>>(h, src, attn, g_wc, g_attn, B, Q, idf, cs, L, g_h, g_src);
+    att_general_bwd20_kernel<<<grid20, ATT_Q, sm20, stream>>>(h, src, attn, g_wc, B, Q, idf, cs, L, g_h, g_src);
     OG_RETURN_LAST_ERROR();
   }
   size_t sm = sizeof(float) * (2 * ATT_Q * (cs + 1) + 2 * ATT_Q * L + idf * L);
   OG_CHECK(cudaFuncSetAttribute(att_general_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
   dim3 grid(og_cdiv(Q, ATT_Q), B);
-  att_general_bwd_kernel<<<grid, ATT_Q, sm, stream>>>(h, src, attn, g_wc, g_attn, B, Q, idf, cs, L, g_h, g_src);
+  att_general_bwd_kernel<<<grid, ATT_Q, sm, stream>>>(h, src, attn, g_wc, B, Q, idf, cs, L, g_h, g_src);
   OG_RETURN_LAST_ERROR();
 }
 

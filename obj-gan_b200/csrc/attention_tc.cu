@@ -27,6 +27,7 @@
 // CTAs are persistent over the query tiles of ONE image (the word-projection operand tiles are built once; tiles are
 // dealt with a fixed stride).  70 KB of shared memory: three CTAs per SM cover each other's MMA round trips.
 #include "common.cuh"
+#include "operand.cuh"
 #include "wgmma.cuh"
 #include <stdlib.h>
 
@@ -46,8 +47,6 @@ constexpr int AT_MAXB = 128;                          // batch sizes whose capti
 constexpr int AT_PSCALE = 13;                          // probabilities enter MMA 2 as p * 2^13 (fp16 subnormals start at 7e-9)
 constexpr uint32_t AT_HALF = 64 * 128;                // byte offset of the second 64-row half of an A tile
 constexpr int AT_FWD_CTAS = 3, AT_BWD_CTAS = 2;       // CTAs per SM that fit the shared memory
-
-__device__ __forceinline__ uint32_t at_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // byte offset of element (row r, 16-bit column k) in a K-major SWIZZLE_128B tile
 __device__ __forceinline__ uint32_t at_sw_off(int r, int k) {
@@ -79,9 +78,6 @@ __device__ __forceinline__ float4 at_lds128(uint32_t addr) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
   return v;
-}
-__device__ __forceinline__ float at_amax4(float m, const float4& v) {
-  return fmaxf(fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
 }
 // max over the CTA's 128 threads (4 warps) through a 4-word shared scratch; every thread gets the result
 __device__ __forceinline__ float at_cta_max(float m, float* scratch) {
@@ -173,7 +169,7 @@ att_general_fwd_tc_kernel(const float* __restrict__ h, const float* __restrict__
                           const unsigned char* __restrict__ mask, int B, int Q, int L, int nslots,
                           float* __restrict__ wc, float* __restrict__ attn) {
   extern __shared__ uint8_t at_smem_raw[];
-  const uint32_t smem = (at_smem_u32(at_smem_raw) + 1023u) & ~1023u;   // shared-window address of the operand tiles
+  const uint32_t smem = (smem_u32(at_smem_raw) + 1023u) & ~1023u;   // shared-window address of the operand tiles
   const uint32_t sA = smem;                            // hi, lo; reused for the probabilities and the staged context
   const uint32_t sB1 = smem + 2 * AT_A_BYTES;
   const uint32_t sB2 = sB1 + 2 * AT_B1_BYTES;
@@ -232,7 +228,7 @@ att_general_fwd_tc_kernel(const float* __restrict__ h, const float* __restrict__
     // reduction is enough (no block-wide barrier).
     float m = 0.f;
 #pragma unroll
-    for (int i = 0; i < 12; ++i) m = at_amax4(m, hv[i]);
+    for (int i = 0; i < 12; ++i) m = amax4(m, hv[i]);
     m = warp_max(m);
     const int kh = og_scale_exp(__float_as_uint(m));
     const float sh = og_exp2i(kh);
@@ -351,7 +347,7 @@ att_general_fwd_tc_kernel(const float* __restrict__ h, const float* __restrict__
 }
 
 // ------------------------------------------------------------------------------------------------
-// Backward (g_attn = null: the attention maps are only visualised in training).  Per query q:
+// Backward (the attention maps are only visualised, so they carry no gradient).  Per query q:
 //   gP[l]   = sum_c g_wc[q][c] src[c][l]                          MMA 1:  Gw (128 x 48)   . B1
 //   gS[l]   = P[l] (gP[l] - sum_l' P[l'] gP[l'])                  registers (P read from the saved attention map)
 //   g_h[c]  = sum_l gS[l] src[c][l]                               MMA 2:  gS (128 x 32)   . B2
@@ -379,7 +375,7 @@ att_general_bwd_tc_kernel(const float* __restrict__ h, const float* __restrict__
                           const float* __restrict__ g_wc, int B, int Q, int L, int nslots, float* __restrict__ g_h,
                           float* __restrict__ g_src) {
   extern __shared__ uint8_t at_smem_raw[];
-  const uint32_t smem = (at_smem_u32(at_smem_raw) + 1023u) & ~1023u;
+  const uint32_t smem = (smem_u32(at_smem_raw) + 1023u) & ~1023u;
   const uint32_t sX = smem;                            // Gw, then H (hi, lo); finally the staged g_h rows
   const uint32_t sY = smem + 2 * AT_A_BYTES;           // P, then gS (hi, lo)
   const uint32_t sB1 = sY + 2 * AT_A_BYTES;
@@ -455,7 +451,7 @@ att_general_bwd_tc_kernel(const float* __restrict__ h, const float* __restrict__
     // ---- (1) Gw -> X, P -> Y ----
     float mg = 0.f, mh = 0.f;
 #pragma unroll
-    for (int i = 0; i < 12; ++i) { mg = at_amax4(mg, gw[i]); mh = at_amax4(mh, hh[i]); }
+    for (int i = 0; i < 12; ++i) { mg = amax4(mg, gw[i]); mh = amax4(mh, hh[i]); }
     at_cta_max2(mg, mh, red + 1);
     const int kg = og_scale_exp(__float_as_uint(mg)), kh = og_scale_exp(__float_as_uint(mh));
     {
@@ -632,7 +628,7 @@ extern "C" int og_att_general_fwd_tc(const float* h, const float* src, const uns
   OG_RETURN_LAST_ERROR();
 }
 
-// Backward on the tensor cores (g_attn == null only); g_src is overwritten.  Same return convention.
+// Backward on the tensor cores; g_src is overwritten.  Same return convention.
 extern "C" int og_att_general_bwd_tc(const float* h, const float* src, const float* attn, const float* g_wc, int B, int Q,
                                      int idf, int cs, int L, float* g_h, float* g_src, cudaStream_t stream) {
   if (idf != AT_C || cs != AT_C || L < 1 || L > AT_LP || Q % AT_Q != 0 || Q < AT_Q || B < 1) return -1;

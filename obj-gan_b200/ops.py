@@ -1117,7 +1117,7 @@ class _AttGeneral(torch.autograd.Function):
         l = src.shape[2]
         g_h = torch.empty_like(h)
         g_src = torch.empty_like(src)
-        _call("og_att_general_bwd", _p(h), _p(src), _p(attn), _p(g_wc.contiguous()), 0, b, ih * iw, ctx.idf, cs, l,
+        _call("og_att_general_bwd", _p(h), _p(src), _p(attn), _p(g_wc.contiguous()), b, ih * iw, ctx.idf, cs, l,
               _p(g_h), _p(g_src))
         return g_h, g_src, None, None
 

@@ -3,10 +3,9 @@ tests/test_gpu_attention.py (which runs every row against a float64 restatement)
 (which checks that the networks issue no shape missing here).
 
 One table of rows per C entry point:
-  og_att_general_fwd / og_att_general_bwd   (B, Q, idf, cs, L, mask, g_attn)
+  og_att_general_fwd / og_att_general_bwd   (B, Q, idf, cs, L, mask)
       Q = H*W queries, idf real channels of the NHWC rows of stride cs, L words; mask: a caption mask is passed (for
-      the backward: the probabilities it reads were computed under one); g_attn: a gradient of the attention map is
-      passed (never by the networks)
+      the backward: the probabilities it reads were computed under one)
   og_bu_att_fwd / og_bu_att_bwd             (B, E, R, L, idf, norm)      E GloVe dims, R roi slots, norm: cosine
   og_paint_max_fwd / og_paint_max_bwd       (B, num, R, Rtot, P, stride, off)
       num channels painted at lane offset off of NHWC rows of `stride` lanes, R of the Rtot mask slots used
@@ -24,8 +23,8 @@ ENTRIES = (FWD, BWD, BU_FWD, BU_BWD, PAINT_FWD, PAINT_BWD, PROJ, PROJ_BWD)
 
 CASES = {
     # ATT_NET of the three generator stages: 64x64 and 128x128 maps, 18-word captions
-    FWD: [(B, Q, 48, 48, 18, True, False) for B in (1, 16) for Q in (4096, 16384)],
-    BWD: [(16, Q, 48, 48, 18, True, False) for Q in (4096, 16384)],
+    FWD: [(B, Q, 48, 48, 18, True) for B in (1, 16) for Q in (4096, 16384)],
+    BWD: [(16, Q, 48, 48, 18, True) for Q in (4096, 16384)],
     # BT_ATT_NET: 10 roi slots
     BU_FWD: [(B, 50, 10, 18, 48, True) for B in (1, 16)],
     BU_BWD: [(16, 50, 10, 18, 48, True)],
@@ -45,38 +44,39 @@ AT_FWD_CTAS, AT_BWD_CTAS = 3, 2          # CTAs per SM of the forward / backward
 EDGE_CASES = {
     FWD: [
         # tensor cores, <20> template: every caption length up to 20, ragged masks on odd batches (mask row wraps)
-        *[(3, 4096, 48, 48, L, True, False) for L in (1, 2, 7, 12, 17, 18, 19, 20)],
+        *[(3, 4096, 48, 48, L, True) for L in (1, 2, 7, 12, 17, 18, 19, 20)],
         # <32> template
-        *[(3, 4096, 48, 48, L, True, False) for L in (21, 25, 32)],
-        (10, 4096 + 128, 48, 48, 18, True, False),    # Q = 4096 + 128: 33 tiles
-        (100, 4096, 48, 48, 18, True, False),         # nslots = 3 (132 SMs): mstep = 384 mod 100 != 0
-        (128, 4096, 48, 48, 13, True, False),         # the largest batch the mask bit table holds
-        (7, 4096, 48, 48, 18, False, False),          # no mask
-        (NSLOTS_EQ, 4096, 48, 48, 18, True, False),
-        (NSLOTS_DIV, 4096, 48, 48, 18, True, False),
-        (NSLOTS_NDIV, 4096, 48, 48, 18, True, False),
+        *[(3, 4096, 48, 48, L, True) for L in (21, 25, 32)],
+        (10, 4096 + 128, 48, 48, 18, True),    # Q = 4096 + 128: 33 tiles
+        (100, 4096, 48, 48, 18, True),         # nslots = 3 (132 SMs): mstep = 384 mod 100 != 0
+        (128, 4096, 48, 48, 13, True),         # the largest batch the mask bit table holds
+        (7, 4096, 48, 48, 18, False),          # no mask
+        (NSLOTS_EQ, 4096, 48, 48, 18, True),
+        (NSLOTS_DIV, 4096, 48, 48, 18, True),
+        (NSLOTS_NDIV, 4096, 48, 48, 18, True),
         # SIMT
-        (3, 3968, 48, 48, 18, True, False),           # Q % 128 == 0 below the Q >= 4096 gate: <20,1>
-        (3, 4160, 48, 48, 18, True, False),           # Q % 128 != 0: two queries per thread
-        (129, 4096, 48, 48, 18, True, False),         # B > 128: two queries per thread
-        (2, 4096, 32, 32, 18, True, False),           # C = 32: two queries per thread
-        (3, 1000, 48, 48, 21, True, False),           # <LMAX,1>
-        (3, 1000, 48, 48, 32, True, False),
-        (2, 4096, 72, 80, 18, True, False),           # idf > 64, cs != idf: two queries per thread, pad lanes
-        (2, 1000, 72, 80, 18, True, False),           # idf > 64 on <20,1>
+        (3, 3968, 48, 48, 18, True),           # Q % 128 == 0 below the Q >= 4096 gate: <20>
+        (3, 4160, 48, 48, 18, True),           # Q % 128 != 0: <20> above the gate
+        (129, 4096, 48, 48, 18, True),         # B > 128: <20>
+        (2, 4096, 32, 32, 18, True),           # C = 32: <20>
+        (3, 4160, 48, 48, 32, True),           # <LMAX> above the gate
+        (3, 1000, 48, 48, 21, True),           # <LMAX>
+        (3, 1000, 48, 48, 32, True),
+        (2, 4096, 72, 80, 18, True),           # idf > 64, cs != idf: <20>, pad lanes
+        (2, 1000, 72, 80, 18, True),           # idf > 64 on <20> below the gate
     ],
     BWD: [
-        *[(3, 4096, 48, 48, L, True, False) for L in (1, 7, 18, 20, 21, 32)],
-        (10, 4096 + 128, 48, 48, 18, True, False),
-        (100, 4096, 48, 48, 18, True, False),
-        (BWD_ONE_SLOT, 4096, 48, 48, 18, True, False),   # nslots == 1: g_src stored without the workspace planes
-        (3, 3968, 48, 48, 18, True, False),           # SIMT bwd20
-        (3, 4096, 48, 48, 18, True, True),            # g_attn: bwd20
-        (3, 1000, 48, 48, 18, False, True),
-        (3, 1000, 48, 48, 21, True, False),           # the general kernel: L > 20
-        (3, 1000, 48, 48, 32, True, True),            # ... with g_attn
-        (2, 1000, 72, 80, 18, True, False),           # ... idf > 64
-        (2, 4096, 72, 80, 12, True, True),
+        *[(3, 4096, 48, 48, L, True) for L in (1, 7, 18, 20, 21, 32)],
+        (10, 4096 + 128, 48, 48, 18, True),
+        (100, 4096, 48, 48, 18, True),
+        (BWD_ONE_SLOT, 4096, 48, 48, 18, True),   # nslots == 1: g_src stored without the workspace planes
+        (3, 3968, 48, 48, 18, True),           # SIMT bwd20
+        (3, 4160, 48, 48, 18, True),           # Q % 128 != 0: bwd20 above the Q >= 4096 gate
+        (3, 1000, 48, 48, 18, False),
+        (3, 1000, 48, 48, 21, True),           # the general kernel: L > 20
+        (3, 1000, 48, 48, 32, True),
+        (2, 1000, 72, 80, 18, True),           # ... idf > 64
+        (2, 4096, 72, 80, 12, True),           # ... above the gate
     ],
     BU_FWD: [(B, 50, R, L, 48, norm) for B, R, L in ((3, 10, 18), (3, 1, 7), (4, 1, 18), (16, 10, 12))
              for norm in (True, False)],
@@ -133,9 +133,9 @@ def att_needs(work):
     needs = set()
     for name, a in work.calls:
         if name == FWD:          # h, src, mask, B, Q, idf, cs, L, wc, attn
-            needs.add((name, (a[3], a[4], a[5], a[6], a[7], bool(a[2]), False)))
-        elif name == BWD:        # h, src, attn, g_wc, g_attn, B, Q, idf, cs, L, g_h, g_src
-            needs.add((name, (a[5], a[6], a[7], a[8], a[9], None, bool(a[4]))))
+            needs.add((name, (a[3], a[4], a[5], a[6], a[7], bool(a[2]))))
+        elif name == BWD:        # h, src, attn, g_wc, B, Q, idf, cs, L, g_h, g_src
+            needs.add((name, (a[4], a[5], a[6], a[7], a[8], None)))
         elif name == BU_FWD:     # labels, glove, src, mask, B, E, R, L, idf, norm, eps, wc, attn
             needs.add((name, (a[4], a[5], a[6], a[7], a[8], bool(a[9]))))
         elif name == BU_BWD:     # attn, g_wc, B, R, L, idf, g_src

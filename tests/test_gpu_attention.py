@@ -127,8 +127,8 @@ def _fwd_on_tc(B, Q, idf, cs, L):
     return Q >= 4096 and Q % 128 == 0 and idf == 48 and cs == 48 and 1 <= L <= 32 and B <= 128
 
 
-def _bwd_on_tc(B, Q, idf, cs, L, g_attn):
-    return not g_attn and Q >= 4096 and Q % 128 == 0 and idf == 48 and cs == 48 and 1 <= L <= 32
+def _bwd_on_tc(B, Q, idf, cs, L):
+    return Q >= 4096 and Q % 128 == 0 and idf == 48 and cs == 48 and 1 <= L <= 32
 
 
 def _att_inputs(B, Q, idf, cs, L, seed):
@@ -149,7 +149,7 @@ def _mask_rows(mask, B, Q):
     return mask.bool()[idx]
 
 
-def _run_fwd(B, Q, idf, cs, L, mask_on, _g_attn, seed=0):
+def _run_fwd(B, Q, idf, cs, L, mask_on, seed=0):
     tc = _fwd_on_tc(B, Q, idf, cs, L)
     ku = KU_TC if tc else KU_SIMT
     h, src = _att_inputs(B, Q, idf, cs, L, seed)
@@ -192,8 +192,8 @@ def _run_fwd(B, Q, idf, cs, L, mask_on, _g_attn, seed=0):
         assert torch.equal(wc, wc2) and torch.equal(attn, attn2)
 
 
-def _run_bwd(B, Q, idf, cs, L, mask_on, g_attn_on, seed=0):
-    tc = _bwd_on_tc(B, Q, idf, cs, L, g_attn_on)
+def _run_bwd(B, Q, idf, cs, L, mask_on, seed=0):
+    tc = _bwd_on_tc(B, Q, idf, cs, L)
     ku = KU_TC if tc else KU_SIMT
     tag = "tc" if tc else "simt"
     h, src = _att_inputs(B, Q, idf, cs, L, seed)
@@ -207,20 +207,14 @@ def _run_bwd(B, Q, idf, cs, L, mask_on, g_attn_on, seed=0):
         s = torch.where(_mask_rows(_caption_mask(B, L, seed), B, Q), -float("inf"), s)
     P = torch.softmax(s, -1).float()
     attn = P.permute(0, 2, 1).contiguous()
-    g_attn = None
-    if g_attn_on:
-        g_attn = (torch.randn(B, L, Q, device=DEV, generator=gen) * 0.5).contiguous()
     g_h = torch.full((B, Q, cs), float("nan"), device=DEV)
     g_src = torch.full((B, idf, L), float("nan"), device=DEV)
-    _call(BWD, h, src, attn, g_wc, g_attn, B, Q, idf, cs, L, g_h, g_src)
+    _call(BWD, h, src, attn, g_wc, B, Q, idf, cs, L, g_h, g_src)
 
     h64, src64, gw64, P64 = h[..., :idf].double(), src.double(), g_wc[..., :idf].double(), P.double()
     asrc = src64.abs().amax((1, 2))[:, None, None]
     gP = torch.einsum("bqc,bcl->bql", gw64, src64)
     gP_abs = torch.einsum("bqc,bcl->bql", gw64.abs(), src64.abs())
-    if g_attn_on:
-        gP = gP + g_attn.double().permute(0, 2, 1)
-        gP_abs = gP_abs + g_attn.double().abs().permute(0, 2, 1)
     dgP = ku * gP_abs
     if tc:
         dgP = dgP + FLOOR * (_group_amax(gw64, 128) * src64.abs().sum(1)[:, None, :]
@@ -254,7 +248,7 @@ def _run_bwd(B, Q, idf, cs, L, mask_on, g_attn_on, seed=0):
     _check(f"{BWD} g_src ({tag})", g_src, ref, bound)
     if tc:
         g_h2, g_src2 = torch.empty_like(g_h), torch.empty_like(g_src)
-        _call(BWD, h, src, attn, g_wc, None, B, Q, idf, cs, L, g_h2, g_src2)
+        _call(BWD, h, src, attn, g_wc, B, Q, idf, cs, L, g_h2, g_src2)
         assert torch.equal(g_h, g_h2) and torch.equal(g_src, g_src2)
 
 
