@@ -11,7 +11,9 @@ the output grid -- 9 taps of the 2x-upsampled map for the upBlock) and issued TF
 padded M x N x K that the launched tiles cover; the upBlock's four-phase form issues 4 taps per output pixel, not 9).
 The operand split of the input (og_prep_split) is done once, outside the timed calls; the input gradient of a
 reflection-padded layer includes its small og_reflect_pad_bwd pass, and the weight gradient its fixed-order partial
-sum and unpack passes.  Each call reads one of several input sets, together larger than the 50 MB L2.
+sum and unpack passes.  Each call reads one of several input sets, together larger than the 50 MB L2.  For the
+column-order 3x3 layers the forward and input gradient also report their operand bytes from L2 per call, computed
+from the tile geometry, in the per-tap form of conv_tc_kernel and the row-run form of conv_tc_rows_kernel.
 
 --step-profile: batch 16 (bench.py's configuration), eager launches (kernels inside graph replays are not recorded
 separately), 2 warm-up steps and 3 profiled ones; prints the GPU time per kernel name and grid, and the share of the
@@ -38,6 +40,10 @@ L2_BYTES = 50 << 20
 LAYERS = [
     ("hmap_res.conv1 194->388 @128", 194, 388, 3, 1, "reflect", 194, 16, 128, 128),
     ("hmap_res.conv2 194->194 @128", 194, 194, 3, 1, "reflect", 0, 16, 128, 128),
+    ("hmap_res.conv1 194->388 @64", 194, 388, 3, 1, "reflect", 194, 16, 64, 64),
+    ("hmap_res.conv2 194->194 @64", 194, 194, 3, 1, "reflect", 0, 16, 64, 64),
+    ("g_hmap 80->24 @256", 80, 24, 3, 1, "reflect", 0, 16, 256, 256),
+    ("img head 48->3 @256", 48, 3, 3, 1, "zero", 0, 16, 256, 256),
     ("upblock 194->96 @256", 194, 96, 3, 1, "up", 48, 16, 128, 128),
     ("patd256.0 3->96 s2 @256", 3, 96, 4, 2, "zero", 0, 16, 256, 256),
     ("patd256.2 96->192 s2 @128", 96, 192, 4, 2, "zero", 0, 16, 128, 128),
@@ -83,6 +89,22 @@ def issued_tc(n, oh, ow, c, k, ntaps):
     if bn == 32 and k <= 32:                       # stacked [w_hi | w_lo]: two MMAs of twice the width
         return 2 * 2.0 * m * (32 if k <= 16 else 64) * kred
     return 3 * 2.0 * m * math.ceil(k / bn) * bn * kred
+
+
+def operand_bytes_tc(n, oh, ow, c, k, ntaps, run=1):
+    """L2 -> shared-memory operand bytes of one og_conv2d_tc launch, from its tile geometry: per (tap, 64-channel
+    chunk) stage every CTA loads an A tile (hi + lo) of its 128 pixels and a B tile (hi + lo) of its output columns.
+    run = 3: conv_tc_rows_kernel's form, one A box of TH + 2 rows per run of three taps and chunk.  Real channels and
+    output columns only (TMA fills the rest of a partial chunk or tile without reading); pixels outside the source are
+    counted as read."""
+    tn, th, tw = _patch(oh, ow)
+    ptiles = math.ceil(n / tn) * math.ceil(oh / th) * math.ceil(ow / tw)
+    ntile = math.ceil(k / 128)
+    bn = next((b for b in BN_SET if b >= (math.ceil(k / ntile) + 7) // 8 * 8), 128)
+    a_pix = 128 if run == 1 else (th + run - 1) * tw
+    a = ptiles * math.ceil(k / bn) * (ntaps // run) * a_pix * c * 2 * 2
+    b = ptiles * ntaps * k * c * 2 * 2
+    return a + b
 
 
 def issued_wgrad(n, oh, ow, kp, c, entries):
@@ -172,6 +194,12 @@ def bench_layer(spec, window_ms, dirs=("fprop", "dgrad", "wgrad")):
         "wgrad": lambda i: ops._tc_wgrad(sets[i % nsets][1], sets[i % nsets][2], wt, c, kp, split, splitp, geo),
     }
     alg, iss = layer_work(cin, cout, k, stride, mode_s, split, n, h, w)
+    nbytes = {}
+    if k == 3 and stride == 1 and mode_s != "up":    # the two forms of a column-order 3x3 tap list
+        halo = 2 if mode_s == "reflect" else 0
+        for d, geo_d in (("fprop", (n, oh, ow, c, kp)), ("dgrad", (n, h + halo, w + halo, kp, c))):
+            nbytes[d] = {"operand_MB_per_tap": round(operand_bytes_tc(*geo_d, 9) / 1e6, 1),
+                         "operand_MB_row_runs": round(operand_bytes_tc(*geo_d, 9, 3) / 1e6, 1)}
     out = {}
     with torch.no_grad():
         for d, fn in calls.items():
@@ -185,7 +213,7 @@ def bench_layer(spec, window_ms, dirs=("fprop", "dgrad", "wgrad")):
             ms = sorted(_time(fn, reps) for _ in range(3))
             out[d] = {"ms": round(ms[1], 4), "ms_min": round(ms[0], 4), "ms_max": round(ms[2], 4),
                       "alg_tflops": round(alg / (ms[1] * 1e-3) / 1e12, 2),
-                      "issued_tflops": round(iss[d] / (ms[1] * 1e-3) / 1e12, 1), "reps": reps}
+                      "issued_tflops": round(iss[d] / (ms[1] * 1e-3) / 1e12, 1), "reps": reps, **nbytes.get(d, {})}
     return out
 
 
@@ -281,8 +309,10 @@ def main():
             r = bench_layer(spec, args.window_ms)
             res["layers"][spec[0]] = r
             for d, v in r.items():
+                mb = (f"  operand MB per call: {v['operand_MB_per_tap']} per-tap A, {v['operand_MB_row_runs']} row runs"
+                      if "operand_MB_per_tap" in v else "")
                 print(f"{spec[0]:32s} {d:5s} {v['ms']:8.3f} ({v['ms_min']:7.3f}-{v['ms_max']:7.3f}) "
-                      f"{v['alg_tflops']:9.1f} {v['issued_tflops']:11.1f}")
+                      f"{v['alg_tflops']:9.1f} {v['issued_tflops']:11.1f}{mb}")
     print(f"card: {res['card']}")
     print(json.dumps(res))
 

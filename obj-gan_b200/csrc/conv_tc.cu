@@ -60,6 +60,8 @@ struct TcParams {
   int ksplit;               // > 1: gridDim.z CTAs share one output tile, each reduces a slice of the (tap, chunk) loop
   float* work;              // ksplit > 1: slice z writes its partial output to work + z * work_plane (y's layout)
   long long work_plane;
+  // conv_tc_rows_kernel only: taps per row run, resident A slot sets (1 or 2), B ring stages
+  int run, asets, bstages;
   TcTaps taps;
 };
 
@@ -154,6 +156,44 @@ __device__ __forceinline__ void tc_stage_mma(Acc& part, uint64_t ah, uint64_t al
 // Warp index as a value ptxas knows to be warp-uniform (threadIdx.x >> 5 is, but the compiler cannot prove it, and
 // a role branch it takes for divergent serializes every wgmma behind it)
 __device__ __forceinline__ int tc_warp_uniform() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
+
+// ===================== epilogue: registers -> global (consumer warpgroup cg = (warp >> 2) - 1) =====================
+template <int BN, bool STACKED>
+__device__ __forceinline__ void tc_epilogue(TcAccWide<BN>& acc, const TcParams& p, int n0, int h0, int w0, int col0,
+                                            int warp, int lane) {
+  const int cg = (warp >> 2) - 1;
+  float* yrow[2];
+  bool row_ok[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = cg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;   // tile row = output pixel within the patch
+    const int tw = row % p.TW;
+    const int th = (row / p.TW) % p.TH;
+    const int tn = row / (p.TW * p.TH);
+    const int n = n0 + tn, hh = h0 + th, w = w0 + tw;
+    const int oy = p.osy * hh + p.opy, ox = p.osx * w + p.opx;
+    row_ok[h] = (n < p.N) && (hh < p.OH) && (w < p.OW) && (oy < p.OHfull) && (ox < p.OWfull);
+    yrow[h] = p.y + (long long)n * p.ysn + (long long)oy * p.ysh + (long long)ox * p.ysw + col0;
+  }
+  const TcScale sc = tc_scale(p.amax_a, p.amax_b);
+  if (STACKED) acc.fold_halves();
+  acc.each(lane, [&](int c, int h, float v0, float v1) {
+    if (STACKED && c >= BN / 2) return;
+    if (!row_ok[h] || col0 + c >= p.K) return;        // K % 4 == 0: the pair (c, c + 1) is in or out together
+    float2 v = make_float2(v0 * sc.fa * sc.fb, v1 * sc.fa * sc.fb);
+    if (p.bias) {
+      const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + c));
+      v.x += b.x; v.y += b.y;
+    }
+    if (p.act != OG_ACT_NONE) {
+      v.x = tc_act(v.x, p.act, p.slope);
+      v.y = tc_act(v.y, p.act, p.slope);
+    }
+    float* dst = yrow[h] + c;
+    if (p.ksplit > 1) dst = p.work + (long long)blockIdx.z * p.work_plane + (dst - p.y);   // partial sum of this slice
+    *reinterpret_cast<float2*>(dst) = v;
+  });
+}
 
 // ------------------------------------------------------------------------------------------------
 // STACKED (<= 32 output channels): B is [w_hi | w_lo] of the same BN / 2 output channels stacked along N, so a k-step
@@ -260,38 +300,151 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
     }
   }
 
-  // ===================== epilogue: registers -> global =====================
-  float* yrow[2];
-  bool row_ok[2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int row = cg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;   // tile row = output pixel within the patch
-    const int tw = row % p.TW;
-    const int th = (row / p.TW) % p.TH;
-    const int tn = row / (p.TW * p.TH);
-    const int n = n0 + tn, hh = h0 + th, w = w0 + tw;
-    const int oy = p.osy * hh + p.opy, ox = p.osx * w + p.opx;
-    row_ok[h] = (n < p.N) && (hh < p.OH) && (w < p.OW) && (oy < p.OHfull) && (ox < p.OWfull);
-    yrow[h] = p.y + (long long)n * p.ysn + (long long)oy * p.ysh + (long long)ox * p.ysw + col0;
+  tc_epilogue<BN, STACKED>(acc, p, n0, h0, w0, col0, warp, lane);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Row runs: a tap list that splits into runs of R taps with equal (dw, dn) and R consecutive dh (the column-by-column
+// order of the 3x3 stride-1 layers, R = 3).  With a TH x TW patch (TN = 1, TW % 8 == 0) the A tile of tap dh + 1 is
+// the tile of tap dh moved down one image row = TW smem rows, a whole number of 1024-byte swizzle atoms.  So one
+// (TH + R - 1) x TW box per channel chunk and operand holds the A operands of all R taps of a run; tap r is the
+// ordinary K-major descriptor at r * TW * 128 bytes into it, and TMA's zero fill gives the box the values the per-tap
+// boxes of conv_tc_kernel read.  A is loaded once per run instead of once per tap.
+//
+// Shared memory: asets x cchunks A slots (hi and lo box each), every chunk's slot resident across the run (chunk c
+// is read at stages c, c + cchunks, ...), then a ring of bstages B tiles, one (tap, chunk) weight tile each.  Two
+// producer threads in different warps: warp 0 refills A slots as they are released (after the consumers' last tap
+// of the run for that chunk), warp 1 streams the B ring; neither blocks the other.  With two slot sets the next run's
+// A loads as soon as the previous run of the same set is done.
+// The consumers walk exactly the stages of conv_tc_kernel (tap-major, chunk-minor, one fresh partial sum per stage
+// added into the accumulator, the same last-chunk k-steps and epilogue): only the A descriptor's address differs, so
+// the results are bitwise those of conv_tc_kernel.  No reduction split (ksplit == 1).
+constexpr int TC_ROWS_MAX_SLOTS = 8;
+constexpr int TC_ROWS_MAX_BSTAGES = 4;
+// dynamic shared memory per block, the 1024-byte alignment slack included: sm_90's opt-in limit of 227 KB, less room
+// for the static barriers
+constexpr size_t TC_ROWS_SMEM_LIMIT = 227 * 1024 - 1024;
+
+template <int BN, bool STACKED>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+conv_tc_rows_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant__ CUtensorMap map_al,
+                    const __grid_constant__ CUtensorMap map_bh, const __grid_constant__ CUtensorMap map_bl,
+                    const TcParams p) {
+  static_assert(BN % 8 == 0 && BN <= 128, "");
+  constexpr uint32_t B_BYTES = BN * 128;
+  constexpr uint32_t B_STAGE = (STACKED ? 1 : 2) * B_BYTES;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  __shared__ __align__(8) uint64_t a_full[TC_ROWS_MAX_SLOTS], a_empty[TC_ROWS_MAX_SLOTS];
+  __shared__ __align__(8) uint64_t b_full[TC_ROWS_MAX_BSTAGES], b_empty[TC_ROWS_MAX_BSTAGES];
+
+  const int warp = tc_warp_uniform(), lane = threadIdx.x & 31;
+  const int R = p.run;
+  const uint32_t a_box = (uint32_t)((p.TH + R - 1) * p.TW) * 128;   // one operand of one slot; TW % 8 == 0: 1024 | a_box
+  const uint32_t slot_bytes = 2 * a_box;
+  const int nslots = p.asets * p.cchunks;
+  uint8_t* const smem_b = smem + (size_t)nslots * slot_bytes;
+  int t = blockIdx.x;
+  const int tw_i = t % p.tiles_w;
+  t /= p.tiles_w;
+  const int th_i = t % p.tiles_h;
+  const int n0 = t / p.tiles_h, h0 = th_i * p.TH, w0 = tw_i * p.TW;   // TN == 1
+  const int col0 = blockIdx.y * (STACKED ? BN / 2 : BN);
+  const int nk = p.taps.n * p.cchunks;
+
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&map_ah);
+    prefetch_tmap(&map_bh);
+    prefetch_tmap(&map_al);
+    prefetch_tmap(&map_bl);
+    for (int s = 0; s < nslots; ++s) {
+      mbar_init(&a_full[s], 1);
+      mbar_init(&a_empty[s], TC_CONSUMER_WARPS);
+    }
+    for (int s = 0; s < p.bstages; ++s) {
+      mbar_init(&b_full[s], 1);
+      mbar_init(&b_empty[s], TC_CONSUMER_WARPS);
+    }
+    fence_barrier_init();
   }
-  const TcScale sc = tc_scale(p.amax_a, p.amax_b);
-  if (STACKED) acc.fold_halves();
-  acc.each(lane, [&](int c, int h, float v0, float v1) {
-    if (STACKED && c >= BN / 2) return;
-    if (!row_ok[h] || col0 + c >= p.K) return;        // K % 4 == 0: the pair (c, c + 1) is in or out together
-    float2 v = make_float2(v0 * sc.fa * sc.fb, v1 * sc.fa * sc.fb);
-    if (p.bias) {
-      const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + c));
-      v.x += b.x; v.y += b.y;
+  __syncthreads();
+
+  if (warp < 4) {
+    // ===================== TMA producers =====================
+    if (threadIdx.x == 0) {
+      // A: run j fills slot set j % asets, one (TH + R - 1)-row box per chunk and operand from the run's first row
+      for (int j = 0; j < p.taps.n / R; ++j) {
+        const int t0 = j * R;
+        const int hs = h0 + min(p.taps.dh[t0], p.taps.dh[t0 + R - 1]), ws = w0 + p.taps.dw[t0];
+        const int ns = n0 + p.taps.dn[t0];
+        const uint32_t phase = (j / p.asets) & 1;
+        for (int cc = 0; cc < p.cchunks; ++cc) {
+          const int s = (j % p.asets) * p.cchunks + cc;
+          mbar_wait(&a_empty[s], phase ^ 1);
+          uint8_t* sa = smem + (size_t)s * slot_bytes;
+          mbar_expect_tx(&a_full[s], slot_bytes);
+          tma_load_4d(sa, &map_ah, &a_full[s], cc * TC_BK, ws, hs, ns);
+          tma_load_4d(sa + a_box, &map_al, &a_full[s], cc * TC_BK, ws, hs, ns);
+        }
+      }
+    } else if (threadIdx.x == 32) {
+      // B: one (tap, chunk) weight tile per stage, as conv_tc_kernel
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int it = 0; it < nk; ++it) {
+        const int tap = it / p.cchunks, cc = it - tap * p.cchunks;
+        mbar_wait(&b_empty[stage], phase ^ 1);
+        uint8_t* sb = smem_b + (size_t)stage * B_STAGE;
+        mbar_expect_tx(&b_full[stage], B_STAGE);
+        tma_load_3d(sb, &map_bh, &b_full[stage], cc * TC_BK, col0, p.taps.widx[tap]);
+        tma_load_3d(sb + (STACKED ? B_BYTES / 2 : B_BYTES), &map_bl, &b_full[stage], cc * TC_BK, col0, p.taps.widx[tap]);
+        if (++stage == p.bstages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
     }
-    if (p.act != OG_ACT_NONE) {
-      v.x = tc_act(v.x, p.act, p.slope);
-      v.y = tc_act(v.y, p.act, p.slope);
+    return;
+  }
+
+  // ===================== MMA: consumer warpgroup cg owns tile rows [64 cg, 64 cg + 64) =====================
+  const int cg = (warp >> 2) - 1;
+  TcAccWide<BN> acc, part;
+  acc.zero();
+  {
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int it = 0; it < nk; ++it) {
+      const int tap = it / p.cchunks, cc = it - tap * p.cchunks;
+      const int j = tap / R, t0 = j * R;
+      const int s = (j % p.asets) * p.cchunks + cc;
+      const int row = p.taps.dh[tap] - min(p.taps.dh[t0], p.taps.dh[t0 + R - 1]);   // tap's first row in the box
+      mbar_wait(&a_full[s], (j / p.asets) & 1);
+      mbar_wait(&b_full[stage], phase);
+      const uint32_t sa = smem_u32(smem + (size_t)s * slot_bytes) + (uint32_t)(row * p.TW) * 128 + cg * 64 * 128;
+      const uint32_t sb = smem_u32(smem_b + (size_t)stage * B_STAGE);
+      const uint64_t ah = wg_desc_k(sa), al = wg_desc_k(sa + a_box);
+      const uint64_t bh = wg_desc_k(sb), bl = wg_desc_k(sb + B_BYTES);
+      const int ks = cc == p.cchunks - 1 ? p.klast : 4;
+      switch (ks) {
+        case 1: tc_stage_mma<1, 32, STACKED>(part, ah, al, bh, bl); break;
+        case 2: tc_stage_mma<2, 32, STACKED>(part, ah, al, bh, bl); break;
+        case 3: tc_stage_mma<3, 32, STACKED>(part, ah, al, bh, bl); break;
+        default: tc_stage_mma<4, 32, STACKED>(part, ah, al, bh, bl); break;
+      }
+      if (lane == 0) {
+        mbar_arrive(&b_empty[stage]);
+        if (tap - t0 == R - 1) mbar_arrive(&a_empty[s]);   // the run's last tap of this chunk: the slot is free
+      }
+      acc.add(part);
+      if (++stage == p.bstages) {
+        stage = 0;
+        phase ^= 1;
+      }
     }
-    float* dst = yrow[h] + c;
-    if (p.ksplit > 1) dst = p.work + (long long)blockIdx.z * p.work_plane + (dst - p.y);   // partial sum of this slice
-    *reinterpret_cast<float2*>(dst) = v;
-  });
+  }
+
+  tc_epilogue<BN, STACKED>(acc, p, n0, h0, w0, col0, warp, lane);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -371,6 +524,52 @@ int launch_tc_bn(int bn, bool stacked, int stk_rows, const CUtensorMap& ah, cons
     case 128: return launch_tc<128>(ah, al, bh, bl, p, grid, stream);
     default:  return (int)cudaErrorInvalidValue;
   }
+}
+
+template <int BN, bool STACKED = false>
+int launch_tc_rows(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
+                   const TcParams& p, dim3 grid, size_t smem, cudaStream_t stream) {
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_rows_kernel<BN, STACKED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)TC_ROWS_SMEM_LIMIT);
+    if (e != cudaSuccess) return (int)e;
+    configured = true;
+  }
+  conv_tc_rows_kernel<BN, STACKED><<<grid, TC_THREADS, smem, stream>>>(ah, al, bh, bl, p);
+  return (int)cudaGetLastError();
+}
+
+int launch_tc_rows_bn(int bn, bool stacked, int stk_rows, const CUtensorMap& ah, const CUtensorMap& al,
+                      const CUtensorMap& bh, const CUtensorMap& bl, const TcParams& p, dim3 grid, size_t smem,
+                      cudaStream_t stream) {
+  if (stacked)
+    return stk_rows == 16 ? launch_tc_rows<32, true>(ah, al, bh, bl, p, grid, smem, stream)
+                          : launch_tc_rows<64, true>(ah, al, bh, bl, p, grid, smem, stream);
+  switch (bn) {
+    case 32:  return launch_tc_rows<32>(ah, al, bh, bl, p, grid, smem, stream);
+    case 48:  return launch_tc_rows<48>(ah, al, bh, bl, p, grid, smem, stream);
+    case 64:  return launch_tc_rows<64>(ah, al, bh, bl, p, grid, smem, stream);
+    case 96:  return launch_tc_rows<96>(ah, al, bh, bl, p, grid, smem, stream);
+    case 104: return launch_tc_rows<104>(ah, al, bh, bl, p, grid, smem, stream);
+    case 112: return launch_tc_rows<112>(ah, al, bh, bl, p, grid, smem, stream);
+    case 128: return launch_tc_rows<128>(ah, al, bh, bl, p, grid, smem, stream);
+    default:  return (int)cudaErrorInvalidValue;
+  }
+}
+
+// Taps per row run if the tap list splits completely into runs of the same length R >= 2 (equal dw and dn, dh
+// stepping by +1 or by -1 through the run), else 0
+int tc_row_run(const TcTaps& t) {
+  int R = 1;
+  while (R < t.n && t.dw[R] == t.dw[0] && t.dn[R] == t.dn[0] && t.dh[R] - t.dh[R - 1] == t.dh[1] - t.dh[0]) ++R;
+  if (R < 2 || t.n % R || abs(t.dh[1] - t.dh[0]) != 1) return 0;
+  for (int b = 0; b < t.n; b += R)
+    for (int i = b + 1; i < b + R; ++i)
+      if (t.dw[i] != t.dw[b] || t.dn[i] != t.dn[b] || t.dh[i] - t.dh[i - 1] != t.dh[b + 1] - t.dh[b] ||
+          abs(t.dh[i] - t.dh[i - 1]) != 1)
+        return 0;
+  return R;
 }
 
 
@@ -681,21 +880,45 @@ OG_API int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, 
     }
   }
 
-  CUtensorMap mah, mal, mbh, mbl;
-  unsigned long long adims[4] = {(unsigned long long)C, (unsigned long long)SW, (unsigned long long)SH, (unsigned long long)SN};
-  unsigned long long astr[3] = {(unsigned long long)C, (unsigned long long)SW * C, (unsigned long long)SH * SW * C};
-  unsigned abox[4] = {(unsigned)TC_BK, (unsigned)TW, (unsigned)TH, (unsigned)TN};
-  unsigned long long bdims[3] = {(unsigned long long)C, (unsigned long long)Kw, (unsigned long long)ntaps_w};
-  unsigned long long bstr[2] = {(unsigned long long)C, (unsigned long long)Kw * C};
   // <= 32 output channels: [w_hi | w_lo] stacked along N (see conv_tc_kernel)
   const int stk_rows = K <= 16 ? 16 : 32;
   const bool stacked = BNsel == 32 && K <= 32;
+
+  // row runs (conv_tc_rows_kernel): every chunk's A slot resident, two slot sets if they fit, then as deep a B ring
+  // (2 to 4 stages) as the rest of the shared memory holds.  Runs of three taps only: the kernel columns of the 3x3
+  // stride-1 layers, where it was measured.  The 7-tap runs of a 7x1 convolution and the 2-tap runs of a stride-2
+  // input-gradient phase keep conv_tc_kernel (a longer first fill, a shallower B ring; not measured).
+  p.run = tc_row_run(p.taps);
+  p.asets = 1;
+  p.bstages = 0;
+  size_t rows_smem = 0;
+  if (p.run == 3 && TN == 1 && TW % 8 == 0 && p.ksplit == 1) {
+    const size_t slot = 2 * (size_t)(TH + p.run - 1) * TW * 128;
+    const size_t bstage = (size_t)2 * (stacked ? stk_rows : BNsel) * 128;   // hi and lo (stacked: the two halves)
+    if (2 * p.cchunks <= TC_ROWS_MAX_SLOTS && 2 * p.cchunks * slot + 2 * bstage + 1024 <= TC_ROWS_SMEM_LIMIT) p.asets = 2;
+    const size_t aslots = (size_t)p.asets * p.cchunks * slot;
+    if (p.asets * p.cchunks <= TC_ROWS_MAX_SLOTS && aslots + 2 * bstage + 1024 <= TC_ROWS_SMEM_LIMIT) {
+      p.bstages = (int)((TC_ROWS_SMEM_LIMIT - 1024 - aslots) / bstage);
+      if (p.bstages > TC_ROWS_MAX_BSTAGES) p.bstages = TC_ROWS_MAX_BSTAGES;
+      rows_smem = aslots + p.bstages * bstage + 1024;
+    }
+  }
+  const bool rows = p.bstages >= 2;
+
+  CUtensorMap mah, mal, mbh, mbl;
+  unsigned long long adims[4] = {(unsigned long long)C, (unsigned long long)SW, (unsigned long long)SH, (unsigned long long)SN};
+  unsigned long long astr[3] = {(unsigned long long)C, (unsigned long long)SW * C, (unsigned long long)SH * SW * C};
+  // a row run's box holds all of its taps' rows
+  unsigned abox[4] = {(unsigned)TC_BK, (unsigned)TW, (unsigned)(rows ? TH + p.run - 1 : TH), (unsigned)TN};
+  unsigned long long bdims[3] = {(unsigned long long)C, (unsigned long long)Kw, (unsigned long long)ntaps_w};
+  unsigned long long bstr[2] = {(unsigned long long)C, (unsigned long long)Kw * C};
   unsigned bbox[3] = {(unsigned)TC_BK, (unsigned)(stacked ? stk_rows : BNsel), 1u};
   int rc;
   if ((rc = make_map(&mah, xh, 4, adims, astr, abox))) return rc;
   if ((rc = make_map(&mbh, wh, 3, bdims, bstr, bbox))) return rc;
   if ((rc = make_map(&mal, xl, 4, adims, astr, abox))) return rc;
   if ((rc = make_map(&mbl, wl, 3, bdims, bstr, bbox))) return rc;
+  if (rows) return launch_tc_rows_bn(BNsel, stacked, stk_rows, mah, mal, mbh, mbl, p, grid, rows_smem, stream);
   if (p.ksplit > 1) OG_CHECK(og_work_alloc(&p.work, (size_t)p.ksplit * p.work_plane, stream));
   rc = launch_tc_bn(BNsel, stacked, stk_rows, mah, mal, mbh, mbl, p, grid, stream);
   if (p.ksplit > 1) {
