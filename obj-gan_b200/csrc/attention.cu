@@ -221,7 +221,8 @@ OG_API int og_att_general_fwd(const float* h, const float* src, const unsigned c
   OG_RETURN_LAST_ERROR();
 }
 
-// backward: g_h [B][Q][cs], g_src [B][idf][L] (accumulated atomically; zeroed by the launcher).
+// backward: g_h [B][Q][cs]; g_src: the CTA's contribution to the image's [idf][L] gradient goes to plane blockIdx.x of
+// [gridDim.x][B][idf][L], which the launcher adds in a fixed order (og_split_sum).
 // The attention map is an output the networks only visualise, so no gradient flows into it.
 __global__ void __launch_bounds__(ATT_Q) att_general_bwd_kernel(const float* __restrict__ h,
                                                                 const float* __restrict__ src,
@@ -290,7 +291,7 @@ __global__ void __launch_bounds__(ATT_Q) att_general_bwd_kernel(const float* __r
     float acc = 0.f;
     for (int r = 0; r < ATT_Q; ++r)
       acc = fmaf(th[r * pitch + c], sG[r * L + l], fmaf(tg[r * pitch + c], sA[r * L + l], acc));
-    atomicAdd(g_src + (long long)b * idf * L + i, acc);
+    g_src[((long long)blockIdx.x * B + b) * idf * L + i] = acc;
   }
   __syncthreads();
   if (t < nq) {
@@ -313,7 +314,8 @@ __global__ void __launch_bounds__(ATT_Q) att_general_bwd_kernel(const float* __r
 // Backward for L <= 20 (the hot path): same arithmetic as above with the forward kernel's register blocking --
 // word-projection rows of 20 floats read with broadcast LDS.128, paired FMAs, no `l < L` predicates (rows are zero
 // padded).  Phases: (A) gA = g_wc . src, softmax backward -> gS in registers; (C) the block's contribution to g_src
-// ([48 c x 2 halves of 10 words] threads, reduction over the block's 128 queries from shared memory); (B) g_h rows.
+// ([48 c x 2 halves of 10 words] threads, reduction over the block's 128 queries from shared memory), stored to plane
+// blockIdx.x as above; (B) g_h rows.
 __global__ void __launch_bounds__(ATT_Q, 3)
 att_general_bwd20_kernel(const float* __restrict__ h, const float* __restrict__ src, const float* __restrict__ attn,
                          const float* __restrict__ g_wc, int B, int Q, int idf, int cs, int L,
@@ -395,12 +397,12 @@ att_general_bwd20_kernel(const float* __restrict__ h, const float* __restrict__ 
 #pragma unroll
       for (int k = 0; k < 5; ++k) acc[k] = ffma2(h2, pg[k], ffma2(g2, pa[k], acc[k]));
     }
-    float* dst = g_src + ((long long)b * idf + c) * L;
+    float* dst = g_src + (((long long)blockIdx.x * B + b) * idf + c) * L;
 #pragma unroll
     for (int k = 0; k < 5; ++k) {
       const int l = 10 * half + 2 * k;
-      if (l < L) atomicAdd(dst + l, acc[k].x);
-      if (l + 1 < L) atomicAdd(dst + l + 1, acc[k].y);
+      if (l < L) dst[l] = acc[k].x;
+      if (l + 1 < L) dst[l + 1] = acc[k].y;
     }
   }
   __syncthreads();
@@ -433,28 +435,34 @@ extern "C" int og_att_general_bwd_tc(const float* h, const float* src, const flo
 OG_API int og_att_general_bwd(const float* h, const float* src, const float* attn, const float* g_wc, int B, int Q,
                               int idf, int cs, int L, float* g_h, float* g_src, cudaStream_t stream) {
   if (L > LMAX || cs % 4 || idf > cs) return (int)cudaErrorInvalidValue;
-  OG_CHECK(cudaMemsetAsync(g_src, 0, sizeof(float) * (size_t)B * idf * L, stream));
-  if (B == 0 || Q == 0) return 0;
+  if (B == 0 || Q == 0) return (int)cudaMemsetAsync(g_src, 0, sizeof(float) * (size_t)B * idf * L, stream);
   if (Q >= 4096) {
     const int rc = og_att_general_bwd_tc(h, src, attn, g_wc, B, Q, idf, cs, L, g_h, g_src, stream);
     if (rc >= 0) return rc;
   }
-  if (L <= 20 && idf <= 64) {
-    const size_t sm20 = sizeof(float) * ((size_t)idf * 20 + 2 * ATT_Q * 20 + 2 * (size_t)ATT_Q * (cs + 1));
-    static size_t configured20 = 0;
-    if (sm20 > configured20) {
-      OG_CHECK(cudaFuncSetAttribute(att_general_bwd20_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm20));
-      configured20 = sm20;
-    }
-    dim3 grid20(og_cdiv(Q, ATT_Q), B);
-    att_general_bwd20_kernel<<<grid20, ATT_Q, sm20, stream>>>(h, src, attn, g_wc, B, Q, idf, cs, L, g_h, g_src);
-    OG_RETURN_LAST_ERROR();
+  const bool k20 = L <= 20 && idf <= 64;
+  const size_t sm20 = sizeof(float) * ((size_t)idf * 20 + 2 * ATT_Q * 20 + 2 * (size_t)ATT_Q * (cs + 1));
+  const size_t sm = sizeof(float) * (2 * ATT_Q * (cs + 1) + 2 * ATT_Q * L + idf * L);
+  static size_t configured20 = 0;
+  if (k20 && sm20 > configured20) {
+    OG_CHECK(cudaFuncSetAttribute(att_general_bwd20_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm20));
+    configured20 = sm20;
   }
-  size_t sm = sizeof(float) * (2 * ATT_Q * (cs + 1) + 2 * ATT_Q * L + idf * L);
-  OG_CHECK(cudaFuncSetAttribute(att_general_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-  dim3 grid(og_cdiv(Q, ATT_Q), B);
-  att_general_bwd_kernel<<<grid, ATT_Q, sm, stream>>>(h, src, attn, g_wc, B, Q, idf, cs, L, g_h, g_src);
-  OG_RETURN_LAST_ERROR();
+  if (!k20) OG_CHECK(cudaFuncSetAttribute(att_general_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  const dim3 grid(og_cdiv(Q, ATT_Q), B);
+  float* work = g_src;                   // one CTA per image: its plane is g_src itself
+  if (grid.x > 1) OG_CHECK(og_work_alloc(&work, (size_t)grid.x * B * idf * L, stream));
+  if (k20)
+    att_general_bwd20_kernel<<<grid, ATT_Q, sm20, stream>>>(h, src, attn, g_wc, B, Q, idf, cs, L, g_h, work);
+  else
+    att_general_bwd_kernel<<<grid, ATT_Q, sm, stream>>>(h, src, attn, g_wc, B, Q, idf, cs, L, g_h, work);
+  int rc = (int)cudaGetLastError();
+  if (grid.x > 1) {
+    if (!rc) rc = og_split_sum(work, (long long)B * idf * L, (int)grid.x, g_src, stream);
+    const cudaError_t e = cudaFreeAsync(work, stream);
+    if (!rc) rc = (int)e;
+  }
+  return rc;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -36,9 +36,10 @@ static inline int og_grid(long long total, int per_sm = 32) {
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 
-// Stream-ordered scratch memory (also valid inside CUDA graph capture).  The device's default pool keeps what is
-// freed for the next call instead of returning it to the driver at every synchronisation.
-static inline cudaError_t og_work_alloc(float** p, size_t elems, cudaStream_t stream) {
+// Stream-ordered scratch memory for elems values of type T (also valid inside CUDA graph capture).  The device's
+// default pool keeps what is freed for the next call instead of returning it to the driver at every synchronisation.
+template <typename T>
+static inline cudaError_t og_work_alloc(T** p, size_t elems, cudaStream_t stream) {
   static bool pool_ready = false;
   if (!pool_ready) {
     int dev = 0;
@@ -50,7 +51,7 @@ static inline cudaError_t og_work_alloc(float** p, size_t elems, cudaStream_t st
     }
     pool_ready = true;
   }
-  return cudaMallocAsync(reinterpret_cast<void**>(p), elems * sizeof(float), stream);
+  return cudaMallocAsync(reinterpret_cast<void**>(p), elems * sizeof(T), stream);
 }
 
 // Deterministic split reductions: the S CTAs that share an output write their partial sums to S planes of a
@@ -91,6 +92,47 @@ __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
+}
+
+// The fp64 per-channel reductions (normalisation statistics and their backward, bias gradients) split the pixels over
+// the CTAs of grid row blockIdx.y; each CTA stores its sums to plane blockIdx.y of a workspace, and og_plane_sum adds
+// the planes in a fixed order, so the totals do not depend on which CTA finishes first.
+//
+// A (32, 8) block: thread (x, y) holds the partials acc[k] of channel quad q = blockIdx.x * 32 + x over its rows.  Entry
+// k belongs to component (k & 7) >> 2 of channel (k >> 3) * Co + 4 q + (k & 3): NV = 4 is one component per channel, 8
+// two, 16 two for each half of a GLU pair (Co apart).  The 8 rows are added in the order y = 0 .. 7 and the sums of the
+// quads q < Co4 stored to plane[component * C + channel], so the plane is written in full for the block's channels and
+// needs no zeroing.  Every thread of the block must call it.
+template <int NV>
+__device__ __forceinline__ void og_cta_channel_sums(const double (&acc)[NV], int Co4, int Co, int C, double* plane) {
+  __shared__ double sh[8][32][NV];
+#pragma unroll
+  for (int i = 0; i < NV; ++i) sh[threadIdx.y][threadIdx.x][i] = acc[i];
+  __syncthreads();
+  for (int item = threadIdx.y * 32 + threadIdx.x; item < 32 * NV; item += 256) {
+    const int cx = item / NV, k = item % NV;
+    double a = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) a += sh[j][cx][k];
+    const int q = blockIdx.x * 32 + cx;
+    if (q < Co4) plane[((k & 7) >> 2) * C + (k >> 3) * Co + q * 4 + (k & 3)] = a;
+  }
+}
+
+// sum[k] = sum_s p[s * stride + k * off] over S planes, for K components, taken by a whole warp: lane l adds the planes
+// l, l + 32, ... in that order and warp_sum_d's shuffle tree adds the lanes, so every lane returns the same totals on
+// every run.  A split can have ~1000 planes (a train-mode BatchNorm over 64 channels on an H100), too many for one
+// thread to walk; the unrolled loop keeps 8 K loads of each lane in flight.
+template <int K>
+__device__ __forceinline__ void og_plane_sum(const double* __restrict__ p, long long off, int S, long long stride,
+                                             double (&sum)[K]) {
+  double a[K] = {};
+#pragma unroll 8
+  for (int s = threadIdx.x & 31; s < S; s += 32)
+#pragma unroll
+    for (int k = 0; k < K; ++k) a[k] += p[s * stride + k * off];
+#pragma unroll
+  for (int k = 0; k < K; ++k) sum[k] = warp_sum_d(a[k]);
 }
 
 // Per-tensor power-of-two scaling of the fp16 tensor-core operands: amax_bits = float bits of max|x| over the tensor;

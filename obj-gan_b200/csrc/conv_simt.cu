@@ -225,7 +225,7 @@ struct WgradArgs {
   const float* g;  // output gradient NHWC, K channels
   int OH, OW, K;
   long long gsn, gsh, gsw;
-  float* dw;  // packed [(KH*KW*C)][K], accumulated with atomicAdd
+  float* dw;  // packed [(KH*KW*C)][K]: written by the one split, else the sum of the work planes (og_split_sum)
   int KH, KW, stride, pad, mode;
   int pix_per_split;  // multiple of 8
   float* work;       // pixel splits: split z writes its partial dw to work + z * R * K (null: one split, into dw)

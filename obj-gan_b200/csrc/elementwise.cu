@@ -85,10 +85,11 @@ OG_API int og_act_backward(const float* out, const float* g, long long n, int ac
 }
 
 // ---------------------------------------------------------------------------------------------
-// per-channel sum over pixels (conv bias gradient).  fp64 partials, one atomic per (block, channel).
+// per-channel sum over pixels (conv bias gradient).  fp64 partials: each CTA stores its sums to plane blockIdx.y of a
+// [chunks][C] workspace, and store_sum_kernel adds the planes in a fixed order.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) channel_sum_kernel(const float* __restrict__ x, int C, long long P,
-                                                          int pix_per_block, double* __restrict__ acc) {
+                                                          int pix_per_block, double* __restrict__ part) {
   const int c4 = blockIdx.x * 32 + threadIdx.x;
   const int C4 = C >> 2;
   const long long p0 = (long long)blockIdx.y * pix_per_block, p1 = min(P, p0 + pix_per_block);
@@ -98,36 +99,36 @@ __global__ void __launch_bounds__(256) channel_sum_kernel(const float* __restric
       float4 v = ldg4(x + p * C + c4 * 4);
       s[0] += v.x; s[1] += v.y; s[2] += v.z; s[3] += v.w;
     }
-  __shared__ double sh[8][32][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) sh[threadIdx.y][threadIdx.x][i] = s[i];
-  __syncthreads();
-  const int t = threadIdx.y * 32 + threadIdx.x;
-  if (t < 128) {
-    int cx = t >> 2, k = t & 3;
-    double a = 0;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) a += sh[j][cx][k];
-    int cc4 = blockIdx.x * 32 + cx;
-    if (cc4 < C4) atomicAdd(&acc[cc4 * 4 + k], a);
-  }
+  og_cta_channel_sums(s, C4, C, C, part + (long long)blockIdx.y * C);
 }
-__global__ void store_sum_kernel(const double* __restrict__ acc, int n, float* out, int accumulate) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = accumulate ? out[i] + (float)acc[i] : (float)acc[i];
+// one warp per channel: acc[c] = the fp64 sum, out[c] (c < n_out) = it rounded to fp32 (added to out[c] when accumulating)
+__global__ void store_sum_kernel(const double* __restrict__ part, int S, int C, double* __restrict__ acc, int n_out,
+                                 float* out, int accumulate) {
+  const int i = (int)((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5);
+  if (i >= C) return;
+  double a[1];
+  og_plane_sum(part + i, 0, S, C, a);
+  if (threadIdx.x & 31) return;
+  acc[i] = a[0];
+  if (i < n_out) out[i] = accumulate ? out[i] + (float)a[0] : (float)a[0];
 }
 OG_API int og_channel_sum(const float* x, long long P, int C, double* scratch, float* out, int n_out, int accumulate,
                           cudaStream_t stream) {
   if (C % 4) return (int)cudaErrorInvalidValue;
-  OG_CHECK(cudaMemsetAsync(scratch, 0, sizeof(double) * C, stream));
   int cg = og_cdiv(C / 4, 32);
   long long chunks = (long long)og_num_sms() * 8 / cg + 1;
   long long ppb = (P + chunks - 1) / chunks;
   if (ppb < 64) ppb = 64;
   dim3 grid(cg, og_cdiv(P, ppb)), block(32, 8);
-  if (P > 0) channel_sum_kernel<<<grid, block, 0, stream>>>(x, C, P, (int)ppb, scratch);
-  store_sum_kernel<<<og_cdiv(n_out, 256), 256, 0, stream>>>(scratch, n_out, out, accumulate);
-  OG_RETURN_LAST_ERROR();
+  double* part = nullptr;
+  if (P > 0) {
+    OG_CHECK(og_work_alloc(&part, (size_t)grid.y * C, stream));
+    channel_sum_kernel<<<grid, block, 0, stream>>>(x, C, P, (int)ppb, part);
+  }
+  store_sum_kernel<<<og_cdiv(C, 8), 256, 0, stream>>>(part, (int)grid.y, C, scratch, n_out, out, accumulate);
+  const int rc = (int)cudaGetLastError();
+  const cudaError_t e = part ? cudaFreeAsync(part, stream) : cudaSuccess;
+  return rc ? rc : (int)e;
 }
 
 // ---------------------------------------------------------------------------------------------

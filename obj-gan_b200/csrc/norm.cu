@@ -18,8 +18,9 @@
 // A thread owns one channel quad and walks the rows p0 + ty, p0 + ty + 8, ...: four rows are loaded back to back (four
 // 16-byte loads in flight), summed pairwise in fp32 (<= 2 roundings: ~1e-7 relative, random) and only the 4-row partial
 // enters the fp64 accumulators -- a quarter of the F2F / DADD / DFMA issue slots of per-element fp64.
+// The CTA's (sum, sum of squares) go to plane blockIdx.y of part: [chunks][groups][2][C] doubles.
 __global__ void __launch_bounds__(256) norm_stats_kernel(const float* __restrict__ x, int C, long long P,
-                                                         int pix_per_block, double* __restrict__ stats) {
+                                                         int pix_per_block, double* __restrict__ part) {
   const int c4 = blockIdx.x * 32 + threadIdx.x;
   const int C4 = C >> 2;
   const long long g = blockIdx.z;
@@ -45,43 +46,34 @@ __global__ void __launch_bounds__(256) norm_stats_kernel(const float* __restrict
       s[3] += v.w; q[3] += (double)v.w * v.w;
     }
   }
-  __shared__ double sh[8][32][8];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    sh[threadIdx.y][threadIdx.x][i] = s[i];
-    sh[threadIdx.y][threadIdx.x][4 + i] = q[i];
-  }
-  __syncthreads();
-  // 256 threads reduce 32 x 8 values over the 8 pixel lanes
-  const int t = threadIdx.y * 32 + threadIdx.x;
-  const int cx = t >> 3, k = t & 7;
-  double acc = 0;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) acc += sh[j][cx][k];
-  const int cc4 = blockIdx.x * 32 + cx;
-  if (cc4 < C4) {
-    int ch = cc4 * 4 + (k & 3);
-    atomicAdd(&stats[(g * C + ch) * 2 + (k >> 2)], acc);
-  }
+  const double acc[8] = {s[0], s[1], s[2], s[3], q[0], q[1], q[2], q[3]};
+  og_cta_channel_sums(acc, C4, C, C, part + ((long long)blockIdx.y * gridDim.z + g) * 2 * C);
 }
 
-// mean / rstd from (sum, sumsq); optional BatchNorm running-stat update.
+// mean / rstd from (sum, sumsq), the planes of norm_stats_kernel added by og_plane_sum (one warp per (group, channel));
+// optional BatchNorm running-stat update.
 // The one-pass variance sumsq / count - mean^2 carries the rounding of the fp32 squares in the 4-row pre-sum: an error of
 // up to ~3 * 2^-24 * sumsq / count.  Where that could exceed 2^-10 of var + eps -- a large offset over a small spread, or
 // a constant channel (a dead filter plus its bias), which would get var = O(2^-24 mean^2) instead of 0 and an rstd far
 // below 1 / sqrt(eps), wrong by the same factor in the input gradient -- the channel is marked for
 // norm_stats_exact_kernel (stats[2 i] = 1, else 0), which recomputes it from shifted fp64 sums and does its running-stat
-// update.  Every other channel keeps the one-pass result.
+// update.  Every other channel keeps the one-pass result.  stats[2 i + 1] = sumsq.
 constexpr double OG_NORM_CANCEL = 1024.0;
-__global__ void norm_finalize_kernel(double* __restrict__ stats, int groups, int C, double count, float eps,
-                                     float* __restrict__ mean, float* __restrict__ rstd, float* running_mean,
-                                     float* running_var, float momentum, int real_c,
-                                     long long* num_batches_tracked) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
+__global__ void norm_finalize_kernel(const double* __restrict__ part, int S, double* __restrict__ stats, int groups,
+                                     int C, double count, float eps, float* __restrict__ mean,
+                                     float* __restrict__ rstd, float* running_mean, float* running_var,
+                                     float momentum, int real_c, long long* num_batches_tracked) {
+  const int i = (int)((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5);
   if (i >= groups * C) return;
+  const int g = i / C;
+  const double* p = part + (long long)g * 2 * C + (i - g * C);
+  double t[2];                                          // sum, sum of squares
+  og_plane_sum(p, C, S, 2LL * groups * C, t);
+  if (threadIdx.x & 31) return;
   if (i == 0 && num_batches_tracked) *num_batches_tracked += 1;
-  double m = stats[i * 2] / count;
-  const double ms = stats[i * 2 + 1] / count;
+  stats[i * 2 + 1] = t[1];
+  double m = t[0] / count;
+  const double ms = t[1] / count;
   double var = ms - m * m;
   if (var < 0) var = 0;
   const bool redo = ms > OG_NORM_CANCEL * (var + (double)eps);
@@ -263,7 +255,8 @@ __device__ __forceinline__ void act_grad4(const ChanConst& k, const float4& v, c
   }
 }
 
-// backward reduce: per (group, channel of y):  bstats[.,0] = sum dn,  bstats[.,1] = sum dn * xhat   (fp64)
+// backward reduce: per (group, channel of y) the CTA's sum dn and sum dn * xhat (fp64), stored to plane blockIdx.y of
+// part: [chunks][groups][2][Cy] doubles.
 // grid: (ceil(Co4/32), chunks, groups)  block (32, 8).  Two rows per trip: their contributions are added in fp32 and the
 // pair enters the fp64 accumulators (half of the fp64 issue slots; the pair sum costs one fp32 rounding).
 template <int ACT>
@@ -273,7 +266,7 @@ __global__ void __launch_bounds__(256) norm_bwd_reduce_kernel(const float* __res
                                                               const float* __restrict__ rstd,
                                                               const float* __restrict__ gamma,
                                                               const float* __restrict__ beta, float slope,
-                                                              double* __restrict__ bstats) {
+                                                              double* __restrict__ part) {
   const int Co = (ACT == OG_NA_GLU) ? Cy / 2 : Cy;
   const int Co4 = Co >> 2;
   const int c4 = blockIdx.x * 32 + threadIdx.x;
@@ -326,24 +319,7 @@ __global__ void __launch_bounds__(256) norm_bwd_reduce_kernel(const float* __res
       }
     }
   }
-  __shared__ double sh[8][32][NV];
-#pragma unroll
-  for (int i = 0; i < NV; ++i) sh[threadIdx.y][threadIdx.x][i] = acc[i];
-  __syncthreads();
-  const int t = threadIdx.y * 32 + threadIdx.x;
-  for (int item = t; item < 32 * NV; item += 256) {
-    int cx = item / NV, k = item % NV;
-    double a = 0;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) a += sh[j][cx][k];
-    int cc4 = blockIdx.x * 32 + cx;
-    if (cc4 < Co4) {
-      int half = k >> 3;            // 0: "a" half, 1: gate half (GLU only)
-      int kk = k & 7;
-      int ch = half * Co + cc4 * 4 + (kk & 3);
-      atomicAdd(&bstats[(grp * Cy + ch) * 2 + (kk >> 2)], a);
-    }
-  }
+  og_cta_channel_sums(acc, Co4, Co, Cy, part + ((long long)blockIdx.y * gridDim.z + grp) * 2 * Cy);
 }
 
 // backward apply: dy = rstd * gamma * (dn - S1/cnt - xhat * S2/cnt).  Same thread mapping as the forward apply: the
@@ -368,8 +344,8 @@ __global__ void __launch_bounds__(256) norm_bwd_apply_kernel(const float* __rest
     const int c = c4 * 4;
     ChanConst k;
     load_chan<ACT>(k, mean, rstd, gamma, beta, grp, Cy, Co, c);
-    // coef[(grp * Cy + ch) * 4 + {0, 1}] = (float)(S1 / count), (float)(S2 / count): written over the fp64 sums by
-    // norm_bwd_coef_kernel (same float values the per-element double products gave)
+    // coef[(grp * Cy + ch) * 4 + {0, 1}] = (float)(S1 / count), (float)(S2 / count): written by norm_bwd_sums_kernel
+    // (same float values the per-element double products gave)
     const float* coef = reinterpret_cast<const float*>(bstats);
     const float* bs = coef + (grp * Cy + c) * 4;
     const float2 k0 = *reinterpret_cast<const float2*>(bs), k1 = *reinterpret_cast<const float2*>(bs + 4);
@@ -411,23 +387,28 @@ __global__ void __launch_bounds__(256) norm_bwd_apply_kernel(const float* __rest
   if (amax) block_amax_256(mx, amax);
 }
 
-// (S1, S2) fp64 -> ((float)(S1 / count), (float)(S2 / count)) stored over the first 8 bytes of the same 16-byte slot
-__global__ void norm_bwd_coef_kernel(double* __restrict__ bstats, long long n, double inv_count) {
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const double s1 = bstats[i * 2], s2 = bstats[i * 2 + 1];
-  float2 k = make_float2((float)(s1 * inv_count), (float)(s2 * inv_count));
-  *reinterpret_cast<float2*>(bstats + i * 2) = k;
-}
-
-// dgamma = S2, dbeta = S1 for batch norm (groups == 1): copy fp64 sums to fp32 parameter-gradient vectors
-__global__ void norm_param_grad_kernel(const double* __restrict__ bstats, int C, float* dgamma, float* dbeta,
-                                       int accumulate) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= C) return;
-  float db = (float)bstats[i * 2], dg = (float)bstats[i * 2 + 1];
-  dgamma[i] = accumulate ? dgamma[i] + dg : dg;
-  dbeta[i] = accumulate ? dbeta[i] + db : db;
+// (S1, S2) = (sum dn, sum dn * xhat) of each (group, channel of y): the planes [S][groups][2][Cy] of
+// norm_bwd_reduce_kernel or bn_eval_bwd_kernel added by og_plane_sum, one warp each.  bstats (optional): slot i gets
+// ((float)(S1 / count), (float)(S2 / count)) in its first 8 bytes and S2 in the second.  dgamma / dbeta (optional,
+// groups == 1): the BatchNorm parameter gradients S2 / S1, added to them when accumulating.
+__global__ void norm_bwd_sums_kernel(const double* __restrict__ part, int S, int groups, int Cy, double inv_count,
+                                     double* __restrict__ bstats, float* dgamma, float* dbeta, int accumulate) {
+  const int i = (int)((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5);
+  if (i >= groups * Cy) return;
+  const int grp = i / Cy;
+  const double* p = part + (long long)grp * 2 * Cy + (i - grp * Cy);
+  double t[2];                                          // S1, S2
+  og_plane_sum(p, Cy, S, 2LL * groups * Cy, t);
+  if (threadIdx.x & 31) return;
+  if (bstats) {
+    *reinterpret_cast<float2*>(bstats + i * 2) = make_float2((float)(t[0] * inv_count), (float)(t[1] * inv_count));
+    bstats[i * 2 + 1] = t[1];
+  }
+  if (dgamma) {
+    const float db = (float)t[0], dg = (float)t[1];
+    dgamma[i] = accumulate ? dgamma[i] + dg : dg;
+    dbeta[i] = accumulate ? dbeta[i] + db : db;
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -534,9 +515,8 @@ __global__ void bn_eval_coef_kernel(const float* __restrict__ running_mean, cons
 
 // Backward of the fixed affine + activation: dy = dn * gamma * rstd, with no batch-statistic terms.  Same thread mapping
 // as norm_bwd_apply_kernel (grid (ceil(Co4/32), chunks), block (32, 8)).  When part is non-null, the CTA's per-channel
-// sums (sum dn, sum dn * xhat) are reduced inside the CTA in a fixed order (fp64) and stored to plane blockIdx.y of
-// part ([chunks][2][Cy] doubles); bn_eval_param_grad_kernel adds the planes in a fixed order -- no atomics, so the
-// parameter gradients are the same on every run.
+// sums (sum dn, sum dn * xhat; fp64) are stored to plane blockIdx.y of part ([chunks][2][Cy] doubles) for
+// norm_bwd_sums_kernel.
 template <int ACT>
 __global__ void __launch_bounds__(256) bn_eval_bwd_kernel(const float* __restrict__ y, const float* __restrict__ g,
                                                           int Cy, long long P, int pix_per_block,
@@ -590,39 +570,7 @@ __global__ void __launch_bounds__(256) bn_eval_bwd_kernel(const float* __restric
     }
   }
   if (amax) block_amax_256(mx, amax);
-  if (!part) return;
-  __shared__ double sh[8][32][NV];
-#pragma unroll
-  for (int i = 0; i < NV; ++i) sh[threadIdx.y][threadIdx.x][i] = acc[i];
-  __syncthreads();
-  const int t = threadIdx.y * 32 + threadIdx.x;
-  double* plane = part + (long long)blockIdx.y * 2 * Cy;
-  for (int item = t; item < 32 * NV; item += 256) {
-    const int cx = item / NV, kk = item % NV;
-    double a = 0;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) a += sh[j][cx][kk];
-    const int cc4 = blockIdx.x * 32 + cx;
-    if (cc4 < Co4) {
-      const int half = kk >> 3;              // 0: "a" half, 1: gate half (GLU only)
-      const int ch = half * Co + cc4 * 4 + (kk & 3);
-      plane[((kk & 7) >> 2) * Cy + ch] = a;  // [0][ch] = sum dn, [1][ch] = sum dn * xhat
-    }
-  }
-}
-
-// dbeta = sum_s part[s][0][c], dgamma = sum_s part[s][1][c], planes added in the order s = 0, 1, ...
-__global__ void bn_eval_param_grad_kernel(const double* __restrict__ part, int S, int C, float* dgamma, float* dbeta,
-                                          int accumulate) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= C) return;
-  double sb = 0, sg = 0;
-  for (int s = 0; s < S; ++s) {
-    sb += part[(long long)s * 2 * C + i];
-    sg += part[(long long)s * 2 * C + C + i];
-  }
-  dgamma[i] = accumulate ? dgamma[i] + (float)sg : (float)sg;
-  dbeta[i] = accumulate ? dbeta[i] + (float)sb : (float)sb;
+  if (part) og_cta_channel_sums(acc, Co4, Co, Cy, part + (long long)blockIdx.y * 2 * Cy);
 }
 
 static int pix_chunk(long long P, int cgroups, int groups) {
@@ -634,22 +582,26 @@ static int pix_chunk(long long P, int cgroups, int groups) {
   return (int)ppb;
 }
 
-// stats: fp64 [groups][C][2] (zeroed here); mean/rstd: fp32 [groups][C]
+// stats: fp64 [groups][C][2] (recompute mark, sum of squares); mean/rstd: fp32 [groups][C]
 OG_API int og_norm_stats(const float* x, int groups, long long P, int C, float eps, double* stats, float* mean,
                          float* rstd, float* running_mean, float* running_var, float momentum, int real_c,
                          long long* num_batches_tracked, cudaStream_t stream) {
   if (C % 4) return (int)cudaErrorInvalidValue;
-  OG_CHECK(cudaMemsetAsync(stats, 0, sizeof(double) * 2 * groups * C, stream));
   int cg = og_cdiv(C / 4, 32);
   int ppb = pix_chunk(P, cg, groups);
   dim3 grid(cg, og_cdiv(P, ppb), groups), block(32, 8);
-  norm_stats_kernel<<<grid, block, 0, stream>>>(x, C, P, ppb, stats);
-  norm_finalize_kernel<<<og_cdiv((long long)groups * C, 256), 256, 0, stream>>>(stats, groups, C, (double)P, eps, mean, rstd,
-                                                                     running_mean, running_var, momentum, real_c,
-                                                                     num_batches_tracked);
+  double* part = nullptr;
+  OG_CHECK(og_work_alloc(&part, (size_t)grid.y * groups * 2 * C, stream));
+  norm_stats_kernel<<<grid, block, 0, stream>>>(x, C, P, ppb, part);
+  norm_finalize_kernel<<<og_cdiv((long long)groups * C, 8), 256, 0, stream>>>(part, (int)grid.y, stats, groups, C,
+                                                                              (double)P, eps, mean, rstd, running_mean,
+                                                                              running_var, momentum, real_c,
+                                                                              num_batches_tracked);
   norm_stats_exact_kernel<<<dim3(C / 4, groups), 256, 0, stream>>>(x, C, P, (double)P, eps, stats, mean, rstd,
                                                                    running_mean, running_var, momentum, real_c);
-  OG_RETURN_LAST_ERROR();
+  const int rc = (int)cudaGetLastError();
+  const cudaError_t e = cudaFreeAsync(part, stream);
+  return rc ? rc : (int)e;
 }
 
 OG_API int og_norm_apply(const float* y, int groups, long long P, int Cy, const float* mean, const float* rstd,
@@ -677,17 +629,20 @@ OG_API int og_norm_backward(const float* y, const float* g, int groups, long lon
                             unsigned* amax_dy, cudaStream_t stream) {
   int Co = act == OG_NA_GLU ? Cy / 2 : Cy;
   if (Cy % 4 || Co % 4) return (int)cudaErrorInvalidValue;
-  OG_CHECK(cudaMemsetAsync(bstats, 0, sizeof(double) * 2 * groups * Cy, stream));
   if (amax_dy) OG_CHECK(cudaMemsetAsync(amax_dy, 0, sizeof(unsigned), stream));
   int cg = og_cdiv(Co / 4, 32);
   int ppb = pix_chunk(P, cg, groups);
   dim3 grid(cg, og_cdiv(P, ppb), groups), block(32, 8);
   double inv = 1.0 / (double)P;
+  double* part = nullptr;
+  OG_CHECK(og_work_alloc(&part, (size_t)grid.y * groups * 2 * Cy, stream));
+  const int S = (int)grid.y;
+  float* dg = groups == 1 ? dgamma : nullptr;
+  float* db = groups == 1 ? dbeta : nullptr;
 #define OG_LAUNCH_BWD(A)                                                                                           \
-  norm_bwd_reduce_kernel<A><<<grid, block, 0, stream>>>(y, g, Cy, P, ppb, mean, rstd, gamma, beta, slope, bstats); \
-  if (dgamma && groups == 1)                                                                                       \
-    norm_param_grad_kernel<<<og_cdiv(Cy, 256), 256, 0, stream>>>(bstats, Cy, dgamma, dbeta, accumulate_param_grads); \
-  norm_bwd_coef_kernel<<<og_cdiv((long long)groups * Cy, 256), 256, 0, stream>>>(bstats, (long long)groups * Cy, inv); \
+  norm_bwd_reduce_kernel<A><<<grid, block, 0, stream>>>(y, g, Cy, P, ppb, mean, rstd, gamma, beta, slope, part);   \
+  norm_bwd_sums_kernel<<<og_cdiv((long long)groups * Cy, 8), 256, 0, stream>>>(part, S, groups, Cy, inv, bstats, dg, \
+                                                                               db, accumulate_param_grads);        \
   norm_bwd_apply_kernel<A><<<grid, block, 0, stream>>>(y, g, Cy, P, ppb, mean, rstd, gamma, beta, slope, bstats, dy, amax_dy);
   if (act == OG_NA_GLU) {
     OG_LAUNCH_BWD(OG_NA_GLU)
@@ -697,7 +652,9 @@ OG_API int og_norm_backward(const float* y, const float* g, int groups, long lon
     OG_LAUNCH_BWD(OG_NA_NONE)
   }
 #undef OG_LAUNCH_BWD
-  OG_RETURN_LAST_ERROR();
+  const int rc = (int)cudaGetLastError();
+  const cudaError_t e = cudaFreeAsync(part, stream);
+  return rc ? rc : (int)e;
 }
 
 // eval-mode BatchNorm: mean = running_mean, rstd = 1 / sqrt(running_var + eps) (fp32 [C]); the buffers are only read
@@ -729,11 +686,7 @@ OG_API int og_bn_eval_backward(const float* y, const float* g, long long P, int 
   const int ppb = pix_chunk(P, cg, 1);
   const dim3 grid(cg, og_cdiv(P, ppb), 1), block(32, 8);
   double* part = nullptr;
-  if (dgamma) {
-    float* w = nullptr;
-    OG_CHECK(og_work_alloc(&w, (size_t)grid.y * 2 * Cy * 2, stream));     // doubles as pairs of floats
-    part = reinterpret_cast<double*>(w);
-  }
+  if (dgamma) OG_CHECK(og_work_alloc(&part, (size_t)grid.y * 2 * Cy, stream));
   if (act == OG_NA_GLU)
     bn_eval_bwd_kernel<OG_NA_GLU><<<grid, block, 0, stream>>>(y, g, Cy, P, ppb, mean, rstd, gamma, beta, slope, dy, part, amax_dy);
   else if (act == OG_NA_LRELU)
@@ -743,8 +696,8 @@ OG_API int og_bn_eval_backward(const float* y, const float* g, long long P, int 
   int rc = (int)cudaGetLastError();
   if (part) {
     if (!rc) {
-      bn_eval_param_grad_kernel<<<og_cdiv(Cy, 256), 256, 0, stream>>>(part, (int)grid.y, Cy, dgamma, dbeta,
-                                                                     accumulate_param_grads);
+      norm_bwd_sums_kernel<<<og_cdiv(Cy, 8), 256, 0, stream>>>(part, (int)grid.y, 1, Cy, 1.0 / (double)P, nullptr,
+                                                               dgamma, dbeta, accumulate_param_grads);
       rc = (int)cudaGetLastError();
     }
     const cudaError_t e = cudaFreeAsync(part, stream);

@@ -71,10 +71,12 @@ EDGE_CASES = {
         (100, 4096, 48, 48, 18, True),
         (BWD_ONE_SLOT, 4096, 48, 48, 18, True),   # nslots == 1: g_src stored without the workspace planes
         (3, 3968, 48, 48, 18, True),           # SIMT bwd20
+        (3, 100, 48, 48, 18, True),            # ... one CTA per image: g_src stored without the workspace planes
         (3, 4160, 48, 48, 18, True),           # Q % 128 != 0: bwd20 above the Q >= 4096 gate
         (3, 1000, 48, 48, 18, False),
         (3, 1000, 48, 48, 21, True),           # the general kernel: L > 20
         (3, 1000, 48, 48, 32, True),
+        (2, 128, 48, 48, 21, True),            # ... one CTA per image
         (2, 1000, 72, 80, 18, True),           # ... idf > 64
         (2, 4096, 72, 80, 12, True),           # ... above the gate
     ],

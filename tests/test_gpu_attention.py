@@ -35,9 +35,8 @@ Inputs: rows of h and g_wc whose magnitudes spread over 2^-7 .. 2^3 inside every
 the probabilities must be exactly uniform over the unmasked words), ragged caption masks, NaN in the pad lanes of the
 inputs (never read) and in the unused roi slots of the paint masks.
 
-Determinism: the tensor-core forward, the tensor-core backward (per-CTA g_src planes added in a fixed order) and the
-paint backward (per-block planes) are called twice on the same inputs and must agree bit for bit.  The SIMT
-backward kernels accumulate g_src with atomics and are not held to that.
+Determinism: the tensor-core forward, every grid-attention backward (per-CTA g_src planes added in a fixed order) and
+the paint backward (per-block planes) are called twice on the same inputs and must agree bit for bit.
 """
 import pytest
 import torch
@@ -246,10 +245,9 @@ def _run_bwd(B, Q, idf, cs, L, mask_on, seed=0):
                                  + torch.einsum("bq,bqc->bc", ags, h64.abs())[..., None]) \
             + PFLOOR * gw64.abs().sum(1)[..., None]
     _check(f"{BWD} g_src ({tag})", g_src, ref, bound)
-    if tc:
-        g_h2, g_src2 = torch.empty_like(g_h), torch.empty_like(g_src)
-        _call(BWD, h, src, attn, g_wc, B, Q, idf, cs, L, g_h2, g_src2)
-        assert torch.equal(g_h, g_h2) and torch.equal(g_src, g_src2)
+    g_h2, g_src2 = torch.empty_like(g_h), torch.empty_like(g_src)       # per-CTA planes added in a fixed order
+    _call(BWD, h, src, attn, g_wc, B, Q, idf, cs, L, g_h2, g_src2)
+    assert torch.equal(g_h, g_h2) and torch.equal(g_src, g_src2)
 
 
 # ---------------------------------------------------------------------------------------------------

@@ -116,7 +116,8 @@ def test_bilinear(N, IH, IW, C, OH, OW):
 @pytest.mark.parametrize("P,C,n_out,acc", [(1, 8, 8, 0), (63, 24, 20, 0), (63, 132, 132, 1), (1 << 20, 16, 12, 0),
                                            (1 << 20, 96, 96, 1)])
 def test_channel_sum(P, C, n_out, acc):
-    """fp64 sums of fp32 values, rounded once to fp32 (and once more when accumulating): <= 2 U |ref| + 2^-30 sum|x|."""
+    """fp64 sums of fp32 values, rounded once to fp32 (and once more when accumulating): <= 2 U |ref| + 2^-30 sum|x|;
+    a second call gives the same bits."""
     x = _randn(P, C, seed=P % 1000 + C) + 0.5
     scratch = torch.empty(C, device=DEV, dtype=torch.float64)
     out0 = _randn(n_out, seed=9)
@@ -124,6 +125,9 @@ def test_channel_sum(P, C, n_out, acc):
     _call("og_channel_sum", x, P, C, scratch, out, n_out, acc)
     ref = x.double().sum(0)[:n_out] + (out0.double() if acc else 0)
     _within("og_channel_sum", out, ref, 2 * U * ref.abs() + 2.0 ** -30 * x.double().abs().sum(0)[:n_out] + 1e-45)
+    out2 = out0.clone()
+    _call("og_channel_sum", x, P, C, scratch, out2, n_out, acc)
+    assert torch.equal(out, out2)                     # the per-CTA sums are added in a fixed order
 
 
 @pytest.mark.parametrize("act", [ACT_LRELU, ACT_TANH, ACT_SIGMOID])
