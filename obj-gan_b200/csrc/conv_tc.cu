@@ -26,6 +26,9 @@
 #include "wgmma.cuh"
 #include <cuda_fp16.h>
 #include <stdlib.h>
+#include <iterator>
+#include <type_traits>
+#include <utility>
 
 namespace {
 
@@ -130,11 +133,11 @@ struct TcAccWide {
 // One stage's MMAs into a fresh partial sum: KS k-steps of 16, KSTEP bytes apart in the operand tiles, as ONE
 // straight-line issue window (fence, the MMAs, commit), then the wait for them.  Nothing in the window branches or
 // touches the accumulator registers; otherwise ptxas waits for every wgmma before issuing the next (C7520 / C7519 /
-// C7514 warnings).  The wait sits in here too, so that a caller choosing KS at run time (a switch) merges the
+// C7514 warnings).  The wait sits in here too, so that tc_stage_mma, which chooses KS at run time, merges the
 // accumulators only after it (C7517 otherwise).
 // al*bh, ah*bl, ah*bh (small terms first); STACKED: al*[bh_hi | bh_lo], ah*[bh_hi | bh_lo].
 template <int KS, uint32_t KSTEP, bool STACKED, class Acc>
-__device__ __forceinline__ void tc_stage_mma(Acc& part, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl) {
+__device__ __forceinline__ void tc_stage_window(Acc& part, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl) {
   wg_fence();
 #pragma unroll
   for (int k = 0; k < KS; ++k) {
@@ -153,9 +156,60 @@ __device__ __forceinline__ void tc_stage_mma(Acc& part, uint64_t ah, uint64_t al
   part.hold();
 }
 
+// One stage's MMAs with ks = 1..4 k-steps (a last channel chunk of fewer than 64 real channels skips the k-steps that
+// would multiply zeros): one issue window per count, since a window whose length is a run-time value is serialized.
+template <uint32_t KSTEP, bool STACKED, class Acc>
+__device__ __forceinline__ void tc_stage_mma(int ks, Acc& part, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl) {
+  switch (ks) {
+    case 1: tc_stage_window<1, KSTEP, STACKED>(part, ah, al, bh, bl); break;
+    case 2: tc_stage_window<2, KSTEP, STACKED>(part, ah, al, bh, bl); break;
+    case 3: tc_stage_window<3, KSTEP, STACKED>(part, ah, al, bh, bl); break;
+    default: tc_stage_window<4, KSTEP, STACKED>(part, ah, al, bh, bl); break;
+  }
+}
+
 // Warp index as a value ptxas knows to be warp-uniform (threadIdx.x >> 5 is, but the compiler cannot prove it, and
 // a role branch it takes for divergent serializes every wgmma behind it)
 __device__ __forceinline__ int tc_warp_uniform() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
+
+// Kernel prologue: thread 0 prefetches the tensor maps and initialises the barriers of the operand ring (full: the
+// producer's arrival with its TMA bytes; empty: one arrival per consumer warp) for the whole CTA.  Returns the dynamic
+// shared memory aligned to 1024 bytes, the atom of the 128-byte swizzle.
+template <class... Maps>
+__device__ __forceinline__ uint8_t* tc_prologue(uint8_t* smem_raw, uint64_t* full, uint64_t* empty, int stages,
+                                                const Maps&... maps) {
+  if (threadIdx.x == 0) {
+    (prefetch_tmap(&maps), ...);
+    for (int s = 0; s < stages; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], TC_CONSUMER_WARPS);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+}
+
+// Steps a walk through a ring of depth pipeline slots to the next slot; the barrier parity flips at each wrap
+__device__ __forceinline__ void tc_ring_next(int& stage, uint32_t& phase, int depth) {
+  if (++stage == depth) {
+    stage = 0;
+    phase ^= 1;
+  }
+}
+
+// Origin (image, row, column) of this CTA's TN x TH x TW output patch; blockIdx.x walks the patches w fastest.
+// ONE_IMAGE: TN == 1.
+struct TcTile { int n0, h0, w0; };
+template <bool ONE_IMAGE = false>
+__device__ __forceinline__ TcTile tc_tile_origin(const TcParams& p) {
+  int t = blockIdx.x;
+  const int tw_i = t % p.tiles_w;
+  t /= p.tiles_w;
+  const int th_i = t % p.tiles_h;
+  const int tn_i = t / p.tiles_h;
+  return {ONE_IMAGE ? tn_i : tn_i * p.TN, th_i * p.TH, tw_i * p.TW};
+}
 
 // ===================== epilogue: registers -> global (consumer warpgroup cg = (warp >> 2) - 1) =====================
 template <int BN, bool STACKED>
@@ -210,17 +264,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
   constexpr uint32_t B_BYTES = BN * 128;            // BN % 8 == 0: a whole number of 1024-byte swizzle atoms
   constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + (STACKED ? 1 : 2) * B_BYTES;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
   const int warp = tc_warp_uniform(), lane = threadIdx.x & 31;
-  // tile coordinates
-  int t = blockIdx.x;
-  const int tw_i = t % p.tiles_w;
-  t /= p.tiles_w;
-  const int th_i = t % p.tiles_h;
-  const int tn_i = t / p.tiles_h;
-  const int n0 = tn_i * p.TN, h0 = th_i * p.TH, w0 = tw_i * p.TW;
+  const auto [n0, h0, w0] = tc_tile_origin(p);
   const int col0 = blockIdx.y * (STACKED ? BN / 2 : BN);
   const int nk_total = p.taps.n * p.cchunks;
   const int per_split = (nk_total + p.ksplit - 1) / p.ksplit;
@@ -228,18 +275,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
   const int nk = min(nk_total, it_beg + per_split) - it_beg;
   if (nk <= 0) return;
 
-  if (threadIdx.x == 0) {
-    prefetch_tmap(&map_ah);
-    prefetch_tmap(&map_bh);
-    prefetch_tmap(&map_al);
-    prefetch_tmap(&map_bl);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], TC_CONSUMER_WARPS);
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
+  uint8_t* const smem = tc_prologue(smem_raw, full_bar, empty_bar, STAGES, map_ah, map_bh, map_al, map_bl);
 
   if (warp < 4) {
     // ===================== TMA producer =====================
@@ -248,20 +284,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
       uint32_t phase = 0;
       for (int it = 0; it < nk; ++it) {
         const int tap = (it_beg + it) / p.cchunks, cc = (it_beg + it) - tap * p.cchunks;
+        uint64_t* const full = &full_bar[stage];
         mbar_wait(&empty_bar[stage], phase ^ 1);
         uint8_t* sa = smem + (size_t)stage * STAGE_BYTES;
-        mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
+        mbar_expect_tx(full, STAGE_BYTES);
         const int c0 = cc * TC_BK, ws = w0 + p.taps.dw[tap], hs = h0 + p.taps.dh[tap], widx = p.taps.widx[tap];
         const int ns = n0 + p.taps.dn[tap];   // image offset: selects a space-to-depth phase block of the source
-        tma_load_4d(sa, &map_ah, &full_bar[stage], c0, ws, hs, ns);
-        tma_load_3d(sa + 2 * A_BYTES, &map_bh, &full_bar[stage], c0, col0, widx);
-        tma_load_4d(sa + A_BYTES, &map_al, &full_bar[stage], c0, ws, hs, ns);
+        tma_load_4d(sa, &map_ah, full, c0, ws, hs, ns);
+        tma_load_3d(sa + 2 * A_BYTES, &map_bh, full, c0, col0, widx);
+        tma_load_4d(sa + A_BYTES, &map_al, full, c0, ws, hs, ns);
         // stacked: the lo rows follow the hi rows inside the same N extent (maps with a box of BN / 2 rows)
-        tma_load_3d(sa + 2 * A_BYTES + (STACKED ? B_BYTES / 2 : B_BYTES), &map_bl, &full_bar[stage], c0, col0, widx);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
+        tma_load_3d(sa + 2 * A_BYTES + (STACKED ? B_BYTES / 2 : B_BYTES), &map_bl, full, c0, col0, widx);
+        tc_ring_next(stage, phase, STAGES);
       }
     }
     return;
@@ -274,30 +308,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
   // partial sum, which is then added into the register accumulator with round-to-nearest fp32 adds.
   TcAccWide<BN> acc, part;
   acc.zero();
-  {
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int it = 0; it < nk; ++it) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_u32(smem + (size_t)stage * STAGE_BYTES);
-      const uint64_t ah = wg_desc_k(sa + cg * 64 * 128), al = wg_desc_k(sa + A_BYTES + cg * 64 * 128);
-      const uint64_t bh = wg_desc_k(sa + 2 * A_BYTES), bl = wg_desc_k(sa + 2 * A_BYTES + B_BYTES);
-      // the last channel chunk may hold fewer than 64 real channels: skip the k-steps that would multiply zeros.
-      // A k-step advances 32 bytes (16 fp16) inside the swizzle row; stacked, bh addresses [w_hi | w_lo].
-      const int ks = ((it_beg + it + 1) % p.cchunks == 0) ? p.klast : 4;
-      switch (ks) {
-        case 1: tc_stage_mma<1, 32, STACKED>(part, ah, al, bh, bl); break;
-        case 2: tc_stage_mma<2, 32, STACKED>(part, ah, al, bh, bl); break;
-        case 3: tc_stage_mma<3, 32, STACKED>(part, ah, al, bh, bl); break;
-        default: tc_stage_mma<4, 32, STACKED>(part, ah, al, bh, bl); break;
-      }
-      if (lane == 0) mbar_arrive(&empty_bar[stage]);   // this stage's MMAs have completed: free its slot
-      acc.add(part);
-      if (++stage == STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
-    }
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int it = 0; it < nk; ++it) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sa = smem_u32(smem + (size_t)stage * STAGE_BYTES);
+    const uint64_t ah = wg_desc_k(sa + cg * 64 * 128), al = wg_desc_k(sa + A_BYTES + cg * 64 * 128);
+    const uint64_t bh = wg_desc_k(sa + 2 * A_BYTES), bl = wg_desc_k(sa + 2 * A_BYTES + B_BYTES);
+    // A k-step advances 32 bytes (16 fp16) inside the swizzle row; stacked, bh addresses [w_hi | w_lo].
+    const int ks = ((it_beg + it + 1) % p.cchunks == 0) ? p.klast : 4;
+    tc_stage_mma<32, STACKED>(ks, part, ah, al, bh, bl);
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);   // this stage's MMAs have completed: free its slot
+    acc.add(part);
+    tc_ring_next(stage, phase, STAGES);
   }
 
   tc_epilogue<BN, STACKED>(acc, p, n0, h0, w0, col0, warp, lane);
@@ -344,11 +367,7 @@ conv_tc_rows_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_con
   const uint32_t slot_bytes = 2 * a_box;
   const int nslots = p.asets * p.cchunks;
   uint8_t* const smem_b = smem + (size_t)nslots * slot_bytes;
-  int t = blockIdx.x;
-  const int tw_i = t % p.tiles_w;
-  t /= p.tiles_w;
-  const int th_i = t % p.tiles_h;
-  const int n0 = t / p.tiles_h, h0 = th_i * p.TH, w0 = tw_i * p.TW;   // TN == 1
+  const auto [n0, h0, w0] = tc_tile_origin<true>(p);
   const int col0 = blockIdx.y * (STACKED ? BN / 2 : BN);
   const int nk = p.taps.n * p.cchunks;
 
@@ -388,20 +407,19 @@ conv_tc_rows_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_con
         }
       }
     } else if (threadIdx.x == 32) {
-      // B: one (tap, chunk) weight tile per stage, as conv_tc_kernel
+      // B: one (tap, chunk) weight tile per stage, as conv_tc_kernel.  The ring's depth is a run-time value: it gets
+      // as many stages as the shared memory left after the layer's A slots holds
       int stage = 0;
       uint32_t phase = 0;
       for (int it = 0; it < nk; ++it) {
         const int tap = it / p.cchunks, cc = it - tap * p.cchunks;
+        uint64_t* const full = &b_full[stage];
         mbar_wait(&b_empty[stage], phase ^ 1);
         uint8_t* sb = smem_b + (size_t)stage * B_STAGE;
-        mbar_expect_tx(&b_full[stage], B_STAGE);
-        tma_load_3d(sb, &map_bh, &b_full[stage], cc * TC_BK, col0, p.taps.widx[tap]);
-        tma_load_3d(sb + (STACKED ? B_BYTES / 2 : B_BYTES), &map_bl, &b_full[stage], cc * TC_BK, col0, p.taps.widx[tap]);
-        if (++stage == p.bstages) {
-          stage = 0;
-          phase ^= 1;
-        }
+        mbar_expect_tx(full, B_STAGE);
+        tma_load_3d(sb, &map_bh, full, cc * TC_BK, col0, p.taps.widx[tap]);
+        tma_load_3d(sb + (STACKED ? B_BYTES / 2 : B_BYTES), &map_bl, full, cc * TC_BK, col0, p.taps.widx[tap]);
+        tc_ring_next(stage, phase, p.bstages);
       }
     }
     return;
@@ -411,37 +429,26 @@ conv_tc_rows_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_con
   const int cg = (warp >> 2) - 1;
   TcAccWide<BN> acc, part;
   acc.zero();
-  {
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int it = 0; it < nk; ++it) {
-      const int tap = it / p.cchunks, cc = it - tap * p.cchunks;
-      const int j = tap / R, t0 = j * R;
-      const int s = (j % p.asets) * p.cchunks + cc;
-      const int row = p.taps.dh[tap] - min(p.taps.dh[t0], p.taps.dh[t0 + R - 1]);   // tap's first row in the box
-      mbar_wait(&a_full[s], (j / p.asets) & 1);
-      mbar_wait(&b_full[stage], phase);
-      const uint32_t sa = smem_u32(smem + (size_t)s * slot_bytes) + (uint32_t)(row * p.TW) * 128 + cg * 64 * 128;
-      const uint32_t sb = smem_u32(smem_b + (size_t)stage * B_STAGE);
-      const uint64_t ah = wg_desc_k(sa), al = wg_desc_k(sa + a_box);
-      const uint64_t bh = wg_desc_k(sb), bl = wg_desc_k(sb + B_BYTES);
-      const int ks = cc == p.cchunks - 1 ? p.klast : 4;
-      switch (ks) {
-        case 1: tc_stage_mma<1, 32, STACKED>(part, ah, al, bh, bl); break;
-        case 2: tc_stage_mma<2, 32, STACKED>(part, ah, al, bh, bl); break;
-        case 3: tc_stage_mma<3, 32, STACKED>(part, ah, al, bh, bl); break;
-        default: tc_stage_mma<4, 32, STACKED>(part, ah, al, bh, bl); break;
-      }
-      if (lane == 0) {
-        mbar_arrive(&b_empty[stage]);
-        if (tap - t0 == R - 1) mbar_arrive(&a_empty[s]);   // the run's last tap of this chunk: the slot is free
-      }
-      acc.add(part);
-      if (++stage == p.bstages) {
-        stage = 0;
-        phase ^= 1;
-      }
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int it = 0; it < nk; ++it) {
+    const int tap = it / p.cchunks, cc = it - tap * p.cchunks;
+    const int j = tap / R, t0 = j * R;
+    const int s = (j % p.asets) * p.cchunks + cc;
+    const int row = p.taps.dh[tap] - min(p.taps.dh[t0], p.taps.dh[t0 + R - 1]);   // tap's first row in the box
+    mbar_wait(&a_full[s], (j / p.asets) & 1);
+    mbar_wait(&b_full[stage], phase);
+    const uint32_t sa = smem_u32(smem + (size_t)s * slot_bytes) + (uint32_t)(row * p.TW) * 128 + cg * 64 * 128;
+    const uint32_t sb = smem_u32(smem_b + (size_t)stage * B_STAGE);
+    const uint64_t ah = wg_desc_k(sa), al = wg_desc_k(sa + a_box);
+    const uint64_t bh = wg_desc_k(sb), bl = wg_desc_k(sb + B_BYTES);
+    tc_stage_mma<32, STACKED>(cc == p.cchunks - 1 ? p.klast : 4, part, ah, al, bh, bl);
+    if (lane == 0) {
+      mbar_arrive(&b_empty[stage]);
+      if (tap - t0 == R - 1) mbar_arrive(&a_empty[s]);   // the run's last tap of this chunk: the slot is free
     }
+    acc.add(part);
+    tc_ring_next(stage, phase, p.bstages);
   }
 
   tc_epilogue<BN, STACKED>(acc, p, n0, h0, w0, col0, warp, lane);
@@ -488,20 +495,17 @@ constexpr int tc_stages(size_t stage_bytes) {
   return TC_SMEM_BUDGET / stage_bytes >= 4 ? 4 : (int)(TC_SMEM_BUDGET / stage_bytes);
 }
 
-template <int BN, bool STACKED = false>
-int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
-              const TcParams& p, dim3 grid, cudaStream_t stream) {
-  constexpr size_t stage = 2 * TC_BM * 128 + (STACKED ? 1 : 2) * BN * 128;
-  constexpr int STAGES = tc_stages(stage);
-  constexpr size_t smem = (size_t)STAGES * stage + 1024;
+// Launches KERNEL with smem bytes of dynamic shared memory.  Its limit is raised to smem_limit on the first launch
+// only: the attribute call would add host time to every convolution.
+template <auto KERNEL, class... Args>
+int tc_launch(size_t smem_limit, dim3 grid, size_t smem, cudaStream_t stream, const Args&... args) {
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES, STACKED>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit);
     if (e != cudaSuccess) return (int)e;
     configured = true;
   }
-  conv_tc_kernel<BN, STAGES, STACKED><<<grid, TC_THREADS, smem, stream>>>(ah, al, bh, bl, p);
+  KERNEL<<<grid, TC_THREADS, smem, stream>>>(args...);
   return (int)cudaGetLastError();
 }
 
@@ -509,53 +513,26 @@ int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
 // 96, 48, ...) each run within 8 columns of their real width
 constexpr int TC_BN_SET[] = {32, 48, 64, 96, 104, 112, 128};
 
-int launch_tc_bn(int bn, bool stacked, int stk_rows, const CUtensorMap& ah, const CUtensorMap& al,
-                 const CUtensorMap& bh, const CUtensorMap& bl, const TcParams& p, dim3 grid, cudaStream_t stream) {
-  if (stacked)
-    return stk_rows == 16 ? launch_tc<32, true>(ah, al, bh, bl, p, grid, stream)
-                          : launch_tc<64, true>(ah, al, bh, bl, p, grid, stream);
-  switch (bn) {
-    case 32:  return launch_tc<32>(ah, al, bh, bl, p, grid, stream);
-    case 48:  return launch_tc<48>(ah, al, bh, bl, p, grid, stream);
-    case 64:  return launch_tc<64>(ah, al, bh, bl, p, grid, stream);
-    case 96:  return launch_tc<96>(ah, al, bh, bl, p, grid, stream);
-    case 104: return launch_tc<104>(ah, al, bh, bl, p, grid, stream);
-    case 112: return launch_tc<112>(ah, al, bh, bl, p, grid, stream);
-    case 128: return launch_tc<128>(ah, al, bh, bl, p, grid, stream);
-    default:  return (int)cudaErrorInvalidValue;
-  }
+// fn(std::integral_constant<int, BN>()) for the width BN of TC_BN_SET equal to bn; cudaErrorInvalidValue for any other
+template <class F, size_t... I>
+int tc_with_width(int bn, F&& fn, std::index_sequence<I...>) {
+  int rc = (int)cudaErrorInvalidValue;
+  (void)((bn == TC_BN_SET[I] && (rc = fn(std::integral_constant<int, TC_BN_SET[I]>()), true)) || ...);
+  return rc;
+}
+template <class F>
+int tc_with_width(int bn, F&& fn) {
+  return tc_with_width(bn, fn, std::make_index_sequence<std::size(TC_BN_SET)>());
 }
 
-template <int BN, bool STACKED = false>
-int launch_tc_rows(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
-                   const TcParams& p, dim3 grid, size_t smem, cudaStream_t stream) {
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_rows_kernel<BN, STACKED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)TC_ROWS_SMEM_LIMIT);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
-  conv_tc_rows_kernel<BN, STACKED><<<grid, TC_THREADS, smem, stream>>>(ah, al, bh, bl, p);
-  return (int)cudaGetLastError();
-}
-
-int launch_tc_rows_bn(int bn, bool stacked, int stk_rows, const CUtensorMap& ah, const CUtensorMap& al,
-                      const CUtensorMap& bh, const CUtensorMap& bl, const TcParams& p, dim3 grid, size_t smem,
-                      cudaStream_t stream) {
+// fn(BN, STACKED) as integral constants for a forward N tile: stacked, [w_hi | w_lo] of stk_rows = 16 or 32 output
+// channels; else the instantiated width bn
+template <class F>
+int tc_with_tile(int bn, bool stacked, int stk_rows, F&& fn) {
   if (stacked)
-    return stk_rows == 16 ? launch_tc_rows<32, true>(ah, al, bh, bl, p, grid, smem, stream)
-                          : launch_tc_rows<64, true>(ah, al, bh, bl, p, grid, smem, stream);
-  switch (bn) {
-    case 32:  return launch_tc_rows<32>(ah, al, bh, bl, p, grid, smem, stream);
-    case 48:  return launch_tc_rows<48>(ah, al, bh, bl, p, grid, smem, stream);
-    case 64:  return launch_tc_rows<64>(ah, al, bh, bl, p, grid, smem, stream);
-    case 96:  return launch_tc_rows<96>(ah, al, bh, bl, p, grid, smem, stream);
-    case 104: return launch_tc_rows<104>(ah, al, bh, bl, p, grid, smem, stream);
-    case 112: return launch_tc_rows<112>(ah, al, bh, bl, p, grid, smem, stream);
-    case 128: return launch_tc_rows<128>(ah, al, bh, bl, p, grid, smem, stream);
-    default:  return (int)cudaErrorInvalidValue;
-  }
+    return stk_rows == 16 ? fn(std::integral_constant<int, 32>(), std::true_type())
+                          : fn(std::integral_constant<int, 64>(), std::true_type());
+  return tc_with_width(bn, [&](auto width) { return fn(width, std::false_type()); });
 }
 
 // Taps per row run if the tap list splits completely into runs of the same length R >= 2 (equal dw and dn, dh
@@ -622,7 +599,6 @@ conv_tc_wgrad_wide_kernel(const __grid_constant__ CUtensorMap map_gh, const __gr
   constexpr uint32_t B_BYTES = NSB * WG_SLAB;
   constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + TAPS * 2 * B_BYTES;   // G hi, G lo, then X hi, X lo per entry
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
   const int warp = tc_warp_uniform(), lane = threadIdx.x & 31;
@@ -635,16 +611,7 @@ conv_tc_wgrad_wide_kernel(const __grid_constant__ CUtensorMap map_gh, const __gr
   const uint32_t tx_bytes = 2 * A_BYTES + ne * 2 * B_BYTES;
   if (nk <= 0) return;
 
-  if (threadIdx.x == 0) {
-    prefetch_tmap(&map_gh);
-    prefetch_tmap(&map_xh);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], TC_CONSUMER_WARPS);
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
+  uint8_t* const smem = tc_prologue(smem_raw, full_bar, empty_bar, STAGES, map_gh, map_xh);
 
   if (warp < 4) {
     if (threadIdx.x == 0) {
@@ -658,17 +625,18 @@ conv_tc_wgrad_wide_kernel(const __grid_constant__ CUtensorMap map_gh, const __gr
         const int t2 = ch / p.wchunks;
         const int hc = t2 % p.hchunks;
         const int w0 = wc * p.cw, h = hc * p.chh, n = (t2 / p.hchunks) * p.cn;
+        uint64_t* const full = &full_bar[stage];
         mbar_wait(&empty_bar[stage], phase ^ 1);
         uint8_t* sa = smem + (size_t)stage * STAGE_BYTES;
-        mbar_expect_tx(&full_bar[stage], tx_bytes);
-        tma_load_5d(sa, &map_gh, &full_bar[stage], 0, w0, h, n + gdn, aslab);
-        tma_load_5d(sa + A_BYTES, &map_gl, &full_bar[stage], 0, w0, h, n + gdn, aslab);
+        mbar_expect_tx(full, tx_bytes);
+        tma_load_5d(sa, &map_gh, full, 0, w0, h, n + gdn, aslab);
+        tma_load_5d(sa + A_BYTES, &map_gl, full, 0, w0, h, n + gdn, aslab);
         for (int t = 0; t < ne; ++t) {
           const int e = e0 + t;
           const int xw = w0 + p.xdw[e], xh = h + p.xdh[e], xn = n + p.xdn[e];
           uint8_t* sb = sa + 2 * A_BYTES + t * 2 * B_BYTES;
-          tma_load_5d(sb, &map_xh, &full_bar[stage], ci0, xw, xh, xn, 0);
-          tma_load_5d(sb + B_BYTES, &map_xl, &full_bar[stage], ci0, xw, xh, xn, 0);
+          tma_load_5d(sb, &map_xh, full, ci0, xw, xh, xn, 0);
+          tma_load_5d(sb + B_BYTES, &map_xl, full, ci0, xw, xh, xn, 0);
         }
         if (++stage == STAGES) {
           stage = 0;
@@ -698,28 +666,26 @@ conv_tc_wgrad_wide_kernel(const __grid_constant__ CUtensorMap map_gh, const __gr
   TcAccWide<BNW, 1, 1> acc[TAPS], part;
 #pragma unroll
   for (int t = 0; t < TAPS; ++t) acc[t].zero();
-  {
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int it = 0; it < nk; ++it) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_u32(smem + (size_t)stage * STAGE_BYTES);
-      const uint64_t ah = make_desc_mn(sa + cg * WG_SLAB), al = make_desc_mn(sa + A_BYTES + cg * WG_SLAB);
-      const uint32_t sb = sa + 2 * A_BYTES;
-      tc_stage_mma<WG_PIX / 16, 16 * 128, false>(part, ah, al, make_desc_mn(sb), make_desc_mn(sb + B_BYTES));
-      acc[0].add(part);
-      if constexpr (TAPS == 2) {
-        if (ne == 2) {
-          const uint32_t sb1 = sb + 2 * B_BYTES;
-          tc_stage_mma<WG_PIX / 16, 16 * 128, false>(part, ah, al, make_desc_mn(sb1), make_desc_mn(sb1 + B_BYTES));
-          acc[1].add(part);
-        }
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int it = 0; it < nk; ++it) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sa = smem_u32(smem + (size_t)stage * STAGE_BYTES);
+    const uint64_t ah = make_desc_mn(sa + cg * WG_SLAB), al = make_desc_mn(sa + A_BYTES + cg * WG_SLAB);
+    const uint32_t sb = sa + 2 * A_BYTES;
+    tc_stage_mma<16 * 128, false>(WG_PIX / 16, part, ah, al, make_desc_mn(sb), make_desc_mn(sb + B_BYTES));
+    acc[0].add(part);
+    if constexpr (TAPS == 2) {
+      if (ne == 2) {
+        const uint32_t sb1 = sb + 2 * B_BYTES;
+        tc_stage_mma<16 * 128, false>(WG_PIX / 16, part, ah, al, make_desc_mn(sb1), make_desc_mn(sb1 + B_BYTES));
+        acc[1].add(part);
       }
-      if (lane == 0) mbar_arrive(&empty_bar[stage]);     // this stage's MMAs have completed: free its slot
-      if (++stage == STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
+    }
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);     // this stage's MMAs have completed: free its slot
+    if (++stage == STAGES) {
+      stage = 0;
+      phase ^= 1;
     }
   }
 
@@ -759,39 +725,8 @@ __global__ void __launch_bounds__(256) wgrad_sum_kernel(const float* __restrict_
   }
 }
 
-template <int BNW, int TAPS>
-int launch_wgrad(const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap& xh, const CUtensorMap& xl,
-                 const TcWgradParams& p, dim3 grid, cudaStream_t stream) {
-  constexpr size_t stage = 2 * 2 * WG_SLAB + TAPS * 2 * ((BNW + WG_CH - 1) / WG_CH) * WG_SLAB;
-  constexpr int STAGES = tc_stages(stage);
-  constexpr size_t smem = (size_t)STAGES * stage + 1024;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_wgrad_wide_kernel<BNW, STAGES, TAPS>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
-  conv_tc_wgrad_wide_kernel<BNW, STAGES, TAPS><<<grid, TC_THREADS, smem, stream>>>(gh, gl, xh, xl, p);
-  return (int)cudaGetLastError();
-}
-
 // widths up to 104 take two entries per CTA (three accumulator sets of BNW / 2 registers fit the 168 of a thread)
 constexpr int WG_PAIR_MAX_BN = 104;
-
-int launch_wgrad_bn(int bn, bool pair, const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap& xh,
-                    const CUtensorMap& xl, const TcWgradParams& p, dim3 grid, cudaStream_t stream) {
-  switch (bn) {
-    case 32:  return pair ? launch_wgrad<32, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<32, 1>(gh, gl, xh, xl, p, grid, stream);
-    case 48:  return pair ? launch_wgrad<48, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<48, 1>(gh, gl, xh, xl, p, grid, stream);
-    case 64:  return pair ? launch_wgrad<64, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<64, 1>(gh, gl, xh, xl, p, grid, stream);
-    case 96:  return pair ? launch_wgrad<96, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<96, 1>(gh, gl, xh, xl, p, grid, stream);
-    case 104: return pair ? launch_wgrad<104, 2>(gh, gl, xh, xl, p, grid, stream) : launch_wgrad<104, 1>(gh, gl, xh, xl, p, grid, stream);
-    case 112: return launch_wgrad<112, 1>(gh, gl, xh, xl, p, grid, stream);
-    case 128: return launch_wgrad<128, 1>(gh, gl, xh, xl, p, grid, stream);
-    default:  return (int)cudaErrorInvalidValue;
-  }
-}
 
 // ci tile: as the forward's N tile (og_conv2d_tc), the smallest number of equal tiles of <= 128 columns, rounded up
 // to the wgmma N step of 8, then to the next instantiated width
@@ -918,9 +853,21 @@ OG_API int og_conv2d_tc(const void* xh, const void* xl, const unsigned* amax_x, 
   if ((rc = make_map(&mbh, wh, 3, bdims, bstr, bbox))) return rc;
   if ((rc = make_map(&mal, xl, 4, adims, astr, abox))) return rc;
   if ((rc = make_map(&mbl, wl, 3, bdims, bstr, bbox))) return rc;
-  if (rows) return launch_tc_rows_bn(BNsel, stacked, stk_rows, mah, mal, mbh, mbl, p, grid, rows_smem, stream);
   if (p.ksplit > 1) OG_CHECK(og_work_alloc(&p.work, (size_t)p.ksplit * p.work_plane, stream));
-  rc = launch_tc_bn(BNsel, stacked, stk_rows, mah, mal, mbh, mbl, p, grid, stream);
+  if (!rows) {
+    rc = tc_with_tile(BNsel, stacked, stk_rows, [&](auto bn, auto stk) {
+      constexpr int BN = decltype(bn)::value;
+      constexpr bool STACKED = decltype(stk)::value;
+      constexpr size_t stage = 2 * TC_BM * 128 + (STACKED ? 1 : 2) * BN * 128;
+      constexpr size_t smem = (size_t)tc_stages(stage) * stage + 1024;
+      return tc_launch<conv_tc_kernel<BN, tc_stages(stage), STACKED>>(smem, grid, smem, stream, mah, mal, mbh, mbl, p);
+    });
+  } else {
+    rc = tc_with_tile(BNsel, stacked, stk_rows, [&](auto bn, auto stk) {
+      return tc_launch<conv_tc_rows_kernel<decltype(bn)::value, decltype(stk)::value>>(
+          TC_ROWS_SMEM_LIMIT, grid, rows_smem, stream, mah, mal, mbh, mbl, p);
+    });
+  }
   if (p.ksplit > 1) {
     if (!rc) rc = og_split_sum(p.work, p.work_plane, p.ksplit, y, stream);
     const cudaError_t e = cudaFreeAsync(p.work, stream);
@@ -1031,7 +978,18 @@ OG_API int og_conv2d_wgrad_tc(const void* gh, const void* gl, const unsigned* am
   p.work = nullptr;
   const long long plane = (long long)Kp * C;
   if (shared_out) OG_CHECK(og_work_alloc(&p.work, (size_t)splits * nentries * plane, stream));
-  rc = launch_wgrad_bn(BNsel, pair, mgh, mgl, mxh, mxl, p, grid, stream);
+  const auto launch = [&](auto bnw, auto taps) {
+    constexpr int BNW = decltype(bnw)::value, TAPS = decltype(taps)::value;
+    constexpr size_t stage = 2 * 2 * WG_SLAB + TAPS * 2 * ((BNW + WG_CH - 1) / WG_CH) * WG_SLAB;
+    constexpr size_t smem = (size_t)tc_stages(stage) * stage + 1024;
+    return tc_launch<conv_tc_wgrad_wide_kernel<BNW, tc_stages(stage), TAPS>>(smem, grid, smem, stream, mgh, mgl, mxh,
+                                                                            mxl, p);
+  };
+  rc = tc_with_width(BNsel, [&](auto bnw) {
+    if constexpr (decltype(bnw)::value <= WG_PAIR_MAX_BN)
+      if (pair) return launch(bnw, std::integral_constant<int, 2>());
+    return launch(bnw, std::integral_constant<int, 1>());
+  });
   if (shared_out) {
     if (!rc) {
       WgradSum ws;
