@@ -642,11 +642,15 @@ def test_cuda_graph_replay_matches_eager():
     ob = b.step(db)                              # graph replay
     torch.cuda.synchronize()
     assert b.launches_per_step > 500
+    # every reduction of the step adds in a fixed order (DESIGN.md, run-to-run determinism): the replay gives the bits
     for k in ("errPatD0", "errPatD1", "errPatD2", "errG", "kl"):
-        assert abs(float(oa[k]) - float(ob[k])) <= 1e-3 * max(1.0, abs(float(oa[k]))), k
+        assert torch.equal(ob[k], oa[k]), (k, float(ob[k]), float(oa[k]))
     for i in range(3):
-        close(ob["fake_imgs"][i], oa["fake_imgs"][i], 1e-4, what=f"fake{i}")   # forward is deterministic
-    assert rel_l2(b.bG.grad, a.bG.grad) < 1e-2                                  # backward has atomics (order varies)
+        assert torch.equal(ob["fake_imgs"][i], oa["fake_imgs"][i]), f"fake{i}"
+    assert torch.equal(b.bG.grad, a.bG.grad), rel_l2(b.bG.grad, a.bG.grad)
+    for i, (x, y) in enumerate(zip([a.bG, *a.bD], [b.bG, *b.bD])):
+        assert torch.equal(y.flat, x.flat), (i, rel_l2(y.flat, x.flat))
+    assert torch.equal(b.bG.avg, a.bG.avg)
     assert int(b.bG.step_dev) == int(a.bG.step_dev) == 1 and b.bG.step == 1
 
 
