@@ -359,7 +359,16 @@ int og_lstm_bidir_state(const float* gx, const float* whh_f, const float* whh_b,
  *                       (mean, std of x, y, w, r), label_to_class [NL] (class row, -1 for the special tokens),
  *                       count_stats [C][2] (mu, sigma of the per-class count), noise_cnt [B][C] standard normals.
  *                       rois [3][B][R][6] at 64, 128 and 256 pixels, fm_rois [B][R][6], roi_cls [B][R], num_rois [B],
- *                       zero-padded to R slots.  S <= 16. */
+ *                       zero-padded to R slots.  S <= 16.  It is og_box_records' rows through the boxes.txt round
+ *                       trip int(float('%.2f' % v)), the ROI_MIN_SIZE filter (min_size) and the three scales.
+ *  og_box_records     : the rows Evaluator.evaluate writes to boxes.txt, per sample in float64, from the same inputs as
+ *                       og_box_layout: rows [B][S][4] (x, y, w, h after the clip; not rounded, no size filter, zero
+ *                       after the end), row_cls [B][S] (class row), n_rows [B], n_valid [B] (valid steps before the
+ *                       last is dropped; the reference writes a dev_bbox_test.txt line only when it is > 1) and
+ *                       n_special [B] (boxes dropped for a special label, where the reference raises).  S <= 16.
+ *  og_box_noise       : noise_box [B][S][6] and noise_cnt [B][C] of captions first .. first + B - 1, each a function of
+ *                       (seed, caption index) only: Philox4x32-10 of (value, stream, index) under the key seed >= 0;
+ *                       columns 0 and 3 of noise_box uniform in [0, 1), every other value a standard normal. */
 int og_box_label_table(const float* emb, const float* w_ih, const float* b_ih, const float* b_hh, int NL, float* table,
                        cudaStream_t stream);
 int og_box_decode(const float* h0, const float* c0, const float* table, const float* wt, const float* xy_w,
@@ -372,6 +381,12 @@ int og_box_layout(const long long* labels, const float* samples, const long long
                   const long long* label_to_class, const double* count_stats, const float* noise_cnt, int B, int S,
                   int NL, int C, int R, int min_size, double* rois, double* fm_rois, long long* roi_cls,
                   long long* num_rois, cudaStream_t stream);
+int og_box_records(const long long* labels, const float* samples, const long long* steps, const double* mean_std,
+                   const long long* label_to_class, const double* count_stats, const float* noise_cnt, int B, int S,
+                   int NL, int C, double* rows, long long* row_cls, long long* n_rows, long long* n_valid,
+                   long long* n_special, cudaStream_t stream);
+int og_box_noise(long long seed, long long first, int B, int S, int C, float* noise_box, float* noise_cnt,
+                 cudaStream_t stream);
 
 /* zero-fill (a memset node when captured in a CUDA graph; no kernel launch) */
 int og_zero_bytes(float* p, long long bytes, cudaStream_t stream);

@@ -2,6 +2,10 @@
 reference's box_generation/sample.py + Evaluator.evaluate + image_generation/miscc/load.py:load_gen_insanns, on the
 device and without files in between.
 
+``Evaluator`` is the other way: a drop-in for the reference's box_generation Evaluator that writes the layout files
+(``<folder><key>/<caption index>/boxes.txt``, or ``dev_bbox_test.txt``) for a whole test split, a chunk of captions per
+launch, with the files written on a background thread while the device runs the next chunk.
+
 ``BoxGenerator.from_reference`` reads the reference's own files.  Its decoder checkpoint (``model.pt``) is a whole
 pickled ``DecoderRNN``; it is read with an unpickler that maps the ``seq2seq.*`` classes to inert stubs, allows only
 the globals a module pickle needs, and raises on anything else, so loading it imports and runs none of the reference's
@@ -13,10 +17,16 @@ import collections
 import io
 import os
 import pickle
+import queue
+import re
+import threading
+import time
 import types
+import warnings
 
 import numpy as np
 import torch
+import torch.distributed as dist
 import torch.nn.backends.thnn
 
 from . import model, ops
@@ -252,3 +262,339 @@ def load_reference_decoder(path: str) -> model.DecoderRNN:
                            use_attention=st["use_attention"])
     dec.load_state_dict(sd, strict=True)
     return dec.eval()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The reference's test split (box_generation/seq2seq/dataset/prepare_dataset.py:81-244), without nltk
+# ---------------------------------------------------------------------------------------------------------------------
+SPECIAL_LABELS = ("<pad>", "<sos>", "<eos>", "<unk>")
+
+
+def normalize_string(s: str) -> list:
+    """normalize_string (prepare_dataset.py:81-91): '��' -> ' ', lower-case, the tokens of ``\\w+`` (what
+    nltk's RegexpTokenizer(r'\\w+') returns), each with its non-ASCII characters removed; empty tokens dropped."""
+    tokens = re.findall(r"\w+", s.replace("��", " ").lower())
+    return [t for t in (t.encode("ascii", "ignore").decode("ascii") for t in tokens) if t]
+
+
+def indexes_from_sentence(word2index, words) -> list:
+    """indexes_from_sentence (prepare_dataset.py:221-235): the known words' indexes, with <sos> / <eos> around them
+    only if the vocabulary has them; unknown words are dropped."""
+    seq = [word2index["<sos>"]] if "<sos>" in word2index else []
+    seq += [word2index[w] for w in words if w in word2index]
+    if "<eos>" in word2index:
+        seq.append(word2index["<eos>"])
+    return seq
+
+
+def _lines(path):
+    with open(path) as f:
+        return f.read().strip().split("\n")
+
+
+def read_test_tuples(dev_path) -> list:
+    """read_langs (prepare_dataset.py:93-113): one [tokens, x, y, w, h, labels] tuple per line of six tab-separated
+    fields, the caption normalised.  A line with another field count raises ValueError naming it."""
+    tuples = []
+    for i, line in enumerate(_lines(dev_path)):
+        f = line.split("\t")
+        if len(f) != 6:
+            raise ValueError(f"{dev_path} line {i + 1}: {len(f)} tab-separated fields, the test split has 6: "
+                             f"{line[:80]!r}")
+        tuples.append([normalize_string(f[0]), *f[1:]])
+    return tuples
+
+
+def read_keys(dev_filename_path) -> list:
+    """The image key of each caption line (filenames_val2014.txt, one per line)."""
+    return _lines(dev_filename_path)
+
+
+def load_cap_vocab(checkpoint_dir):
+    """(cap_word2index, cap_index2word) of a box checkpoint (seq2seq/util/checkpoint.py:83-86), read through the
+    restricted unpickler in either pickle format."""
+    return (_restricted_load(os.path.join(checkpoint_dir, "cap_word2index.pt")),
+            _restricted_load(os.path.join(checkpoint_dir, "cap_index2word.pt")))
+
+
+def caption_indices(keys) -> list:
+    """The caption index of every tuple: how many earlier tuples have its key, in file order (evaluator.py:48-52,
+    87-89).  Computed from the full key list, so a shard's numbering is the one-process numbering."""
+    seen = collections.Counter()
+    out = []
+    for k in keys:
+        out.append(seen[k])
+        seen[k] += 1
+    return out
+
+
+def caption_sequences(data, keys, word2index) -> list:
+    """Every tuple's caption as token indexes, after checking the split: one key per tuple, and no caption that maps to
+    no token (the reference's encoder fails on it).  Raises ValueError naming the first offending line."""
+    if len(keys) != len(data):
+        raise ValueError(f"{len(keys)} image keys for {len(data)} captions: the key file must have one line per "
+                         f"caption line")
+    seqs = []
+    for i, item in enumerate(data):
+        seq = indexes_from_sentence(word2index, item[0])
+        if not seq:
+            raise ValueError(f"caption line {i + 1} ({' '.join(item[0])!r}, key {keys[i]}) has no word of the caption "
+                             f"vocabulary")
+        seqs.append(seq)
+    return seqs
+
+
+def box_rows_text(rows, names) -> str:
+    """A boxes.txt: one '%.2f,%.2f,%.2f,%.2f,<category id>,0' line per row (evaluator.py:137-139)."""
+    return "".join("%.2f,%.2f,%.2f,%.2f,%s,0\n" % (x, y, w, h, names[c]) for (x, y, w, h), c in rows)
+
+
+def dev_bbox_line(key, words, rows, names) -> str:
+    """A dev_bbox_test.txt line (evaluator.py:142-149)."""
+    return "%s - %s - " % (key, words) + "".join("%.2f,%.2f,%.2f,%.2f,%s - " % (x, y, w, h, names[c])
+                                                for (x, y, w, h), c in rows) + "\n"
+
+
+class _FileWriter:
+    """Writes the files of each chunk on one background thread.  ``submit`` takes a job (its arrays may still be on
+    their way from the device: the job's event is waited on first) and blocks while two earlier chunks are queued; an
+    error of the writer is raised by the next ``submit`` or by ``close``.  The dev_bbox_test.txt lines are kept in
+    ``lines`` for the caller to write."""
+
+    def __init__(self, write):
+        self._write = write
+        self._q = queue.Queue(maxsize=2)
+        self._thread = threading.Thread(target=self._run, name="box-files", daemon=True)
+        self._error = None
+        self._thread.start()
+
+    def _raise(self):
+        if self._error is not None:
+            err, self._error = self._error, None
+            raise RuntimeError("writing the box layout files failed") from err
+
+    def _run(self):
+        while True:
+            job = self._q.get()
+            try:
+                if job is None:
+                    return
+                if self._error is None:
+                    self._write(*job)
+            except BaseException as e:      # surfaced on the caller's thread
+                self._error = e
+            finally:
+                self._q.task_done()
+
+    def submit(self, *job):
+        self._raise()
+        self._q.put(job)
+
+    def close(self, raise_error=True):
+        if self._thread is not None:
+            self._q.put(None)
+            self._thread.join()
+            self._thread = None
+        if raise_error:
+            self._raise()
+
+
+def _library_modules(encoder, decoder, label_word2index):
+    """This library's PreEncoderRNN / DecoderRNN for the given modules: as they are, or loaded from the state_dict of
+    the reference's (whose keys and shapes are the same)."""
+    if not isinstance(encoder, model.PreEncoderRNN):
+        sd = {k: v.detach().cpu() for k, v in encoder.state_dict().items()}
+        enc = model.PreEncoderRNN(sd["encoder.weight"].shape[0], ninput=sd["encoder.weight"].shape[1], nhidden=256)
+        enc.load_state_dict(sd, strict=True)
+        encoder = enc
+    if not isinstance(decoder, model.DecoderRNN):
+        sd = {k: v.detach().cpu() for k, v in decoder.state_dict().items()}
+        dec = model.DecoderRNN(label_word2index, decoder.x_mean, decoder.y_mean, decoder.w_mean, decoder.r_mean, 1,
+                               getattr(decoder, "max_length", 150), decoder.hidden_size, decoder.gmm_comp_num,
+                               n_layers=getattr(decoder, "n_layers", 1),
+                               rnn_cell="gru" if "GRU" in str(getattr(decoder, "rnn_cell", "lstm")) else "lstm",
+                               bidirectional=decoder.bidirectional_encoder,
+                               use_attention=getattr(decoder, "use_attention", False))
+        dec.load_state_dict(sd, strict=True)
+        decoder = dec
+    return encoder, decoder
+
+
+class Evaluator:
+    """Drop-in for the reference's box_generation Evaluator (seq2seq/evaluator/evaluator.py): the same constructor, and
+    ``evaluate(encoder, decoder, data, keys)`` writes the same files -- with ``output_opt`` 0 one
+    ``box_saving_folder + key + '/<j>/boxes.txt'`` per tuple (j: the tuple's caption index among those of its key), with
+    1 ``expt_dir/dev_bbox_test.txt`` -- running ``chunk`` captions per launch on the device.
+
+    ``batch_size`` must be 1: every tuple is evaluated once, in file order (the reference's loop at a larger batch runs
+    only the first len / batch_size tuples).  The noise of tuple i depends only on (``seed``, i) (og_box_noise), so the
+    files do not depend on ``chunk`` or on the number of ranks; it is not numpy's draw sequence.  Under torchrun with an
+    initialised process group every rank writes the boxes.txt files of its own contiguous share of the tuples, and rank
+    0 writes dev_bbox_test.txt from the rows of all.  A box whose label is a special token (where the reference raises)
+    is dropped, with one warning giving the number of captions affected."""
+
+    def __init__(self, batch_size, early_stop_len, expt_dir, dev_cap_lang, dev_label_lang, x_mean_std, y_mean_std,
+                 w_mean_std, r_mean_std, gaussian_dict, box_saving_folder, output_opt, *, chunk: int = 1024,
+                 seed: int = 0, device=None, process_group=None):
+        if batch_size != 1:
+            raise ValueError(f"batch_size must be 1 (every tuple once, in file order); got {batch_size}.  The captions "
+                             f"per launch are set by chunk=")
+        if output_opt not in (0, 1):
+            raise ValueError(f"output_opt must be 0 (boxes.txt per caption) or 1 (dev_bbox_test.txt), got {output_opt}")
+        if int(chunk) < 1:
+            raise ValueError(f"chunk must be >= 1, got {chunk}")
+        self.batch_size, self.early_stop_len, self.expt_dir = batch_size, int(early_stop_len), expt_dir
+        self.dev_cap_lang, self.dev_label_lang = dev_cap_lang, dev_label_lang
+        self.mean_std = np.array([x_mean_std, y_mean_std, w_mean_std, r_mean_std], dtype=np.float64).reshape(4, 2)
+        self.gaussian_dict = gaussian_dict
+        self.box_saving_folder, self.output_opt = box_saving_folder, output_opt
+        self.display_step = 200
+        self.chunk, self.seed = int(chunk), int(seed)
+        self.device = torch.device(device) if device is not None else \
+            torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
+        self.pg = process_group
+        self.world = dist.get_world_size(process_group) if (dist.is_available() and dist.is_initialized()) else 1
+        self.rank = dist.get_rank(process_group) if self.world > 1 else 0
+        # class rows: the category ids of the label vocabulary in index order; the special tokens have none
+        i2w = dev_label_lang.index2word
+        self.label_to_class, self.class_names, stats = [], [], []
+        for i in range(len(i2w)):
+            w = i2w[i]
+            if w in SPECIAL_LABELS:
+                self.label_to_class.append(-1)
+                continue
+            cid = int(w)
+            if cid not in gaussian_dict:
+                raise ValueError(f"gaussian_dict has no statistics for category id {cid} (label {i})")
+            self.label_to_class.append(len(self.class_names))
+            self.class_names.append(str(cid))
+            stats.append([float(gaussian_dict[cid][0]), float(gaussian_dict[cid][1])])
+        self.count_stats = stats
+
+    @classmethod
+    def from_reference(cls, checkpoint_dir: str, text_snapshot: str, dev_path: str, dev_filename_path: str, mean_std,
+                       gaussian_dict, box_saving_folder: str, output_opt: int, expt_dir: str = "experiment",
+                       early_stop_len: int = 10, **kw) -> "Evaluator":
+        """The evaluator of the reference's sample.py --is_training 0, from its files alone: a box checkpoint directory
+        (model.pt, the cap_* / label_* vocabularies), the text encoder snapshot, the test split (dev_path, its keys in
+        dev_filename_path), mean_std_train2014.txt (or its (4, 2) table) and gaussian_dict.npy (or the dict).  Call
+        ``evaluate()`` with no arguments to write the files of that split."""
+        cap_w2i, cap_i2w = load_cap_vocab(checkpoint_dir)
+        label_i2w = _restricted_load(os.path.join(checkpoint_dir, "label_index2word.pt"))
+        label_w2i = {w: i for i, w in label_i2w.items()}
+        ms = np.loadtxt(mean_std) if isinstance(mean_std, (str, os.PathLike)) else np.asarray(mean_std)
+        ms = np.asarray(ms, dtype=np.float64).reshape(4, 2)
+        gd = np.load(gaussian_dict, allow_pickle=True).item() if isinstance(gaussian_dict, (str, os.PathLike)) \
+            else gaussian_dict
+        ev = cls(1, early_stop_len, expt_dir, types.SimpleNamespace(word2index=cap_w2i, index2word=cap_i2w),
+                 types.SimpleNamespace(word2index=label_w2i, index2word=label_i2w), *[tuple(r) for r in ms], gd,
+                 box_saving_folder, output_opt, **kw)
+        data = read_test_tuples(dev_path)
+        keys = read_keys(dev_filename_path)
+        caption_sequences(data, keys, cap_w2i)            # refuse a bad split before loading any weights
+        from .sampler import strip_module_prefix
+        text_sd = strip_module_prefix(torch.load(text_snapshot, map_location="cpu"))
+        enc = model.PreEncoderRNN(text_sd["encoder.weight"].shape[0], ninput=text_sd["encoder.weight"].shape[1],
+                                  nhidden=256)
+        enc.load_state_dict(text_sd, strict=True)
+        dec = load_reference_decoder(os.path.join(checkpoint_dir, "model.pt"))
+        ev._split = (enc, dec, data, keys)
+        return ev
+
+    # ------------------------------------------------------------------ evaluation
+    def evaluate(self, encoder=None, decoder=None, data=None, keys=None):
+        """Writes the files of every tuple of ``data`` (the reference's dev_tuples: [caption tokens, x, y, w, h,
+        labels]) with ``keys`` its image keys, and returns when every file is closed.  With from_reference, the
+        arguments default to the files it read."""
+        if encoder is None:
+            encoder, decoder, data, keys = self._split
+        seqs = caption_sequences(data, keys, self.dev_cap_lang.word2index)
+        jidx = caption_indices(keys)
+        enc, dec = _library_modules(encoder, decoder, self.dev_label_lang.word2index)
+        self.generator = BoxGenerator(enc.to(self.device), dec.to(self.device), self.mean_std, self.count_stats,
+                                      self.label_to_class, self.early_stop_len)
+        n = len(seqs)
+        lo, hi = n * self.rank // self.world, n * (self.rank + 1) // self.world
+        i2w = self.dev_cap_lang.index2word
+        lines, affected = [], [0]
+
+        busy = [0.0]
+
+        def write(start, host, event):
+            if event is not None:
+                event.synchronize()
+            t0 = time.perf_counter()
+            b, s = len(host) // (5 * self.early_stop_len + 3), self.early_stop_len
+            rows, cls, n_rows, n_valid, n_special = (t.numpy() for t in ops.unpack_box_records(host, b, s))
+            rows, cls = rows.tolist(), cls.tolist()
+            n_rows, n_valid = n_rows.tolist(), n_valid.tolist()
+            affected[0] += int((n_special > 0).sum())
+            for q in range(b):
+                i = start + q
+                r = list(zip(rows[q][:n_rows[q]], cls[q][:n_rows[q]]))
+                if self.output_opt == 0:
+                    d = self.box_saving_folder + keys[i] + "/%d/" % jidx[i]
+                    os.makedirs(d, exist_ok=True)
+                    with open(d + "boxes.txt", "w") as f:
+                        f.write(box_rows_text(r, self.class_names))
+                elif n_valid[q] > 1:
+                    lines.append(dev_bbox_line(keys[i], [i2w[w] for w in seqs[i]], r, self.class_names))
+            busy[0] += time.perf_counter() - t0
+
+        writer = _FileWriter(write)
+        try:
+            with torch.no_grad():
+                for start in range(lo, hi, self.chunk):
+                    stop = min(start + self.chunk, hi)
+                    packed = self._device_records(start, seqs[start:stop])
+                    if packed.is_cuda:
+                        host = torch.empty(packed.shape, dtype=packed.dtype, pin_memory=True)
+                        host.copy_(packed, non_blocking=True)
+                        event = torch.cuda.Event()
+                        event.record()
+                    else:
+                        host, event = packed, None
+                    writer.submit(start, host, event)
+                    if self.rank == 0:
+                        for d in range((start - lo) * self.world, (stop - lo) * self.world):
+                            if (d + 1) % self.display_step == 0 and d < n:
+                                print("%07d / %07d" % (d, n))
+        except BaseException:
+            writer.close(raise_error=False)
+            raise
+        writer.close()
+        t0 = time.perf_counter()
+        self._finish(lines, affected[0])
+        self.write_seconds = busy[0] + time.perf_counter() - t0      # this rank's time formatting and writing files
+
+    def _device_records(self, start, seqs):
+        """The packed og_box_records buffer of tuples start .. start + len(seqs) - 1: encoder state, decoder, rows --
+        six library calls whatever the caption lengths."""
+        bg, b = self.generator, len(seqs)
+        width = max(len(q) for q in seqs)
+        caps = np.zeros((b, width), dtype=np.int64)
+        for q, seq in enumerate(seqs):
+            caps[q, :len(seq)] = seq
+        caps = torch.from_numpy(caps).to(self.device, non_blocking=True)
+        lens = torch.tensor([len(q) for q in seqs], dtype=torch.int64).to(self.device, non_blocking=True)
+        nb, nc = ops.box_noise(self.seed, start, b, self.early_stop_len, bg.num_classes, self.device)
+        _, h, c = bg.encoder.encode_state(caps, lens, width)
+        labels, samples, steps, _ = bg.decoder.sample_state(h, c, nb, self.early_stop_len)
+        return ops.box_records_packed(labels, samples, steps, bg.mean_std, bg.label_to_class, bg.count_stats, nc)
+
+    def _finish(self, lines, affected):
+        if self.world > 1:
+            got = [None] * self.world if self.rank == 0 else None
+            dist.gather_object((lines, affected), got, dst=0, group=self.pg)
+            if self.rank == 0:
+                lines = [ln for part, _ in got for ln in part]
+                affected = sum(a for _, a in got)
+        if self.rank == 0:
+            if self.output_opt == 1:
+                with open("%s/dev_bbox_test.txt" % self.expt_dir, "w") as f:
+                    f.writelines(lines)
+            if affected:
+                warnings.warn(f"{affected} captions sampled a box with a special label (<pad>, <sos> or <unk>); the "
+                              f"reference raises on these, here the boxes were dropped")
+        if self.world > 1:
+            dist.barrier(group=self.pg)                  # every rank's files are closed before any rank returns

@@ -330,11 +330,109 @@ OG_API int og_box_decode(const float* h0, const float* c0, const float* table, c
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Samples to layout, one thread per sample (at most S <= BOXES_NUM + 1 steps): de-normalise in float64, keep the
-// steps with x, y, w, h > 0, drop the last kept one (or keep nothing when only one is kept), drop boxes with a
-// special label, cap each class at max(trunc(mu + sigma * n), 2) boxes in order, centre -> corner and clip to the
-// 256-pixel frame, the boxes.txt round trip int(float('%.2f' % v)), the ROI_MIN_SIZE filter and the three scales.
+// Samples to the evaluator's rows, one thread per sample (at most S <= BOXES_NUM + 1 steps): de-normalise in float64,
+// keep the steps with x, y, w, h > 0, drop the last kept one (or keep nothing when only one is kept), drop boxes with
+// a special label, cap each class at max(trunc(mu + sigma * n), 2) boxes in order, centre -> corner and clip to the
+// 256-pixel frame.  Both og_box_records (the rows boxes.txt holds) and og_box_layout (those rows after the boxes.txt
+// round trip) start from this one function.
 // ---------------------------------------------------------------------------------------------------------------
+constexpr int BOX_MAXS = 16;               // steps per sample (S <= BOXES_NUM + 1 for the sampler)
+
+struct BoxRows {
+  double v[BOX_MAXS][4];                   // x, y, w, h of each row (corner, clipped)
+  int cls[BOX_MAXS];
+  int n;                                   // rows
+  int n_valid;                             // valid steps before the last one is dropped
+  int n_special;                           // boxes dropped for a special label
+};
+
+__device__ __forceinline__ void box_rows_of(const long long* __restrict__ labels, const float* __restrict__ samples,
+                                            const long long* __restrict__ steps, const double* __restrict__ mean_std,
+                                            const long long* __restrict__ label_to_class,
+                                            const double* __restrict__ count_stats,
+                                            const float* __restrict__ noise_cnt, int b, int S, int NL, int C,
+                                            BoxRows& r) {
+  int kept[BOX_MAXS], cls[BOX_MAXS];
+  double box[BOX_MAXS][4];
+  int n = 0;
+  const int st = (int)steps[b];
+  for (int t = 0; t < st && t < S; ++t) {
+    const float* p = samples + ((long long)b * S + t) * 4;
+    // product and sum rounded separately, as numpy does (a contracted fma could move a value across a boundary)
+    const double x = __dadd_rn(__dmul_rn((double)p[0], mean_std[1]), mean_std[0]);
+    const double y = __dadd_rn(__dmul_rn((double)p[1], mean_std[3]), mean_std[2]);
+    const double w = __dadd_rn(__dmul_rn((double)p[2], mean_std[5]), mean_std[4]);
+    const double h = __dmul_rn(w, __dadd_rn(__dmul_rn((double)p[3], mean_std[7]), mean_std[6]));
+    if (x > 0 && y > 0 && w > 0 && h > 0) {
+      box[n][0] = x; box[n][1] = y; box[n][2] = w; box[n][3] = h;
+      kept[n++] = t;
+    }
+  }
+  r.n_valid = n;
+  n = n > 1 ? n - 1 : 0;                   // drop the last kept step
+  int m = 0;
+  for (int i = 0; i < n; ++i) {            // special labels (<pad>, <sos>, <unk>) have no class: drop the box
+    const long long l = labels[(long long)b * S + kept[i]];
+    const long long c = (l >= 0 && l < NL) ? label_to_class[l] : -1;
+    if (c < 0) continue;
+    for (int q = 0; q < 4; ++q) box[m][q] = box[i][q];
+    cls[m++] = (int)c;
+  }
+  r.n_special = n - m;
+  int out = 0;
+  for (int i = 0; i < m; ++i) {
+    int before = 0;
+    for (int j = 0; j < i; ++j) before += cls[j] == cls[i];
+    const double draw = __dadd_rn(count_stats[2 * cls[i]],
+                                  __dmul_rn(count_stats[2 * cls[i] + 1], (double)noise_cnt[(long long)b * C + cls[i]]));
+    const double thr = fmax(trunc(draw), 2.0);
+    if ((double)before >= thr) continue;
+    double x = __dsub_rn(box[i][0], __dmul_rn(box[i][2], 0.5));     // x - w / 2.0
+    x = fmin(fmax(x, 1.0), 255.0);
+    double y = __dsub_rn(box[i][1], __dmul_rn(box[i][3], 0.5));
+    y = fmin(fmax(y, 1.0), 255.0);
+    r.v[out][0] = x; r.v[out][1] = y;
+    r.v[out][2] = fmin(box[i][2], 256.0 - x); r.v[out][3] = fmin(box[i][3], 256.0 - y);
+    r.cls[out++] = cls[i];
+  }
+  r.n = out;
+}
+
+__global__ void box_records_kernel(const long long* __restrict__ labels, const float* __restrict__ samples,
+                                   const long long* __restrict__ steps, const double* __restrict__ mean_std,
+                                   const long long* __restrict__ label_to_class,
+                                   const double* __restrict__ count_stats, const float* __restrict__ noise_cnt, int B,
+                                   int S, int NL, int C, double* __restrict__ rows, long long* __restrict__ row_cls,
+                                   long long* __restrict__ n_rows, long long* __restrict__ n_valid,
+                                   long long* __restrict__ n_special) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  BoxRows r;
+  box_rows_of(labels, samples, steps, mean_std, label_to_class, count_stats, noise_cnt, b, S, NL, C, r);
+  for (int i = 0; i < S; ++i) {
+    double* o = rows + ((long long)b * S + i) * 4;
+    for (int q = 0; q < 4; ++q) o[q] = i < r.n ? r.v[i][q] : 0.0;
+    row_cls[(long long)b * S + i] = i < r.n ? r.cls[i] : 0;
+  }
+  n_rows[b] = r.n;
+  n_valid[b] = r.n_valid;
+  n_special[b] = r.n_special;
+}
+
+OG_API int og_box_records(const long long* labels, const float* samples, const long long* steps,
+                          const double* mean_std, const long long* label_to_class, const double* count_stats,
+                          const float* noise_cnt, int B, int S, int NL, int C, double* rows, long long* row_cls,
+                          long long* n_rows, long long* n_valid, long long* n_special, cudaStream_t stream) {
+  if (B < 0 || S < 1 || S > BOX_MAXS || NL < 1 || C < 1) return (int)cudaErrorInvalidValue;
+  if (B == 0) return 0;
+  box_records_kernel<<<og_cdiv(B, 64), 64, 0, stream>>>(labels, samples, steps, mean_std, label_to_class, count_stats,
+                                                        noise_cnt, B, S, NL, C, rows, row_cls, n_rows, n_valid,
+                                                        n_special);
+  OG_RETURN_LAST_ERROR();
+}
+
+// The rows through the boxes.txt round trip int(float('%.2f' % v)), the ROI_MIN_SIZE filter and the three scales
+// (image_generation/miscc/load.py:653-776).
 __device__ __forceinline__ double box_txt_int(double v) {
   // v > 0 here.  '%.2f' rounds the exact binary value to two decimals, so it reaches the next integer exactly when
   // the fraction is at least 0.995; the double 0.995 lies just below 0.995 and the next double just above it.
@@ -350,58 +448,24 @@ __global__ void box_layout_kernel(const long long* __restrict__ labels, const fl
                                   long long* __restrict__ roi_cls, long long* __restrict__ num_rois) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
-  constexpr int MAXS = 16;                 // steps per sample (S <= BOXES_NUM + 1 for the sampler)
-  int kept[MAXS], cls[MAXS];
-  double box[MAXS][4];
-  int n = 0;
-  const int st = (int)steps[b];
-  for (int t = 0; t < st && t < S; ++t) {
-    const float* p = samples + ((long long)b * S + t) * 4;
-    // product and sum rounded separately, as numpy does (a contracted fma could move a value across a boundary)
-    const double x = __dadd_rn(__dmul_rn((double)p[0], mean_std[1]), mean_std[0]);
-    const double y = __dadd_rn(__dmul_rn((double)p[1], mean_std[3]), mean_std[2]);
-    const double w = __dadd_rn(__dmul_rn((double)p[2], mean_std[5]), mean_std[4]);
-    const double h = __dmul_rn(w, __dadd_rn(__dmul_rn((double)p[3], mean_std[7]), mean_std[6]));
-    if (x > 0 && y > 0 && w > 0 && h > 0) {
-      box[n][0] = x; box[n][1] = y; box[n][2] = w; box[n][3] = h;
-      kept[n++] = t;
-    }
-  }
-  n = n > 1 ? n - 1 : 0;                   // drop the last kept step
-  int m = 0;
-  for (int i = 0; i < n; ++i) {            // special labels (<pad>, <sos>, <unk>) have no class: drop the box
-    const long long l = labels[(long long)b * S + kept[i]];
-    const long long c = (l >= 0 && l < NL) ? label_to_class[l] : -1;
-    if (c < 0) continue;
-    for (int q = 0; q < 4; ++q) box[m][q] = box[i][q];
-    cls[m++] = (int)c;
-  }
+  BoxRows r;
+  box_rows_of(labels, samples, steps, mean_std, label_to_class, count_stats, noise_cnt, b, S, NL, C, r);
   int out = 0;
-  for (int i = 0; i < m; ++i) {
-    int before = 0;
-    for (int j = 0; j < i; ++j) before += cls[j] == cls[i];
-    const double draw = __dadd_rn(count_stats[2 * cls[i]],
-                                  __dmul_rn(count_stats[2 * cls[i] + 1], (double)noise_cnt[(long long)b * C + cls[i]]));
-    const double thr = fmax(trunc(draw), 2.0);
-    if ((double)before >= thr) continue;
-    double x = __dsub_rn(box[i][0], __dmul_rn(box[i][2], 0.5));     // x - w / 2.0
-    x = fmin(fmax(x, 1.0), 255.0);
-    double y = __dsub_rn(box[i][1], __dmul_rn(box[i][3], 0.5));
-    y = fmin(fmax(y, 1.0), 255.0);
-    const double w = fmin(box[i][2], 256.0 - x), h = fmin(box[i][3], 256.0 - y);
-    const double v[4] = {box_txt_int(x), box_txt_int(y), box_txt_int(w), box_txt_int(h)};
+  for (int i = 0; i < r.n; ++i) {
+    const double v[4] = {box_txt_int(r.v[i][0]), box_txt_int(r.v[i][1]), box_txt_int(r.v[i][2]),
+                         box_txt_int(r.v[i][3])};
     if (v[2] < min_size && v[3] < min_size) continue;
     if (out >= R) break;
     for (int k = 0; k < 3; ++k) {
-      double* r = rois + (((long long)k * B + b) * R + out) * 6;
+      double* o = rois + (((long long)k * B + b) * R + out) * 6;
       const double sc = (double)(64 << k) / 256.0;
-      for (int q = 0; q < 4; ++q) r[q] = v[q] * sc;
-      r[4] = cls[i]; r[5] = 0.0;
+      for (int q = 0; q < 4; ++q) o[q] = v[q] * sc;
+      o[4] = r.cls[i]; o[5] = 0.0;
     }
     double* f = fm_rois + ((long long)b * R + out) * 6;
     for (int q = 0; q < 4; ++q) f[q] = v[q] * 0.25 / 2.0;
-    f[4] = cls[i]; f[5] = 0.0;
-    roi_cls[(long long)b * R + out] = cls[i];
+    f[4] = r.cls[i]; f[5] = 0.0;
+    roi_cls[(long long)b * R + out] = r.cls[i];
     ++out;
   }
   num_rois[b] = out;
@@ -417,10 +481,61 @@ OG_API int og_box_layout(const long long* labels, const float* samples, const lo
                          const double* mean_std, const long long* label_to_class, const double* count_stats,
                          const float* noise_cnt, int B, int S, int NL, int C, int R, int min_size, double* rois,
                          double* fm_rois, long long* roi_cls, long long* num_rois, cudaStream_t stream) {
-  if (B < 0 || S < 1 || S > 16 || NL < 1 || C < 1 || R < 1) return (int)cudaErrorInvalidValue;
+  if (B < 0 || S < 1 || S > BOX_MAXS || NL < 1 || C < 1 || R < 1) return (int)cudaErrorInvalidValue;
   if (B == 0) return 0;
   box_layout_kernel<<<og_cdiv(B, 64), 64, 0, stream>>>(labels, samples, steps, mean_std, label_to_class, count_stats,
                                                        noise_cnt, B, S, NL, C, R, min_size, rois, fm_rois, roi_cls,
                                                        num_rois);
+  OG_RETURN_LAST_ERROR();
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The box stage's noise for captions first .. first + B - 1, each a function of (seed, caption index) alone, so the
+// draws of a caption do not depend on the batch it runs in.  Value j of stream s (0: noise_box at j = 6 t + k, 1:
+// noise_cnt at j = class) of caption i is Philox4x32-10 (Salmon et al., SC'11) of the counter (j, s, i_lo, i_hi) under
+// the key (seed_lo, seed_hi): a uniform is (w0 >> 8) 2^-24 in [0, 1), a standard normal is the Box-Muller transform
+// sqrt(-2 ln((w0 + 1) 2^-32)) cos(2 pi w1 2^-32) in float64, rounded to float32.
+// ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint4 box_philox(uint4 c, uint2 k) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r) { k.x += 0x9E3779B9u; k.y += 0xBB67AE85u; }
+    const unsigned lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+    const unsigned lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+  }
+  return c;
+}
+
+__global__ void box_noise_kernel(unsigned long long seed, long long first, int B, int S, int C,
+                                 float* __restrict__ noise_box, float* __restrict__ noise_cnt) {
+  const int per = S * 6 + C;
+  const long long total = (long long)B * per;
+  const uint2 key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total;
+       e += (long long)gridDim.x * blockDim.x) {
+    const long long b = e / per;
+    const int j = (int)(e % per);
+    const int box = j < S * 6;
+    const unsigned long long i = (unsigned long long)(first + b);
+    const uint4 w = box_philox(make_uint4(box ? j : j - S * 6, box ? 0u : 1u, (unsigned)i, (unsigned)(i >> 32)), key);
+    float v;
+    if (box && (j % 3) == 0) {
+      v = (float)(w.x >> 8) * 0x1p-24f;
+    } else {
+      const double u1 = ((double)w.x + 1.0) * 0x1p-32, u2 = (double)w.y * 0x1p-32;
+      v = (float)(sqrt(-2.0 * log(u1)) * cospi(2.0 * u2));
+    }
+    if (box) noise_box[b * S * 6 + j] = v;
+    else noise_cnt[b * C + (j - S * 6)] = v;
+  }
+}
+
+OG_API int og_box_noise(long long seed, long long first, int B, int S, int C, float* noise_box, float* noise_cnt,
+                        cudaStream_t stream) {
+  if (B < 0 || S < 1 || C < 1 || seed < 0 || first < 0) return (int)cudaErrorInvalidValue;
+  if (B == 0) return 0;
+  box_noise_kernel<<<tblocks((long long)B * (S * 6 + C)), 256, 0, stream>>>((unsigned long long)seed, first, B, S, C,
+                                                                            noise_box, noise_cnt);
   OG_RETURN_LAST_ERROR();
 }

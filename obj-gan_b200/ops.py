@@ -1815,6 +1815,52 @@ def boxes_to_layout(labels, samples, steps, mean_std, label_to_class, count_stat
     return list(rois.unbind(0)), fm_rois, roi_cls, num_rois
 
 
+def box_records(labels, samples, steps, mean_std, label_to_class, count_stats, noise_cnt):
+    """The rows Evaluator.evaluate writes to boxes.txt (ref: box_generation/seq2seq/evaluator/evaluator.py:74-139) on
+    the device (og_box_records), from the inputs of ``boxes_to_layout``: rows (B, S, 4) float64 (x, y, w, h, neither
+    rounded nor size-filtered, zero after the end), row_cls (B, S) int64 class rows, n_rows (B,), n_valid (B,) the valid
+    steps before the last is dropped, and n_special (B,) the boxes dropped for a special label.  All five are views of
+    one int64 buffer (``box_records_packed``), so a single copy brings them to the host."""
+    return unpack_box_records(box_records_packed(labels, samples, steps, mean_std, label_to_class, count_stats,
+                                                 noise_cnt), *labels.shape)
+
+
+def box_records_packed(labels, samples, steps, mean_std, label_to_class, count_stats, noise_cnt):
+    """``box_records``' outputs in one int64 buffer (B*S*5 + 3*B,): the float64 bits of rows, then row_cls, n_rows,
+    n_valid and n_special; ``unpack_box_records`` gives the views."""
+    ms, cs = mean_std.to(torch.float64).contiguous(), count_stats.to(torch.float64).contiguous()
+    ncnt = noise_cnt.to(torch.float32).contiguous()
+    _chk(labels, samples, steps, ms, label_to_class, cs, ncnt)
+    b, s = labels.shape
+    nl, c = label_to_class.shape[0], cs.shape[0]
+    assert samples.shape == (b, s, 4) and ms.shape == (4, 2) and cs.shape == (c, 2) and ncnt.shape == (b, c)
+    packed = torch.empty((b * s * 5 + 3 * b,), device=labels.device, dtype=torch.int64)
+    rows, row_cls, n_rows, n_valid, n_special = unpack_box_records(packed, b, s)
+    _call("og_box_records", _p(_i64(labels)), _p(samples.contiguous()), _p(_i64(steps)), _p(ms), _p(_i64(label_to_class)),
+          _p(cs), _p(ncnt), b, s, nl, c, _p(rows), _p(row_cls), _p(n_rows), _p(n_valid), _p(n_special))
+    return packed
+
+
+def unpack_box_records(packed, b, s):
+    """(rows, row_cls, n_rows, n_valid, n_special) as views of box_records' int64 buffer (on any device)."""
+    rows = packed[:b * s * 4].view(torch.float64).view(b, s, 4)
+    row_cls = packed[b * s * 4:b * s * 5].view(b, s)
+    n_rows, n_valid, n_special = packed[b * s * 5:].view(3, b).unbind(0)
+    return rows, row_cls, n_rows, n_valid, n_special
+
+
+def box_noise(seed, first, b, steps, num_classes, device):
+    """The box stage's noise of captions first .. first + b - 1 (og_box_noise): noise_box (b, steps, 6) with uniforms
+    in columns 0 and 3 and standard normals elsewhere, noise_cnt (b, num_classes) standard normals.  Each caption's
+    values depend only on (seed, its index), not on b or first."""
+    if not 0 <= int(seed) < 2 ** 63:
+        raise ValueError(f"seed must lie in [0, 2**63), got {seed}")
+    nb = torch.empty((b, steps, BOX_NOISE), device=device, dtype=torch.float32)
+    nc = torch.empty((b, num_classes), device=device, dtype=torch.float32)
+    _call("og_box_noise", int(seed), int(first), b, steps, num_classes, _p(nb), _p(nc))
+    return nb, nc
+
+
 # --------------------------------------------------------------------------------------------------
 # Inception-v3 image encoder (CNN_ENCODER, ref: model.py:182-287).  Its convolutions take the tensor cores at every
 # kernel shape (1x1, 1xN, Nx1, 3x3, 5x5, valid 3x3 stride 2; conv_path's general form), the exact-fp32 SIMT kernel
